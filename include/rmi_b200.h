@@ -1,4 +1,4 @@
-/* rmi_b200.h — C ABI of the B200-native two-layer RMI trainer (librmi_b200.so).
+/* rmi_b200.h — C ABI of the H100-native two-layer RMI trainer (librmi_b200.so).
  *
  * Drop-in boundary for the reference's `rmi_lib::train`
  *   pub fn train<T: TrainingKey>(data: &RMITrainingData<T>, model_spec: &str,
@@ -311,7 +311,7 @@ void rmi_thread_release(void);
 const char* rmi_last_error(void);
 /* Number of kernels this library has launched in this process (bench.py's gpu_launches). */
 uint64_t rmi_kernel_launch_count(void);
-/* Library / build identification, e.g. "rmi_b200 0.1 sm_100a". */
+/* Library / build identification, e.g. "rmi_b200 0.1 (sm_90a)". */
 const char* rmi_version(void);
 
 #ifdef __cplusplus

@@ -14,7 +14,7 @@
 // ("parity unpinned" for blobs; see DESIGN.md).
 //
 // Every function cites the reference file:line it restates (paths relative to
-// /root/reference/rmi_lib/src/).  Release-build semantics are used throughout (the
+// the reference repository's rmi_lib/src/).  Release-build semantics are used throughout (the
 // reference's tests build --release, tests/Makefile:20): wrapping integer arithmetic,
 // masked shift amounts, saturating float->int `as` casts, no debug_assert, no FP
 // contraction (compile with -ffp-contract=off), fused multiply-add only where the

@@ -1,6 +1,6 @@
-"""rmi_b200 — B200-native two-layer RMI trainer behind the reference's `rmi_lib::train` surface.
+"""rmi_b200 — H100-native two-layer RMI trainer behind the reference's `rmi_lib::train` surface.
 
-The product is the C-ABI shared library ``rmi_b200/lib/librmi_b200.so`` (CUDA, sm_100a;
+The product is the C-ABI shared library ``rmi_b200/lib/librmi_b200.so`` (CUDA, sm_90a;
 ``include/rmi_b200.h``).  This package is the thin Python host side used by the tests and
 ``bench.py``: it mirrors the reference's public API names
 

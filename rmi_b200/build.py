@@ -1,4 +1,4 @@
-"""Builds librmi_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Builds librmi_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import os
@@ -24,7 +24,7 @@ NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 # -fmad=false: the reference fuses a multiply-add only where it writes mul_add; everything
 # else must round twice (see csrc/rust_math.cuh).
 EXTRA_DEFS = os.environ.get("RMI_NVCC_DEFS", "").split()
-NVCC_FLAGS = EXTRA_DEFS + ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-fmad=false",
+NVCC_FLAGS = EXTRA_DEFS + ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-fmad=false",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-O2"]
 
 
@@ -58,7 +58,7 @@ def build_library(force: bool = False, verbose: bool = False) -> str:
     with ThreadPoolExecutor(max_workers=len(SOURCES)) as ex:
         list(ex.map(run, jobs))
     if force or jobs or _stale(LIB_PATH, objs):
-        run([NVCC, "-shared", "-o", LIB_PATH] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"])
+        run([NVCC, "-shared", "-o", LIB_PATH] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"])
     return LIB_PATH
 
 

@@ -226,7 +226,7 @@ extern "C" {
 
 const char* rmi_last_error(void) { return g_last_error.c_str(); }
 uint64_t rmi_kernel_launch_count(void) { return g_launches.load(); }
-const char* rmi_version(void) { return "rmi_b200 0.1 (sm_100a)"; }
+const char* rmi_version(void) { return "rmi_b200 0.1 (sm_90a)"; }
 
 int rmi_dataset_create(const void* host_keys, uint64_t n, rmi_key_type key_type, int device, rmi_dataset** out) {
   if (!out || (!host_keys && n) || (int)key_type < 0 || (int)key_type > 2)
@@ -544,8 +544,7 @@ struct Arena {   // stream-ordered scratch; everything is released when the call
 // slr() (linear.rs:12-59) is a loop-carried chain — sub, div, add per item on mean_x — that no parallel schedule can
 // reproduce bit for bit.  A CPU core runs that chain at ~20 cycles per item (the division's latency); one GPU warp
 // needs ~300.  So the exact mode streams the keys back to pinned host memory (64 MiB pieces on a side stream, the copy
-// of piece c+1 behind the arithmetic on piece c: the 1.6 GB of a 200M-key set cross PCIe in 30 ms, the chain takes
-// ~1.3 s) and runs the recurrence there, exactly as the reference does; the coefficients are then injected like
+// of piece c+1 behind the arithmetic on piece c: the copy is far shorter than the chain) and runs the recurrence there, exactly as the reference does; the coefficients are then injected like
 // rmi_train_with_top's.  Returns StatusBits (0 = ok).
 template <class T> inline double host_as_float(T k) { return (double)k; }
 inline uint64_t host_scale(uint64_t off, double sf, bool use_sf) { return use_sf ? (uint64_t)((double)off * sf) : off; }
@@ -1730,7 +1729,7 @@ static int shard_train_typed(rmi_shard_build* b, rmi_shard_comm* c, uint32_t fla
   // ---- leaves owned by this rank ---------------------------------------------------------------------------------
   // With a shared result region the host waits for the ownership ranges first (a few microseconds of idle GPU) and
   // launches only the owned leaf window, in slices whose records cross PCIe while the next slice computes — after the
-  // kernel that copy would be exposed (12 MiB at two ranks: 0.2 ms).  Otherwise the whole leaf range is launched at
+  // kernel that copy would be exposed.  Otherwise the whole leaf range is launched at
   // once (blocks without an owned leaf return immediately) and the host learns the ranges while it runs.
   LeafCopyOut* co = nullptr;
   if (shared && rc == RMI_OK) {

@@ -63,8 +63,8 @@ template <class T> inline Shard<T> whole_array(u64 n) {
 }
 
 // Optional: hand the leaf results to the host slice by slice while later slices still compute
-// (N x (8*ppm + 8) bytes cross PCIe in about the time the leaf kernel itself takes; copied after
-// the kernel they would add ~45% to a 200M-key build).  The bulk leaf kernel is launched as
+// (N x (8*ppm + 8) bytes cross PCIe in about the time the leaf kernel itself takes, so copied
+// after the kernel they would be fully exposed).  The bulk leaf kernel is launched as
 // `slices` consecutive block ranges on separate streams (so a slice's tail overlaps the next
 // slice's start); each slice's parameter / error (/ count) ranges are copied to pinned host
 // memory on the slice's stream as soon as the slice is done.

@@ -13,7 +13,7 @@
 //   :207-217  forward pass over every key: per-leaf (count, max |pred - offset|)
 //   :226-259  widening by the neighbours' keys and the longest duplicate run
 //
-// B200 formulation.  The clamped top prediction is non-decreasing over the sorted keys (the
+// GPU formulation.  The clamped top prediction is non-decreasing over the sorted keys (the
 // reference asserts it, :50), so leaf j owns the contiguous index range [S[j], S[j+1]) with
 // S[j] = first index whose prediction is >= j.  One streaming pass produces S (k_bounds);
 // after that every quantity the reference derives by walking all n keys three more times is a
@@ -142,11 +142,11 @@ k_bounds_search(const T* __restrict__ keys, u64 n, const TopModel* __restrict__ 
   u64 lo = 0, hi = n;
   if (j == N) lo = n;
   else if (j > 0) {
-    // (measured alternatives, all dropped: a two-level search — every 32nd boundary first, the others between their
-    //  brackets, ~13 probes in a 48 KB window — 0.141 ms against 0.144, round 2; galloping outwards from the interpolated index j*n/N
-    //  — 0.22 ms instead of 0.14 at 200M keys / 2^20 leaves, the divergent gallop loops cost more
-    //  than the saved probes — and a 4-ary search with three independent probes per level — no
-    //  change: the phase is bound by DRAM sectors per boundary, not by levels of latency)
+    // (alternatives tried and dropped: a two-level search — every 32nd boundary first, the others between their
+    //  brackets, ~13 probes in a 48 KB window — no faster; galloping outwards from the interpolated index j*n/N
+    //  — slower, the divergent gallop loops cost more than the saved probes — and a 4-ary search with three
+    //  independent probes per level — no change: the phase is bound by DRAM sectors per boundary, not by levels
+    //  of latency)
     while (lo < hi) {
       u64 mid = lo + ((hi - lo) >> 1);
       if (top_predict<TOP>(m, keys[mid]) >= j) hi = mid; else lo = mid + 1;
@@ -194,10 +194,9 @@ __global__ void k_split(const T* __restrict__ keys, u64 n, const TopModel* __res
 // Layout of one stage: row-major, 128 B of keys + 16 B pad per row.  The copies are issued 8 lanes per row (each
 // instruction moves four contiguous 128-byte segments: 4 cycles in the load/store unit's address stage and
 // conflict-free shared-memory writes), and the pad makes the 8 lanes of a 128-bit read phase — the same piece of 8
-// neighbouring rows — hit 8 distinct bank quads.  Measured alternatives (profiles/r02_ring_layouts.md): an unpadded
-// piece-major stage turns the copies' writes into 8-way bank conflicts (leaf kernel 0.98 ms instead of 0.53), and
-// letting every lane copy its own row costs 32 address-stage cycles per copy instruction instead of 4 — the LSU
-// becomes the bottleneck (0.90 ms).
+// neighbouring rows — hit 8 distinct bank quads.  Alternatives: an unpadded piece-major stage turns the copies'
+// writes into 8-way bank conflicts, and letting every lane copy its own row costs 32 address-stage cycles per copy
+// instruction instead of 4 — the LSU becomes the bottleneck.
 constexpr int ROW_BYTES = 144;
 constexpr int STAGE_BYTES = 32 * ROW_BYTES;
 constexpr int PIECE_STRIDE = 16;   // bytes between a row's consecutive pieces
@@ -584,8 +583,7 @@ template <bool CHECKED> struct LeafWelford {
   // differ by at most 2, plus a remote first item), so one window of counts serves all of them; a chunk needs 16 new
   // entries, computed by lanes 0-15 (one __drcp_rn each — the values of the shared table, for any count).  The step
   // is then the table step: no branch, the value fetched one step ahead.  (The general step's selection between the
-  // shared table, the global table and a division cost ~11 instructions per item and 19% of the stall samples of a
-  // build with 1525-key vectors.)
+  // shared table, the global table and a division costs ~11 instructions per item.)
   unsigned ring;       // shared address of the warp's ring, 512-byte aligned
   unsigned rq;         // 8 x (items pushed + 1): byte offset of the next step's entry, before wrapping
   unsigned ring_hi;    // warp-uniform: entries [.., ring_hi) are in the ring
@@ -1548,9 +1546,8 @@ k_leaf(const T* __restrict__ keys, const Shard<T> sh, u64 N, const u64* __restri
   // memory (the ring is idle now); results return to the owner lane.
   I max_err = 0, run_max = 0;
 #if !RMI_COOP_FORWARD
-  // Forward pass: every lane walks its own leaf through the copy ring a second time.  Measured against the two
-  // warp-cooperative variants below (coop_forward; profiles/r02_forward_variants.md): 0.533 ms for the leaf kernel
-  // of the headline build against 0.619 (bulk-copy tiles) and 0.682 (register look-ahead).
+  // Forward pass: every lane walks its own leaf through the copy ring a second time.  On the headline build this is
+  // faster than the two warp-cooperative variants below (coop_forward: bulk-copy tiles, register look-ahead).
   // Leaves much longer than their warp's other leaves skip the lane-serial walk (one lane would walk it alone while 31
   // wait): the whole warp evaluates them afterwards with coop_forward, 32 keys per step from bulk-copied tiles.  Worth it
   // only when a few lanes are long (when all 32 are, the lane-serial walks are balanced already).
@@ -1561,8 +1558,8 @@ k_leaf(const T* __restrict__ keys, const Shard<T> sh, u64 N, const u64* __restri
   // ... or when (nearly) all are: lane-serial walks over vectors this long are balanced but DRAM-latency bound (two 16-key
   // stages per lane are consumed faster than a copy returns, nothing is left in L2 of a 390 KB warp span), while the
   // cooperative walk streams 2 KB tiles two ahead and its per-leaf bookkeeping is amortised over 32+ steps.
-  // Measured (profiles/r02_leaf_kernel_experiments.md, 1525-key vectors): cubic leaves 1.10 ms against 1.40 lane-serial;
-  // linear leaves 0.84 against 0.80 — so only where the evaluation is the longer part of a step.
+  // With ~1500-key vectors this wins for cubic leaves and loses slightly for linear ones — so only where the
+  // evaluation is the longer part of a step.
   const bool long_fwd = is_long && (__popc(long_mask) <= 4 || (LEAF == M_CUBIC && __popc(long_mask) >= 28));
 #else
   const bool long_fwd = is_long && __popc(long_mask) <= 4;
@@ -1935,8 +1932,8 @@ void launch_leaf_inst(const Launch& L, const T* keys, const Shard<T>& sh, u64 N,
   // i.e. leaf groups [c*per/2, (c+1)*per/2) from the front and the mirrored range from the back ----
   constexpr int PPM = leaf_params_per_model(LEAF);
   const u32 total = (u32)blocks;
-  // Slice sizes taper towards the end: the copy engine keeps up with the kernel (24 MiB cross PCIe in 0.46 ms, the
-  // kernel produces them in 0.53), so what stays exposed is the LAST slice's copy — the last two slices are 16% and 8%
+  // Slice sizes taper towards the end: the copy engine keeps up with the kernel (the records cross PCIe in about the
+  // time the kernel takes to produce them), so what stays exposed is the LAST slice's copy — the last two slices are 16% and 8%
   // of the blocks, the others share the rest equally.  (even offsets: block ids alternate between front and back groups)
   u32 bounds_[MAX_LEAF_SLICES + 1];
   {

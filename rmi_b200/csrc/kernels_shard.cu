@@ -36,7 +36,7 @@ namespace rmi {
 namespace {
 
 constexpr int SH_THREADS = 256;
-constexpr int SH_MAX_BLOCKS = 148 * 8;
+constexpr int SH_MAX_BLOCKS = 132 * 8;   // 8 blocks per SM of an H100 (sh_grid: min(num_sms * 8, this))
 
 __device__ __forceinline__ void set_status(BuildAux* aux, unsigned bit) { atomicOr(&aux->status, bit); }
 

@@ -21,7 +21,7 @@ namespace rmi {
 namespace {
 
 constexpr int TOP_THREADS = 256;
-constexpr int MAX_PARTIAL_BLOCKS = 148 * 8;
+constexpr int MAX_PARTIAL_BLOCKS = 132 * 8;   // 8 blocks per SM of an H100 (grid_for: min(num_sms * 8, this))
 
 __device__ __forceinline__ void set_status(BuildAux* aux, unsigned bit) { atomicOr(&aux->status, bit); }
 

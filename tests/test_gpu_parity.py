@@ -57,13 +57,15 @@ EXACT_LEAVES = ["linear", "linear_spline"]
 
 
 def run_both(rmi, oracle, dname, spec, bf, flags=0, l0=None):
+    """(GPU result, oracle result); None where the reference panics — after checking that the GPU path panics too,
+    which is then the whole of what the configuration can be checked for."""
     keys = data(dname)
     try:
         o = oracle.train(keys, spec, bf, l0_override=l0)
-    except oracle.OraclePanic as e:
+    except oracle.OraclePanic:
         with pytest.raises(rmi.RMIPanic):
             rmi.train(dataset(rmi, dname), spec, bf, flags, l0_params=l0)
-        pytest.skip(f"reference panics here and so does the GPU path: {e}")
+        return None
     g = rmi.train(dataset(rmi, dname), spec, bf, flags, l0_params=l0)
     return g, o
 
@@ -73,8 +75,9 @@ def run_both(rmi, oracle, dname, spec, bf, flags=0, l0=None):
 @pytest.mark.parametrize("top", EXACT_TOPS)
 @pytest.mark.parametrize("bf", [64, 1000, 4096])
 def test_integer_and_spline_tops_bit_exact(rmi, oracle, top, leaf, bf, dname):
-    g, o = run_both(rmi, oracle, dname, f"{top},{leaf}", bf)
-    parity.assert_same_rmi(g, o)
+    r = run_both(rmi, oracle, dname, f"{top},{leaf}", bf)
+    if r is not None:
+        parity.assert_same_rmi(*r)
 
 
 @pytest.mark.parametrize("dname", list(DATA))
@@ -82,9 +85,10 @@ def test_integer_and_spline_tops_bit_exact(rmi, oracle, top, leaf, bf, dname):
 @pytest.mark.parametrize("top", SERIAL_TOPS)
 @pytest.mark.parametrize("bf", [100, 4096])
 def test_serial_tops_exact_mode_bit_exact(rmi, oracle, top, leaf, bf, dname):
-    g, o = run_both(rmi, oracle, dname, f"{top},{leaf}", bf, flags=rmi.FLAG_TOP_FIT_EXACT)
-    assert g.top_fit_exact
-    parity.assert_same_rmi(g, o)
+    r = run_both(rmi, oracle, dname, f"{top},{leaf}", bf, flags=rmi.FLAG_TOP_FIT_EXACT)
+    if r is not None:
+        assert r[0].top_fit_exact
+        parity.assert_same_rmi(*r)
 
 
 @pytest.mark.parametrize("dname", list(DATA))
@@ -121,11 +125,11 @@ def test_log_and_normal_tops_single_gpu(rmi, oracle, top, bf, dname):
     keys = data(dname)
     try:
         o_ref = oracle.train(keys, spec, bf)
-    except oracle.OraclePanic as e_ref:
+    except oracle.OraclePanic:
         # with tolerance-level coefficients the GPU run lands on the same side in every case below
         with pytest.raises(rmi.RMIPanic):
             rmi.train(dataset(rmi, dname), spec, bf)
-        pytest.skip(f"reference panics here and so does the GPU path: {e_ref}")
+        return
     g = rmi.train(dataset(rmi, dname), spec, bf)
     parity.assert_top_equal(g, o_ref, exact=False, N=bf)
     try:
@@ -146,8 +150,9 @@ def test_log_and_normal_tops_single_gpu(rmi, oracle, top, bf, dname):
 def test_large_radix_tables_bit_exact(rmi, oracle, top, dname):
     """radix22 is in the optimizer's default profile (optimizer.rs:110-151); radix26 is the next template size.
     16 MiB / 256 MiB hint tables (radix.rs:90-134), bit-exact."""
-    g, o = run_both(rmi, oracle, dname, f"{top},linear", 1024)
-    parity.assert_same_rmi(g, o)
+    r = run_both(rmi, oracle, dname, f"{top},linear", 1024)
+    if r is not None:
+        parity.assert_same_rmi(*r)
 
 
 @pytest.mark.parametrize("dname", ["uniform_u64", "lognormal_u64", "dups_u64", "uniform_f64"])

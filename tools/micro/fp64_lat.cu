@@ -1,5 +1,5 @@
 // Microbenchmark (developer tool): FP64 dependent-op latency and the cost of one Welford step
-// for a single resident warp on sm_100a.  nvcc -arch=sm_100a -fmad=false -O3 fp64_lat.cu
+// for a single resident warp on sm_90a.  nvcc -arch=sm_90a -fmad=false -O3 fp64_lat.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 __global__ void k_lat(double* out, long long* cyc, int iters, double a, double b) {

@@ -1,7 +1,7 @@
 """BASELINE.json configs[4]: the `--optimize` sweep (optimizer.rs:110-151, :220-249) on 800M synthetic f64 keys over the
 GPUs of one node, measured; plus the parity of the search itself on a sample the CPU oracle can sweep.
 
-    python tools/optimize_bench.py [--keys 800e6] [--gpus 8] [--sample 4e6] > profiles/r02_optimize_<N>gpu.json
+    python tools/optimize_bench.py [--keys 800e6] [--gpus 8] [--sample 4e6] > optimize_<N>gpu.json
 
 One process: the keys are generated and sorted on GPU 0, replicated to the other GPUs over NVLink
 (rmi_dataset_replicate), and rmi_find_pareto_efficient_configs spreads the (top, branching factor) groups over one
