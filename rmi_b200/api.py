@@ -61,10 +61,9 @@ def load_library():
     """Load librmi_b200.so (built in-tree by rmi_b200.build / __graft_entry__.build)."""
     global _lib
     if _lib is None:
-        path = os.environ.get("RMI_B200_LIB") or _LIB_PATH     # RMI_B200_LIB: an experiment build of the same library
-        if not os.path.exists(path):
-            raise RMIError(f"{path} is missing: run `python -m rmi_b200.build` (there is no CPU fallback)")
-        L = C.CDLL(path)
+        if not os.path.exists(_LIB_PATH):
+            raise RMIError(f"{_LIB_PATH} is missing: run `python -m rmi_b200.build` (there is no CPU fallback)")
+        L = C.CDLL(_LIB_PATH)
         L.rmi_last_error.restype = C.c_char_p
         L.rmi_version.restype = C.c_char_p
         L.rmi_kernel_launch_count.restype = C.c_uint64

@@ -9,11 +9,8 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
-# RMI_BUILD_TAG=<name> (with RMI_NVCC_DEFS="-DFOO ...") builds an experiment variant next to the
-# default library: lib/librmi_b200_<name>.so, loaded by dev tools through RMI_B200_LIB.
-_TAG = os.environ.get("RMI_BUILD_TAG", "")
-LIB_PATH = os.path.join(LIB_DIR, f"librmi_b200{'_' + _TAG if _TAG else ''}.so")
-OBJ_DIR = os.path.join(HERE, "build" + ("_" + _TAG if _TAG else ""))
+LIB_PATH = os.path.join(LIB_DIR, "librmi_b200.so")
+OBJ_DIR = os.path.join(HERE, "build")
 
 SOURCES = ["kernels_top.cu", "kernels_leaf.cu", "kernels_shard.cu", "api.cu"]
 HEADERS = ["rust_math.cuh", "models.cuh", "device_util.cuh", "spline.cuh", "kernels.h",
@@ -23,8 +20,7 @@ HEADERS = ["rust_math.cuh", "models.cuh", "device_util.cuh", "spline.cuh", "kern
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 # -fmad=false: the reference fuses a multiply-add only where it writes mul_add; everything
 # else must round twice (see csrc/rust_math.cuh).
-EXTRA_DEFS = os.environ.get("RMI_NVCC_DEFS", "").split()
-NVCC_FLAGS = EXTRA_DEFS + ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-fmad=false",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-fmad=false",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-O2"]
 
 

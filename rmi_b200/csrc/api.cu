@@ -462,7 +462,7 @@ struct SliceResources {
   LeafCopyOut co;
   void release() {
     if (device < 0) return;
-    for (int c = 0; c < MAX_LEAF_SLICES; ++c) {
+    for (int c = 0; c < LEAF_SLICES; ++c) {
       if (co.streams[c]) cudaStreamDestroy(co.streams[c]);
       if (co.ev_kernel[c]) cudaEventDestroy(co.ev_kernel[c]);
       if (co.ev_copied[c]) cudaEventDestroy(co.ev_copied[c]);
@@ -475,7 +475,7 @@ struct SliceResources {
     if (device == dev) return &co;
     release();
     bool ok = cudaEventCreateWithFlags(&co.ev_ready, cudaEventDisableTiming) == cudaSuccess;
-    for (int c = 0; c < MAX_LEAF_SLICES && ok; ++c)
+    for (int c = 0; c < LEAF_SLICES && ok; ++c)
       ok = cudaStreamCreateWithFlags(&co.streams[c], cudaStreamNonBlocking) == cudaSuccess &&
            cudaEventCreateWithFlags(&co.ev_kernel[c], cudaEventDisableTiming) == cudaSuccess &&
            cudaEventCreateWithFlags(&co.ev_copied[c], cudaEventDisableTiming) == cudaSuccess;
@@ -519,11 +519,6 @@ struct BuildContext {
   }
 };
 thread_local BuildContext t_build_ctx;
-
-int leaf_slices_default() {
-  static const int k = [] { const char* e = getenv("RMI_DEV_LEAF_SLICES"); int v = e ? atoi(e) : 5; return v < 1 ? 1 : (v > MAX_LEAF_SLICES ? MAX_LEAF_SLICES : v); }();
-  return k;
-}
 
 struct Arena {   // stream-ordered scratch; everything is released when the call ends
   cudaStream_t st;
@@ -663,6 +658,9 @@ unsigned host_exact_top(const rmi_dataset* ds, int kind, uint64_t N, double* out
   return status;
 }
 inline bool host_exact_kind(int kind) { return kind == M_LINEAR || kind == M_ROBUST_LINEAR || kind == M_NORMAL; }
+// exact serial tops on at least this many keys run on a host core (host_exact_top); smaller sets keep the one-warp
+// device chain (no PCIe round trip, and the CPU tests of the chain itself stay meaningful)
+constexpr uint64_t HOST_EXACT_MIN = (uint64_t)1 << 20;
 
 template <class T>
 int train_typed(const rmi_dataset* ds, const ModelName& top, const ModelName& leaf, uint64_t N, uint32_t flags,
@@ -733,11 +731,8 @@ int train_typed(const rmi_dataset* ds, const ModelName& top, const ModelName& le
       cudaEventRecord(ev0, st);
       unsigned host_status = 0;
       bool exact = (flags & RMI_FLAG_TOP_FIT_EXACT) != 0;
-      // exact serial tops on large key sets: the recurrence runs on a host core (host_exact_top); small sets keep the
-      // one-warp device chain (no PCIe round trip, and the CPU tests of the chain itself stay meaningful)
-      static const uint64_t host_exact_min = [] { const char* e = getenv("RMI_DEV_HOST_EXACT_MIN"); return e ? (uint64_t)atoll(e) : (uint64_t)1 << 20; }();
       bool host_top = false;
-      if (exact && !l0_over && host_exact_kind(top.kind) && n >= host_exact_min) {
+      if (exact && !l0_over && host_exact_kind(top.kind) && n >= HOST_EXACT_MIN) {
         cudaEventSynchronize(ev0);
         unsigned hs = host_exact_top<T>(ds, top.kind, N, h_top.f);
         if (hs == 0x80000000u) rc = fail(RMI_ERR_CUDA, "exact top fit: copying the keys back to the host failed");
@@ -762,7 +757,7 @@ int train_typed(const rmi_dataset* ds, const ModelName& top, const ModelName& le
           if (co) {
             co->h_params = box->l1_params.data(); co->h_errors = reinterpret_cast<u64*>(box->l1_errors.data());
             co->h_counts = want_counts ? reinterpret_cast<u64*>(box->l1_counts.data()) : nullptr;
-            co->slices = leaf_slices_default(); co->used = 0;
+            co->used = 0;
             L.copy = co;
             leaf_results_copied = true;
           }
@@ -1738,7 +1733,7 @@ static int shard_train_typed(rmi_shard_build* b, rmi_shard_comm* c, uint32_t fla
     co = rc == RMI_OK ? t_slices.get(b->ds->device) : nullptr;
     if (co) {
       co->h_params = sh_params; co->h_errors = sh_errors; co->h_counts = sh_counts;
-      co->slices = leaf_slices_default(); co->used = 0;
+      co->used = 0;
       b->leaf_copy = co;
       b->leaf_lo = b->h_off[rank]; b->leaf_hi = b->h_off[rank + 1];
       if (b->leaf_hi == 0) b->leaf_lo = b->leaf_hi = N;   // owns nothing (0 would mean "no window")

@@ -65,20 +65,19 @@ template <class T> inline Shard<T> whole_array(u64 n) {
 // Optional: hand the leaf results to the host slice by slice while later slices still compute
 // (N x (8*ppm + 8) bytes cross PCIe in about the time the leaf kernel itself takes, so copied
 // after the kernel they would be fully exposed).  The bulk leaf kernel is launched as
-// `slices` consecutive block ranges on separate streams (so a slice's tail overlaps the next
+// LEAF_SLICES consecutive block ranges on separate streams (so a slice's tail overlaps the next
 // slice's start); each slice's parameter / error (/ count) ranges are copied to pinned host
 // memory on the slice's stream as soon as the slice is done.
-constexpr int MAX_LEAF_SLICES = 16;
+constexpr int LEAF_SLICES = 5;
 struct LeafCopyOut {
   double* h_params = nullptr;   // N x ppm (pinned)
   u64* h_errors = nullptr;      // N
   u64* h_counts = nullptr;      // N or null
-  int slices = 0;               // <= 1: disabled
-  cudaStream_t streams[MAX_LEAF_SLICES] = {};
-  cudaEvent_t ev_ready = nullptr;                 // main stream: leaf boundaries are final
-  cudaEvent_t ev_kernel[MAX_LEAF_SLICES] = {};    // slice kernel finished
-  cudaEvent_t ev_copied[MAX_LEAF_SLICES] = {};    // slice results are on the host
-  mutable int used = 0;                           // slices actually launched (set by fit_leaves)
+  cudaStream_t streams[LEAF_SLICES] = {};
+  cudaEvent_t ev_ready = nullptr;             // main stream: leaf boundaries are final
+  cudaEvent_t ev_kernel[LEAF_SLICES] = {};    // slice kernel finished
+  cudaEvent_t ev_copied[LEAF_SLICES] = {};    // slice results are on the host
+  mutable int used = 0;                       // slices actually launched (set by fit_leaves)
 };
 
 struct Launch {

@@ -24,8 +24,6 @@
 // bit-identical; parallelism comes from the N independent leaves.
 #include "device_util.cuh"
 #include "kernels.h"
-#include <cstdio>
-#include <cstdlib>
 #include <mutex>
 #include <type_traits>
 #include <vector>
@@ -35,46 +33,11 @@ namespace rmi {
 namespace {
 
 constexpr int BOUNDS_THREADS = 256;
-// Compile-time experiment knobs (defaults = the measured best; variants are built next to the default
-// library with RMI_BUILD_TAG / RMI_NVCC_DEFS, rmi_b200/build.py, and timed by tools/gpu_variants.sh).
-#ifndef RMI_LEAF_THREADS
-#define RMI_LEAF_THREADS 128
-#endif
+constexpr int LEAF_THREADS = 128;
 // Resident blocks per SM the compiler must allow for: 20 warps (the padded copy ring takes 41 KB of shared memory per
 // 128-lane block, so 5 blocks fit), i.e. at most 96 registers.
-#ifndef RMI_LEAF_MIN_BLOCKS
-#define RMI_LEAF_MIN_BLOCKS (640 / RMI_LEAF_THREADS)
-#endif
-#define RMI_LEAF_BOUNDS __launch_bounds__(RMI_LEAF_THREADS, RMI_LEAF_MIN_BLOCKS)
-constexpr int LEAF_THREADS = RMI_LEAF_THREADS;
-#ifndef RMI_COOP_FORWARD
-#define RMI_COOP_FORWARD 0   // 1 = warp-cooperative forward pass (coop_forward) instead of the lane-serial one
-#endif
-#ifndef RMI_FWD_BULK
-#define RMI_FWD_BULK 1   // forward pass fed by 1-D bulk copies (cp.async.bulk + mbarrier); 0 = register look-ahead
-#endif
-#ifndef RMI_FWD_DEPTH
-#define RMI_FWD_DEPTH 8   // 32-key loads in flight per warp in the forward pass
-#endif
-#ifndef RMI_LONG_FWD_ALL
-#define RMI_LONG_FWD_ALL 1
-#endif
-#ifndef RMI_LONG_FWD_MIN
-#define RMI_LONG_FWD_MIN 1024
-#endif
-#ifndef RMI_RCP_RING
-#define RMI_RCP_RING 1
-#endif
-#ifndef RMI_PARTIAL_UNROLLED
-#define RMI_PARTIAL_UNROLLED 0
-#endif
-#ifndef RMI_RC_PREFETCH
-#define RMI_RC_PREFETCH 1
-#endif
-#ifndef RMI_RCP_TABLE
-#define RMI_RCP_TABLE 512
-#endif
-constexpr int RCP_TABLE = RMI_RCP_TABLE;   // reciprocals of the counts below this live in shared memory
+constexpr int LEAF_MIN_BLOCKS = 640 / LEAF_THREADS;
+constexpr int RCP_TABLE = 512;   // reciprocals of the counts below this live in shared memory
 
 __device__ __forceinline__ void set_status(BuildAux* aux, unsigned bit) { atomicOr(&aux->status, bit); }
 
@@ -200,10 +163,7 @@ __global__ void k_split(const T* __restrict__ keys, u64 n, const TopModel* __res
 constexpr int ROW_BYTES = 144;
 constexpr int STAGE_BYTES = 32 * ROW_BYTES;
 constexpr int PIECE_STRIDE = 16;   // bytes between a row's consecutive pieces
-#ifndef RMI_SSTAGES
-#define RMI_SSTAGES 2
-#endif
-constexpr int SSTAGES = RMI_SSTAGES;
+constexpr int SSTAGES = 2;
 constexpr int WARP_STREAM_BYTES = SSTAGES * STAGE_BYTES + 32 * 4 + 32 * 4;
 
 // createpolicy for an L2 eviction priority: 0 evict_normal, 1 evict_first, 2 evict_last.
@@ -409,31 +369,6 @@ __device__ __forceinline__ void stream_pass(const T* __restrict__ keys, u64 l2_p
       const I lo_k = (c == 0) ? skip : (I)0;
       const I rem = rlen > cbase ? (I)(rlen - cbase) : (I)0;
       const int p1 = rem < (I)SW ? (int)rem : SW;
-#if RMI_PARTIAL_UNROLLED
-      // The lanes of a warp end in different chunks (190 +- 14 keys per leaf: the last three or four chunks of a warp
-      // each hold some lane's end), so about a quarter of all keys pass through here, most of them on lanes that still
-      // have the whole chunk.  Fixed trip count and compile-time shared-memory offsets like the vector path, with one
-      // predicate per piece and one per further key of the piece, instead of three position-driven loops.
-      {
-        const int lo = (int)lo_k;
-        const I idx0 = a + cbase;
-#pragma unroll
-        for (int pp = 0; pp < 8; ++pp) {
-          if (pp * KPP < p1) {
-            uint4 v = *reinterpret_cast<const uint4*>(row + pp * PIECE_STRIDE);
-            T kk[KPP];
-            memcpy(kk, &v, 16);
-#pragma unroll
-            for (int t = 0; t < KPP; ++t) {
-              const int q = pp * KPP + t;
-              if ((pp > 0 || q >= lo) && (t == 0 || q < p1)) fn(kk[t], (I)(idx0 + (I)q));
-            }
-          }
-        }
-      }
-      __syncwarp();
-      continue;
-#endif
       int pos = (int)lo_k;
       auto key_at = [&](int q) {   // key at position q of this lane's row
         return *reinterpret_cast<const T*>(row + (q / KPP) * PIECE_STRIDE + (q % KPP) * (int)sizeof(T));
@@ -536,22 +471,15 @@ template <bool CHECKED> struct LeafWelford {
     return rc;
   }
   __device__ __forceinline__ double next_rc() {
-#if RMI_RC_PREFETCH
     const double rc = rc_next;
     ra += (unsigned)sizeof(double);
     rc_next = fetch_rc(ra + (unsigned)sizeof(double), __dadd_rn(nf, 2.0));   // this step divides by nf + 1, the next by nf + 2
     return rc;
-#else   // experiment knob: the load issued in the step that uses it (round 1's behaviour)
-    ra += (unsigned)sizeof(double);
-    return fetch_rc(ra, __dadd_rn(nf, 1.0));
-#endif
   }
   // after a stretch in which `ra` was not advanced (solo mode): later steps divide
   __device__ __forceinline__ void rc_cursor_off() {
     ra = ra_end + RCP_FAR * (unsigned)sizeof(double);
-#if RMI_RC_PREFETCH
     rc_next = rcp_beyond_table(__dadd_rn(nf, 1.0));
-#endif
   }
   __device__ __forceinline__ double dv(double a, double rc) const {
     if (CHECKED) return div_by_count(a, nf, rc);
@@ -619,9 +547,6 @@ template <bool CHECKED> struct LeafWelford {
   // back to the general cursor (ra, rc_next stays valid: it is the reciprocal of items + 1)
   __device__ __forceinline__ void ring_end() {
     ra = (ra_end - (unsigned)((RCP_TABLE - 1) * sizeof(double))) + (rq - (unsigned)sizeof(double));
-#if !RMI_RC_PREFETCH
-    (void)0;
-#endif
   }
   // Items whose y are CONSECUTIVE integers y0, y0+1, ... (a data set without equal keys): the
   // reference's mean_y recurrence is then exact at every step — dy = k/2, dy/k = 0.5, mean_y =
@@ -894,12 +819,8 @@ __device__ __forceinline__ void fit_leaf(const T* __restrict__ keys, const Shard
     }
     int solo_lane;
     I solo_at;
-#if RMI_RCP_RING
     // vectors below 2^28 items (the ring's 32-bit cursor); a warp with a longer one takes the general step
     const bool ring_ok = LEAF == M_LINEAR && !__any_sync(0xffffffffu, (u64)L >= (1ull << 28));
-#else
-    const bool ring_ok = false;
-#endif
     if (ring_ok) {
       w.ring_begin(rcp_ring);
       if (ND) {
@@ -1135,13 +1056,10 @@ __device__ __forceinline__ void coop_forward(const T* __restrict__ keys, const S
   // The leaves of a warp's lanes are consecutive, so their key ranges tile one contiguous span
   // (interrupted only where a lane has no leaf of its own: another rank's, a long leaf built elsewhere).
   // The warp walks every such SEGMENT as a flat stream, 32 consecutive keys per step whatever leaf they
-  // belong to: the loads of the step FWD_DEPTH ahead are issued before a step is evaluated (the keys come
-  // from L2 / HBM, the latency is that of a miss), and a step that straddles a leaf boundary is evaluated
-  // once per leaf it touches.  Per-leaf maxima are reduced when the stream leaves the leaf.
+  // belong to, read from bulk-copied key tiles (below), and a step that straddles a leaf boundary is
+  // evaluated once per leaf it touches.  Per-leaf maxima are reduced when the stream leaves the leaf.
   constexpr int PPM = leaf_params_per_model(LEAF);
-  constexpr int FWD_DEPTH = RMI_FWD_DEPTH;
   constexpr int REC = 16 + ((PPM * 8 + 15) / 16) * 16;   // {lo, hi} + parameters, 16-byte aligned
-#if RMI_FWD_BULK
   // the warp's ring memory during the forward pass: FB_STAGES key tiles | 32 leaf descriptors | FB_STAGES mbarriers
   constexpr int FB_STAGES = 3, FB_TILE_BYTES = 2048;
   constexpr int DESC_OFF = FB_STAGES * FB_TILE_BYTES;
@@ -1152,9 +1070,6 @@ __device__ __forceinline__ void coop_forward(const T* __restrict__ keys, const S
   unsigned fb_uses = 0;   // bit s = parity of the number of completed uses of stage s
   u64 fb_policy;
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(fb_policy));
-#else
-  unsigned char* const dsc = wsm;
-#endif
   const unsigned FULL = 0xffffffffu;
   const int lane = threadIdx.x & 31;
   const unsigned le_mask = (2u << lane) - 1u;            // lanes at or below this one
@@ -1163,13 +1078,11 @@ __device__ __forceinline__ void coop_forward(const T* __restrict__ keys, const S
   unsigned todo = __ballot_sync(FULL, mine);
   if (todo == 0) return;
   __syncwarp();
-#if RMI_FWD_BULK
   if (lane == 0) {
 #pragma unroll
     for (int sidx = 0; sidx < FB_STAGES; ++sidx) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(fb_bar0 + sidx * 8u) : "memory");
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-#endif
   {
     unsigned char* rec = dsc + lane * REC;
     *reinterpret_cast<ulonglong2*>(rec) = make_ulonglong2((u64)lo, (u64)hi);
@@ -1202,7 +1115,6 @@ __device__ __forceinline__ void coop_forward(const T* __restrict__ keys, const S
     I w_err = 0, w_run = 0;
     I carry_F = (I)(seg_lo + baseI);
     T carry_k = T();
-    const I last_readable = (I)(sh.n_avail - 1);
     auto leave_leaf = [&]() {   // the stream has passed leaf q: hand its maxima to the owner, move to the next leaf
       const I r_err = warp_max<I>(w_err);
       I r_run = 0;
@@ -1217,7 +1129,6 @@ __device__ __forceinline__ void coop_forward(const T* __restrict__ keys, const S
         for (int t = 0; t < PPM; ++t) cf[t] = reinterpret_cast<const double*>(dsc + q * REC + 16)[t];
       }
     };
-#if RMI_FWD_BULK
     // ---- key tiles by 1-D bulk copy (TMA engine, cp.async.bulk + mbarrier): the segment is one contiguous byte range, so
     // ONE elected lane moves it through shared memory in 2 KB tiles, FB_STAGES tiles in flight, and every step reads its
     // 32 keys from the landed tile.  Unlike register look-ahead (whose loads share the warp's six scoreboards, so a wait
@@ -1311,83 +1222,6 @@ __device__ __forceinline__ void coop_forward(const T* __restrict__ keys, const S
       __syncwarp();                                        // every lane is done with the tile: its stage may be refilled
       if (t + FB_STAGES < ntiles) issue_tile(t + FB_STAGES);
     }
-#else
-    // FWD_DEPTH + 1 register slots: the step that consumes slot u refills the slot the PREVIOUS step consumed, so a
-    // load never targets the register it is just reading (with FWD_DEPTH slots the compiler loads into a temporary
-    // and copies it — and the copy waits for the load: measured, it serialised every step on the load latency)
-    constexpr int FWD_SLOTS = FWD_DEPTH + 1;
-    T kk[FWD_SLOTS];
-#pragma unroll
-    for (int u = 0; u < FWD_DEPTH; ++u) {
-      const I iu = seg_lo + (I)(u * 32 + lane);
-      kk[u] = __ldcs(keys + (iu < last_readable ? iu : last_readable));     // streaming: the line's last use
-    }
-    kk[FWD_DEPTH] = T();
-    I pos = seg_lo;
-    // look-ahead loads are unconditional: the index is clamped to the last readable key instead of predicated
-    // (a predicated load costs a branch per step; a clamped one past the segment's end is simply not used)
-    I inext = (I)(seg_lo + (I)(FWD_DEPTH * 32 + lane));
-    I Fi = (I)(seg_lo + (I)lane + baseI);                 // global index of this lane's key in the current step
-    bool done = false;
-    while (!done) {
-#pragma unroll
-      for (int u = 0; u < FWD_SLOTS; ++u) {
-        const T k = kk[u];
-        kk[(u + FWD_DEPTH) % FWD_SLOTS] = __ldcs(keys + (inext < last_readable ? inext : last_readable));
-        inext += 32;
-        const double x = Key<T>::as_float(k);
-        if (!DUPS && (I)(hi_q - pos) >= (I)32) {
-          // the whole step lies inside leaf q (the common case: 5 of 6 steps at 190 keys per leaf)
-          const I pred = leaf_predict_clamped<LEAF, I, NANCHECK>(cf, x, nI);
-          const I e = pred > Fi ? pred - Fi : Fi - pred;
-          w_err = e > w_err ? e : w_err;
-          pos += 32;
-          Fi += 32;
-          continue;
-        }
-        if (pos >= seg_hi) { done = true; break; }        // warp-uniform
-        const I i = pos + (I)lane;
-        const I step_end = (seg_hi - pos) > (I)32 ? (I)(pos + 32) : seg_hi;
-        const bool valid = i < step_end;
-        I F = Fi, len = 0;
-        bool pend = valid, pend_run = false;
-        if (DUPS) {
-          T kp = __shfl_up_sync(FULL, k, 1);
-          if (lane == 0) kp = carry_k;
-          const bool starts = valid && (i == seg_lo || k != kp);   // a segment's (and every leaf's) first key starts a run
-          const unsigned sm = __ballot_sync(FULL, starts);
-          const unsigned below = sm & le_mask;
-          F = below ? (I)(pos + baseI + (I)(31 - __clz(below))) : carry_F;
-          I Fm1 = __shfl_up_sync(FULL, F, 1);
-          if (lane == 0) Fm1 = carry_F;
-          // the run BEFORE a run start ends here; its length belongs to the leaf of the key before this one
-          pend_run = starts && i != seg_lo;
-          len = (I)(Fi - Fm1);
-          const int lastv = (int)(step_end - pos) - 1;
-          carry_F = __shfl_sync(FULL, F, lastv);
-          carry_k = __shfl_sync(FULL, k, lastv);
-        }
-        for (;;) {
-          const I pred = leaf_predict_clamped<LEAF, I, NANCHECK>(cf, x, nI);
-          I e = pred > F ? pred - F : F - pred;
-          const bool take = pend && i < hi_q;
-          e = take ? e : (I)0;
-          w_err = e > w_err ? e : w_err;
-          pend = pend && !take;
-          if (DUPS) {
-            const bool take_run = pend_run && i <= hi_q;
-            const I l = take_run ? len : (I)0;
-            w_run = l > w_run ? l : w_run;
-            pend_run = pend_run && !take_run;
-          }
-          if (hi_q >= step_end) break;                    // warp-uniform: leaf q covers the rest of the step
-          leave_leaf();
-        }
-        pos = step_end;
-        Fi += 32;
-      }
-    }
-#endif
     // the segment's last leaf: its final run counts only if another run follows it in the data set
     if (DUPS && (u64)seg_hi + sh.base < sh.n_global) {
       const I l = (I)((I)(seg_hi + baseI) - carry_F);
@@ -1424,7 +1258,7 @@ constexpr size_t leaf_smem_bytes() {
 }
 
 template <class T, class I, int LEAF, bool DUPS>
-__global__ void RMI_LEAF_BOUNDS
+__global__ void __launch_bounds__(LEAF_THREADS, LEAF_MIN_BLOCKS)
 k_leaf(const T* __restrict__ keys, const Shard<T> sh, u64 N, const u64* __restrict__ S, BuildAux* aux,
        double* __restrict__ params, u64* __restrict__ errors, u64* __restrict__ counts,
        const u32* __restrict__ long_list, int mode_word, u32 block_offset, u32 total_blocks, u32 group_base) {
@@ -1539,31 +1373,21 @@ k_leaf(const T* __restrict__ keys, const Shard<T> sh, u64 N, const u64* __restri
     if (sh.n_local > 0) { prev_key = keys[sh.n_local - 1]; have_prev = true; }
     else if (sh.has_prev) { prev_key = sh.prev_key; have_prev = true; }
   }
-  // The forward pass has no order dependence, so the WARP walks each of its lanes' leaves in turn,
-  // 32 consecutive keys per step straight from global memory (coalesced; the fit pass read the same
-  // lines moments ago, so they come from L2), instead of every lane walking its own leaf through the
-  // row ring a second time.  Owners park their leaf's range and parameters in the warp's shared
-  // memory (the ring is idle now); results return to the owner lane.
   I max_err = 0, run_max = 0;
-#if !RMI_COOP_FORWARD
   // Forward pass: every lane walks its own leaf through the copy ring a second time.  On the headline build this is
-  // faster than the two warp-cooperative variants below (coop_forward: bulk-copy tiles, register look-ahead).
+  // faster than letting the warp walk all of its lanes' leaves cooperatively (coop_forward).
   // Leaves much longer than their warp's other leaves skip the lane-serial walk (one lane would walk it alone while 31
   // wait): the whole warp evaluates them afterwards with coop_forward, 32 keys per step from bulk-copied tiles.  Worth it
   // only when a few lanes are long (when all 32 are, the lane-serial walks are balanced already).
-  constexpr u64 LONG_FWD = RMI_LONG_FWD_MIN;
+  constexpr u64 LONG_FWD = 1024;
   const bool is_long = live && (g_hi - g_lo) > LONG_FWD;
   const unsigned long_mask = __ballot_sync(0xffffffffu, is_long);   // (all lanes vote: no short-circuit)
-#if RMI_LONG_FWD_ALL
   // ... or when (nearly) all are: lane-serial walks over vectors this long are balanced but DRAM-latency bound (two 16-key
   // stages per lane are consumed faster than a copy returns, nothing is left in L2 of a 390 KB warp span), while the
   // cooperative walk streams 2 KB tiles two ahead and its per-leaf bookkeeping is amortised over 32+ steps.
   // With ~1500-key vectors this wins for cubic leaves and loses slightly for linear ones — so only where the
   // evaluation is the longer part of a step.
   const bool long_fwd = is_long && (__popc(long_mask) <= 4 || (LEAF == M_CUBIC && __popc(long_mask) >= 28));
-#else
-  const bool long_fwd = is_long && __popc(long_mask) <= 4;
-#endif
   {
     const u64 pol_fwd = l2_policy_of((mode_word >> 6) & 3);
     const I fwd_hi = long_fwd ? r.lo : r.hi;
@@ -1590,9 +1414,6 @@ k_leaf(const T* __restrict__ keys, const Shard<T> sh, u64 N, const u64* __restri
     }
   }
   coop_forward<T, I, LEAF, DUPS, NANCHECK>(keys, sh, wsm, long_fwd && r.hi > r.lo, r.lo, r.hi, f, max_err, run_max);
-#else
-  coop_forward<T, I, LEAF, DUPS, NANCHECK>(keys, sh, wsm, live && r.hi > r.lo, r.lo, r.hi, f, max_err, run_max);
-#endif
   if (!DUPS) {
     // no two keys of the data set are equal: every run has length 1 (and the data set's final run
     // is never recorded, lower_bound_correction.rs:108-119)
@@ -1866,29 +1687,14 @@ void launch_leaf_inst(const Launch& L, const T* keys, const Shard<T>& sh, u64 N,
   // leaf window of this launch (Launch::leaf_lo/hi), in leaf groups of LEAF_THREADS leaves
   const u64 win_lo = L.leaf_hi ? (L.leaf_lo < N ? L.leaf_lo : N) : 0, win_hi = L.leaf_hi ? (L.leaf_hi < N ? L.leaf_hi : N) : N;
   const u64 G0 = win_lo / LEAF_THREADS, G1 = win_hi > win_lo ? (win_hi + LEAF_THREADS - 1) / LEAF_THREADS : G0;
-  u64 blocks = G1 - G0;
+  const u64 blocks = G1 - G0;
   const u32 gbase = (u32)G0;
-  static const size_t pad = [] { const char* e = getenv("RMI_DEV_LEAF_SMEM_PAD"); return e ? (size_t)atol(e) : (size_t)0; }();
-  const size_t smem = leaf_smem_bytes() + pad;   // dev knob: extra shared memory = fewer resident blocks
+  const size_t smem = leaf_smem_bytes();
   // L2 eviction priority of the key copies: fit pass (bits 4-5), forward pass (bits 6-7);
-  // 0 normal, 1 evict_first, 2 evict_last.  Default: keep what the fit pass read, release after the re-read.
-  static const int l2_mode = [] {
-    const char* e = getenv("RMI_DEV_L2_HINT");
-    int fit = 2, fwd = 1;
-    if (e && e[0] && e[1]) { fit = (e[0] - '0') & 3; fwd = (e[1] - '0') & 3; }
-    return (fit << 4) | (fwd << 6);
-  }();
+  // 0 normal, 1 evict_first, 2 evict_last.  Keep what the fit pass read, release it after the re-read.
+  constexpr int L2_MODE = (2 << 4) | (1 << 6);
   ensure_rcp_far();
   cudaFuncSetAttribute(k_leaf<T, I, LEAF, DUPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, LONG_LEAF_SMEM);
-  static const bool print_occ = getenv("RMI_DEV_PRINT_OCC") != nullptr;
-  if (print_occ) {
-    int nb = 0;
-    cudaFuncAttributes fa;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_leaf<T, I, LEAF, DUPS>, LEAF_THREADS, smem);
-    cudaFuncGetAttributes(&fa, k_leaf<T, I, LEAF, DUPS>);
-    fprintf(stderr, "[rmi_b200] k_leaf: %d threads/block, %zu B dynamic smem, %d registers -> %d blocks/SM\n", LEAF_THREADS, smem,
-            fa.numRegs, nb);
-  }
   const bool fork = LEAF == M_LINEAR && L.side && L.ev_fork && L.ev_join && L.d_long && N < 0xffffffffull;
   if (fork) {
     // Long leaves (the two end leaves of a regression top model collect every key it places
@@ -1901,18 +1707,17 @@ void launch_leaf_inst(const Launch& L, const T* keys, const Shard<T>& sh, u64 N,
     cudaEventRecord(L.ev_fork, L.stream);
     cudaStreamWaitEvent(L.side, L.ev_fork, 0);
     k_leaf<T, I, LEAF, DUPS><<<LONG_LEAF_CAP, 32, LONG_LEAF_SMEM, L.side>>>(keys, sh, N, d_S, d_aux, d_params, d_errors, d_counts, L.d_long,
-                                                                            1 | l2_mode, 0u, LONG_LEAF_CAP, 0u);
+                                                                            1 | L2_MODE, 0u, LONG_LEAF_CAP, 0u);
     count_launch();
     cudaEventRecord(L.ev_join, L.side);
   }
   const u32* long_list = fork ? L.d_long : nullptr;
   const LeafCopyOut* co = L.copy;
-  int K = (co && co->slices > 1) ? (co->slices < MAX_LEAF_SLICES ? co->slices : MAX_LEAF_SLICES) : 1;
-  if (blocks < (u64)K * 64 || blocks >= 0xffffffffull) K = 1;   // too small to be worth slicing
-  if (K == 1) {
+  const bool sliced = co && blocks >= (u64)LEAF_SLICES * 64 && blocks < 0xffffffffull;   // else too small to be worth slicing
+  if (!sliced) {
     if (blocks) {
       k_leaf<T, I, LEAF, DUPS><<<(unsigned)blocks, LEAF_THREADS, smem, L.stream>>>(keys, sh, N, d_S, d_aux, d_params, d_errors, d_counts,
-                                                                                  long_list, l2_mode, 0u, (u32)blocks, gbase);
+                                                                                  long_list, L2_MODE, 0u, (u32)blocks, gbase);
       count_launch();
     }
     if (fork) cudaStreamWaitEvent(L.stream, L.ev_join, 0);
@@ -1935,15 +1740,15 @@ void launch_leaf_inst(const Launch& L, const T* keys, const Shard<T>& sh, u64 N,
   // Slice sizes taper towards the end: the copy engine keeps up with the kernel (the records cross PCIe in about the
   // time the kernel takes to produce them), so what stays exposed is the LAST slice's copy — the last two slices are 16% and 8%
   // of the blocks, the others share the rest equally.  (even offsets: block ids alternate between front and back groups)
-  u32 bounds_[MAX_LEAF_SLICES + 1];
+  u32 bounds_[LEAF_SLICES + 1];
   {
-    const double tail2 = K >= 4 ? 0.16 : 0.0, tail1 = K >= 4 ? 0.08 : 0.0;
-    const int nbody = K >= 4 ? K - 2 : K;
+    constexpr double tail2 = 0.16, tail1 = 0.08;
+    constexpr int nbody = LEAF_SLICES - 2;
     double acc = 0.0;
     bounds_[0] = 0;
-    for (int c = 0; c < K; ++c) {
-      acc += c < nbody ? (1.0 - tail2 - tail1) / nbody : (c == K - 2 ? tail2 : tail1);
-      u32 b = c + 1 == K ? total : (u32)((u64)((double)total * acc + 1.0) & ~1ull);
+    for (int c = 0; c < LEAF_SLICES; ++c) {
+      acc += c < nbody ? (1.0 - tail2 - tail1) / nbody : (c == LEAF_SLICES - 2 ? tail2 : tail1);
+      u32 b = c + 1 == LEAF_SLICES ? total : (u32)((u64)((double)total * acc + 1.0) & ~1ull);
       if (b > total) b = total;
       if (b < bounds_[c]) b = bounds_[c];
       bounds_[c + 1] = b;
@@ -1951,7 +1756,7 @@ void launch_leaf_inst(const Launch& L, const T* keys, const Shard<T>& sh, u64 N,
   }
   cudaEventRecord(co->ev_ready, L.stream);
   int used = 0;
-  for (int c = 0; c < K; ++c) {
+  for (int c = 0; c < LEAF_SLICES; ++c) {
     const u32 off = bounds_[c];
     if (off >= total) break;
     const u32 cnt = bounds_[c + 1] - off;
@@ -1959,7 +1764,7 @@ void launch_leaf_inst(const Launch& L, const T* keys, const Shard<T>& sh, u64 N,
     cudaStream_t st = co->streams[used];
     cudaStreamWaitEvent(st, co->ev_ready, 0);
     k_leaf<T, I, LEAF, DUPS><<<cnt, LEAF_THREADS, smem, st>>>(keys, sh, N, d_S, d_aux, d_params, d_errors, d_counts, long_list,
-                                                              l2_mode, off, total, gbase);
+                                                              L2_MODE, off, total, gbase);
     count_launch();
     cudaEventRecord(co->ev_kernel[used], st);
     cudaStreamWaitEvent(L.stream, co->ev_kernel[used], 0);
@@ -1991,7 +1796,7 @@ template <class T, int LEAF>
 void launch_leaf(const Launch& L, const T* keys, const Shard<T>& sh, u64 N, const u64* d_S, BuildAux* d_aux,
                  double* d_params, u64* d_errors, u64* d_counts) {
   constexpr bool SPECIALISED = LEAF == M_LINEAR || LEAF == M_LINEAR_SPLINE || LEAF == M_CUBIC;
-  if (sh.n_global < 0xfffffc00ull) {   // 32-bit indices (with room for the forward pass's look-ahead: no index arithmetic wraps)
+  if (sh.n_global < 0xfffffc00ull) {   // 32-bit indices (with room for the forward pass's 32-key steps past a leaf's end: no index arithmetic wraps)
     if (SPECIALISED && sh.no_dups)
       launch_leaf_inst<T, u32, SPECIALISED ? LEAF : M_LINEAR, false>(L, keys, sh, N, d_S, d_aux, d_params, d_errors, d_counts);
     else

@@ -39,7 +39,6 @@ for spec, bf, flags in configs:
         print(json.dumps({"spec": spec, "bf": bf, "flags": flags, "wall_ms": (t1 - t0) * 1e3,
                           "wall_ms_min": walls[0], "wall_ms_med": walls[len(walls) // 2], "device_ms_min": devs[0],
                           "leaf_ms_min": leafs[0], "leaf_ms_med": leafs[len(leafs) // 2],
-                          "env": {k: v for k, v in os.environ.items() if k.startswith("RMI_DEV")},
                           "lib_wall_ms": r.build_time / 1e6, "device_ms": r.device_time_ns / 1e6,
                           "phases_ms": [p / 1e6 for p in r.phase_device_ns], "max_err": r.model_max_error, "max_leaf_keys": int(r.l1_counts.max()) if r.l1_counts is not None else None,
                           "avg_log2": r.model_avg_log2_error, "keys_per_s_device": n / (r.device_time_ns / 1e9)}))
