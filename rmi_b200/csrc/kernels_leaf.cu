@@ -34,9 +34,11 @@ namespace {
 
 constexpr int BOUNDS_THREADS = 256;
 constexpr int LEAF_THREADS = 128;
-// Resident blocks per SM the compiler must allow for: 20 warps (the padded copy ring takes 41 KB of shared memory per
-// 128-lane block, so 5 blocks fit), i.e. at most 96 registers.
-constexpr int LEAF_MIN_BLOCKS = 640 / LEAF_THREADS;
+// Resident blocks per SM: exactly this many (leaf_smem_bytes() keeps one more from fitting), 8 warps.  A leaf's keys
+// are read twice, by the fit pass and one whole leaf later by the forward pass, and the fewer leaves are in flight
+// per SM, the more of the second read L2 still holds (DESIGN §4).  Measured on an H100 SXM (400 W limit) on the
+// headline build, k_leaf takes 1.46 ms at 5 blocks, 1.39 ms at 4, 1.26 ms at 3, 1.18 ms at 2 and 1.52 ms at 1.
+constexpr int LEAF_MIN_BLOCKS = 2;
 constexpr int RCP_TABLE = 512;   // reciprocals of the counts below this live in shared memory
 
 __device__ __forceinline__ void set_status(BuildAux* aux, unsigned bit) { atomicOr(&aux->status, bit); }
@@ -1252,10 +1254,15 @@ k_find_long(const Shard<T> sh, u64 N, const u64* __restrict__ S, u32* __restrict
 }
 
 constexpr int RCP_RING_BYTES = 64 * 8;   // per warp (LeafWelford::ring), 512-byte aligned: one extra ring of slack per block
+constexpr size_t SM_SMEM_BYTES = 228 * 1024;   // an H100 SM's shared memory; the runtime reserves 1 KB of it per block
+// What a block uses, raised so that LEAF_MIN_BLOCKS + 1 blocks do not fit on an SM.
 constexpr size_t leaf_smem_bytes() {
-  return (size_t)RCP_TABLE * sizeof(double) + (size_t)(LEAF_THREADS / 32) * WARP_STREAM_BYTES +
-         (size_t)(LEAF_THREADS / 32 + 1) * RCP_RING_BYTES;
+  constexpr size_t used = (size_t)RCP_TABLE * sizeof(double) + (size_t)(LEAF_THREADS / 32) * WARP_STREAM_BYTES +
+                          (size_t)(LEAF_THREADS / 32 + 1) * RCP_RING_BYTES;
+  constexpr size_t cap = SM_SMEM_BYTES / (LEAF_MIN_BLOCKS + 1) - 1024 + 16;
+  return used > cap ? used : cap;
 }
+static_assert(LEAF_MIN_BLOCKS * (leaf_smem_bytes() + 1024) <= SM_SMEM_BYTES, "LEAF_MIN_BLOCKS blocks must fit an SM");
 
 template <class T, class I, int LEAF, bool DUPS>
 __global__ void __launch_bounds__(LEAF_THREADS, LEAF_MIN_BLOCKS)
