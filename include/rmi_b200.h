@@ -161,6 +161,31 @@ void rmi_result_free(rmi_result* r);
 int rmi_train_stats_batch(const rmi_dataset* ds, const char* top_model, const char* const* leaf_models, int num_leaf_models,
                           uint64_t branch_factor, uint32_t flags, rmi_result** out);
 
+/* ---- Batched lookups on the GPU ------------------------------------------------------------------
+ * A trained RMI bound to the device-resident keys it was trained on.  For a query q of the dataset's key type:
+ *   predict      pos = the generated code's lookup(q, &err) (codegen.rs:612-718): t = min(N-1, top(q)),
+ *                pos = min(n-1, leaf[t](q)), err = the error bound of leaf t; a NaN prediction maps to 0.
+ *   lower_bound  the number of keys k with k < q (std::lower_bound; n past the last key, 0 for a NaN query),
+ *                always exact: a binary search over [pos-err, pos+err], confirmed by the keys just outside that
+ *                window, and a galloping search outward when the window misses (never, for a key of the data set). */
+typedef struct rmi_index rmi_index;
+/* Upload r's top model (incl. radix table / histogram arrays) and its leaf tables, packed, to ds's device and
+ * bind them to ds's keys.  r must hold the leaf tables (not RMI_FLAG_STATS_ONLY) and r->num_rmi_rows must equal
+ * rmi_dataset_len(ds); ds must outlive the index.  Immutable: concurrent calls on different streams are fine. */
+int rmi_index_create(const rmi_result* r, const rmi_dataset* ds, rmi_index** out);
+void rmi_index_destroy(rmi_index* idx);
+/* n queries (ds's key type) in device memory on the index's device; enqueued on cuda_stream, no host sync.
+ * One kernel launch per call (n == 0: none).  d_err may be NULL. */
+int rmi_index_predict(const rmi_index* idx, const void* d_queries, uint64_t n, uint64_t* d_pos, uint64_t* d_err,
+                      void* cuda_stream);
+/* Exact lower bounds; *d_fallbacks (may be NULL) is incremented by the number of queries whose window missed. */
+int rmi_index_lower_bound(const rmi_index* idx, const void* d_queries, uint64_t n, uint64_t* d_out,
+                          uint64_t* d_fallbacks, void* cuda_stream);
+/* The same on host arrays, synchronously: copies the queries to the device, runs predict (lower_bound == 0; host_err
+ * may be NULL) or lower_bound (*fallbacks, may be NULL, is SET to the fallback count) and copies the results back. */
+int rmi_index_lookup_host(const rmi_index* idx, const void* host_queries, uint64_t n, int lower_bound,
+                          uint64_t* host_out, uint64_t* host_err, uint64_t* fallbacks);
+
 /* ---- Range-partitioned (multi-GPU) build ----------------------------------------------------
  * One process per GPU; rank r holds the r-th contiguous slab of the globally sorted key array
  * in an rmi_dataset.  The leaf fits are independent once the top model and the leaf boundaries

@@ -87,6 +87,12 @@ def load_library():
                                      C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64]
         L.rmi_find_pareto_efficient_configs.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_uint64, C.c_uint32,
                                                         C.POINTER(_ConfigStats), C.c_uint64, C.POINTER(C.c_uint64)]
+        L.rmi_index_create.argtypes = [C.POINTER(_Result), C.c_void_p, C.POINTER(C.c_void_p)]
+        L.rmi_index_destroy.argtypes = [C.c_void_p]
+        L.rmi_index_predict.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.rmi_index_lower_bound.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.rmi_index_lookup_host.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_void_p, C.c_void_p,
+                                            C.c_void_p]
         _lib = L
     return _lib
 
@@ -390,3 +396,67 @@ def result_from_pointer(res, model_spec: str) -> TrainedRMI:
             l1_counts=_arr(r.l1_counts, N, C.c_uint64, np.uint64, owner),
             could_not_replace=bool(r.could_not_replace), top_fit_exact=bool(r.top_fit_exact), _res=owner)
     return out
+
+
+class RMIIndex:
+    """A trained RMI bound to the device-resident keys it was trained on, for batched lookups on the GPU.
+
+    ``predict(q)`` returns the generated code's ``lookup(key, &err)`` for every query as ``(pos, err)``;
+    ``lower_bound(q)`` returns the exact number of keys below each query (``std::lower_bound``).  Both take a
+    numpy array of the dataset's key type and return ``np.uint64`` arrays.  The ``*_device`` forms take raw device
+    pointers and a CUDA stream handle (torch: ``t.data_ptr()``, ``torch.cuda.current_stream().cuda_stream``) and
+    enqueue one kernel without synchronising.  ``trained`` must hold its leaf tables (not FLAG_STATS_ONLY) and
+    ``data`` must be the key set it was trained on; the index keeps ``data`` alive.
+    """
+
+    def __init__(self, trained: TrainedRMI, data: RMITrainingData):
+        self._h = C.c_void_p()
+        self.data = data
+        self.key_type = data.key_type
+        self._trained = trained
+        _check(load_library().rmi_index_create(_result_ptr(trained), data._h, C.byref(self._h)))
+
+    def _queries(self, q) -> np.ndarray:
+        if not isinstance(q, np.ndarray) or q.dtype != np.dtype(_NP_OF_KEY[self.key_type]):
+            got = q.dtype if isinstance(q, np.ndarray) else type(q).__name__
+            raise TypeError(f"queries must be a numpy array of {np.dtype(_NP_OF_KEY[self.key_type])}, got {got}")
+        return np.ascontiguousarray(q)
+
+    def predict(self, q: np.ndarray):
+        """(pos, err) per query, as np.uint64 arrays."""
+        q = self._queries(q)
+        pos = np.empty(q.size, dtype=np.uint64)
+        err = np.empty(q.size, dtype=np.uint64)
+        _check(load_library().rmi_index_lookup_host(self._h, q.ctypes.data_as(C.c_void_p), q.size, 0,
+                                                     pos.ctypes.data_as(C.c_void_p), err.ctypes.data_as(C.c_void_p),
+                                                     None))
+        return pos, err
+
+    def lower_bound(self, q: np.ndarray, return_fallbacks: bool = False):
+        """Exact lower bound per query (np.uint64); with return_fallbacks also the number of queries whose
+        error window missed the answer."""
+        q = self._queries(q)
+        out = np.empty(q.size, dtype=np.uint64)
+        fb = C.c_uint64(0)
+        _check(load_library().rmi_index_lookup_host(self._h, q.ctypes.data_as(C.c_void_p), q.size, 1,
+                                                     out.ctypes.data_as(C.c_void_p), None, C.byref(fb)))
+        return (out, int(fb.value)) if return_fallbacks else out
+
+    def predict_device(self, q_ptr: int, n: int, pos_ptr: int, err_ptr: int = 0, stream: int = 0) -> None:
+        _check(load_library().rmi_index_predict(self._h, C.c_void_p(q_ptr), int(n), C.c_void_p(pos_ptr),
+                                                C.c_void_p(err_ptr or None), C.c_void_p(stream or None)))
+
+    def lower_bound_device(self, q_ptr: int, n: int, out_ptr: int, fallbacks_ptr: int = 0, stream: int = 0) -> None:
+        _check(load_library().rmi_index_lower_bound(self._h, C.c_void_p(q_ptr), int(n), C.c_void_p(out_ptr),
+                                                    C.c_void_p(fallbacks_ptr or None), C.c_void_p(stream or None)))
+
+    def close(self):
+        if getattr(self, "_h", None) and self._h.value:
+            load_library().rmi_index_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

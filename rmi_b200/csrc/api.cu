@@ -453,6 +453,185 @@ void rmi_result_free(rmi_result* r) { delete reinterpret_cast<ResultBox*>(r); }
 
 }  // extern "C"
 
+// A trained RMI bound to the device-resident keys it was trained on: the top model by value (its tables in device
+// memory) and one packed record per leaf (kernels.h: lookup_record_bytes).  Immutable after creation.
+struct rmi_index {
+  const rmi_dataset* ds = nullptr;
+  TopModel top;              // t32 / pivots / radix_index point at the device copies below
+  int leaf_kind = 0;
+  uint64_t N = 0;
+  void* d_records = nullptr;
+  u32* d_t32 = nullptr;
+  u64* d_pivots = nullptr;
+  u64* d_radix_index = nullptr;
+  int num_sms = 0;
+};
+
+namespace {
+void index_free_device(rmi_index* idx) {
+  cudaFree(idx->d_records);
+  cudaFree(idx->d_t32);
+  cudaFree(idx->d_pivots);
+  cudaFree(idx->d_radix_index);
+}
+
+int index_check_call(const rmi_index* idx, const void* d_queries, uint64_t n, const void* d_out, const char* fn) {
+  if (!idx) return fail(RMI_ERR_INVALID, std::string(fn) + ": null index");
+  if (n && (!d_queries || !d_out)) return fail(RMI_ERR_INVALID, std::string(fn) + ": null query or output pointer");
+  return RMI_OK;
+}
+
+int index_launch(const rmi_index* idx, const void* d_queries, uint64_t n, uint64_t* d_out, uint64_t* d_err,
+                 uint64_t* d_fallbacks, void* cuda_stream, bool lower_bound) {
+  if (n == 0) return RMI_OK;
+  const rmi_dataset* ds = idx->ds;
+  CUDA_TRY(cudaSetDevice(ds->device));
+  Launch L{(cudaStream_t)cuda_stream, idx->num_sms};
+  switch (ds->key_type) {
+    case RMI_KEY_U64:
+      lookup_batch<u64>(L, idx->top, idx->leaf_kind, idx->d_records, idx->N, (const u64*)ds->d_keys, ds->n,
+                        (const u64*)d_queries, n, (u64*)d_out, (u64*)d_err, (u64*)d_fallbacks, lower_bound);
+      break;
+    case RMI_KEY_U32:
+      lookup_batch<u32>(L, idx->top, idx->leaf_kind, idx->d_records, idx->N, (const u32*)ds->d_keys, ds->n,
+                        (const u32*)d_queries, n, (u64*)d_out, (u64*)d_err, (u64*)d_fallbacks, lower_bound);
+      break;
+    default:
+      lookup_batch<double>(L, idx->top, idx->leaf_kind, idx->d_records, idx->N, (const double*)ds->d_keys, ds->n,
+                           (const double*)d_queries, n, (u64*)d_out, (u64*)d_err, (u64*)d_fallbacks,
+                           lower_bound);
+      break;
+  }
+  CUDA_TRY(cudaGetLastError());
+  return RMI_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int rmi_index_create(const rmi_result* r, const rmi_dataset* ds, rmi_index** out) {
+  if (!r || !ds || !out) return fail(RMI_ERR_INVALID, "rmi_index_create: null argument");
+  if (!r->l1_params || !r->l1_errors)
+    return fail(RMI_ERR_INVALID, "rmi_index_create: the result holds no leaf tables (trained with RMI_FLAG_STATS_ONLY)");
+  if (r->num_rmi_rows != ds->n)
+    return fail(RMI_ERR_INVALID, "rmi_index_create: the result was trained on " + std::to_string(r->num_rmi_rows) +
+                                     " keys, the dataset holds " + std::to_string(ds->n));
+  if (ds->n == 0 || r->branching_factor == 0) return fail(RMI_ERR_INVALID, "rmi_index_create: empty index");
+  if (lookup_top_group((int)r->l0_model_id) < 0 || lookup_leaf_group((int)r->l1_model_id) < 0)
+    return fail(RMI_ERR_UNSUPPORTED, "rmi_index_create: unsupported model id (top " + std::to_string(r->l0_model_id) +
+                                         ", leaf " + std::to_string(r->l1_model_id) + ")");
+  if (r->l1_params_per_model != (uint32_t)leaf_params_per_model((int)r->l1_model_id))
+    return fail(RMI_ERR_INVALID, "rmi_index_create: wrong number of leaf parameters");
+  if (r->l0_model_id == M_RADIX_TABLE &&
+      (!r->l0_table32 || r->l0_table_bits > 32 || r->l0_table32_len != ((uint64_t)1 << r->l0_table_bits)))
+    return fail(RMI_ERR_INVALID, "rmi_index_create: radix table missing or of the wrong size");
+  if (r->l0_model_id == M_HISTOGRAM && (!r->l0_array2 || !r->l0_array2_len))
+    return fail(RMI_ERR_INVALID, "rmi_index_create: histogram pivots missing");
+
+  CUDA_TRY(cudaSetDevice(ds->device));
+  DeviceInfo di;
+  if (int rc = device_info(ds->device, &di)) return rc;
+  auto* idx = new rmi_index();
+  idx->ds = ds;
+  idx->leaf_kind = (int)r->l1_model_id;
+  idx->N = r->branching_factor;
+  idx->num_sms = di.num_sms;
+  TopModel& t = idx->top;
+  memset(&t, 0, sizeof(t));
+  t.kind = (int)r->l0_model_id;
+  t.high = (int)r->l0_bradix_high;
+  t.table_bits = (int)r->l0_table_bits;
+  for (int q = 0; q < 4; ++q) { t.f[q] = r->l0_fparams[q]; t.ip[q] = r->l0_iparams[q]; }
+  std::vector<char> packed((size_t)idx->N * lookup_record_bytes(idx->leaf_kind));
+  pack_leaf_records(idx->leaf_kind, r->l1_params, (const u64*)r->l1_errors, idx->N, packed.data());
+  cudaError_t e = cudaMalloc(&idx->d_records, packed.size());
+  if (e == cudaSuccess) e = cudaMemcpy(idx->d_records, packed.data(), packed.size(), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess && t.kind == M_RADIX_TABLE) {
+    e = cudaMalloc(&idx->d_t32, sizeof(u32) * r->l0_table32_len);
+    if (e == cudaSuccess) e = cudaMemcpy(idx->d_t32, r->l0_table32, sizeof(u32) * r->l0_table32_len, cudaMemcpyHostToDevice);
+    t.t32 = idx->d_t32;
+  }
+  if (e == cudaSuccess && t.kind == M_HISTOGRAM) {
+    e = cudaMalloc(&idx->d_pivots, sizeof(u64) * r->l0_array2_len);
+    if (e == cudaSuccess) e = cudaMemcpy(idx->d_pivots, r->l0_array2, sizeof(u64) * r->l0_array2_len, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && r->l0_array1 && r->l0_array1_len) {
+      e = cudaMalloc(&idx->d_radix_index, sizeof(u64) * r->l0_array1_len);
+      if (e == cudaSuccess)
+        e = cudaMemcpy(idx->d_radix_index, r->l0_array1, sizeof(u64) * r->l0_array1_len, cudaMemcpyHostToDevice);
+    }
+    t.pivots = idx->d_pivots;
+    t.radix_index = idx->d_radix_index;
+    t.npivots = r->l0_array2_len;
+  }
+  if (e != cudaSuccess) {
+    index_free_device(idx);
+    delete idx;
+    return fail(RMI_ERR_CUDA, std::string("rmi_index_create: ") + cudaGetErrorString(e));
+  }
+  *out = idx;
+  return RMI_OK;
+}
+
+void rmi_index_destroy(rmi_index* idx) {
+  if (!idx) return;
+  cudaSetDevice(idx->ds->device);
+  index_free_device(idx);
+  delete idx;
+}
+
+int rmi_index_predict(const rmi_index* idx, const void* d_queries, uint64_t n, uint64_t* d_pos, uint64_t* d_err,
+                      void* cuda_stream) {
+  if (int rc = index_check_call(idx, d_queries, n, d_pos, "rmi_index_predict")) return rc;
+  return index_launch(idx, d_queries, n, d_pos, d_err, nullptr, cuda_stream, false);
+}
+
+int rmi_index_lower_bound(const rmi_index* idx, const void* d_queries, uint64_t n, uint64_t* d_out,
+                          uint64_t* d_fallbacks, void* cuda_stream) {
+  if (int rc = index_check_call(idx, d_queries, n, d_out, "rmi_index_lower_bound")) return rc;
+  return index_launch(idx, d_queries, n, d_out, nullptr, d_fallbacks, cuda_stream, true);
+}
+
+int rmi_index_lookup_host(const rmi_index* idx, const void* host_queries, uint64_t n, int lower_bound,
+                          uint64_t* host_out, uint64_t* host_err, uint64_t* fallbacks) {
+  if (int rc = index_check_call(idx, host_queries, n, host_out, "rmi_index_lookup_host")) return rc;
+  if (n == 0) return RMI_OK;
+  CUDA_TRY(cudaSetDevice(idx->ds->device));
+  const size_t qb = (size_t)n * key_bytes(idx->ds->key_type), ob = (size_t)n * sizeof(uint64_t);
+  cudaStream_t st = nullptr;
+  char* d = nullptr;   // queries | out | err | fallback counter
+  cudaError_t e = cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking);
+  if (e == cudaSuccess) e = cudaMallocAsync((void**)&d, qb + 2 * ob + 8 + 8, st);
+  int rc = RMI_OK;
+  if (e == cudaSuccess) {
+    char* d_q = d;
+    uint64_t* d_out = (uint64_t*)(d + ((qb + 7) & ~(size_t)7));
+    uint64_t* d_err = d_out + n;
+    uint64_t* d_fb = d_err + n;
+    e = cudaMemcpyAsync(d_q, host_queries, qb, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(d_fb, 0, sizeof(u64), st);
+    if (e == cudaSuccess) {
+      rc = lower_bound ? index_launch(idx, d_q, n, d_out, nullptr, d_fb, st, true)
+                       : index_launch(idx, d_q, n, d_out, host_err ? d_err : nullptr, nullptr, st, false);
+    }
+    if (e == cudaSuccess && rc == RMI_OK) e = cudaMemcpyAsync(host_out, d_out, ob, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess && rc == RMI_OK && !lower_bound && host_err)
+      e = cudaMemcpyAsync(host_err, d_err, ob, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess && rc == RMI_OK && lower_bound && fallbacks)
+      e = cudaMemcpyAsync(fallbacks, d_fb, sizeof(u64), cudaMemcpyDeviceToHost, st);
+    cudaFreeAsync(d, st);
+  }
+  if (st) {
+    cudaError_t es = cudaStreamSynchronize(st);
+    if (e == cudaSuccess) e = es;
+    cudaStreamDestroy(st);
+  }
+  if (rc != RMI_OK) return rc;
+  if (e != cudaSuccess) return fail(RMI_ERR_CUDA, std::string("rmi_index_lookup_host: ") + cudaGetErrorString(e));
+  return RMI_OK;
+}
+
+}  // extern "C"
+
 namespace {
 
 // Streams / events of the sliced leaf launch (kernels.h: LeafCopyOut), created once per host

@@ -141,6 +141,23 @@ void leaf_statistics_owned(const Launch& L, u64 n, u64 N, const u64* d_errors, c
                            int world, void* d_part_out, void* scratch);
 void leaf_statistics_merge(const Launch& L, const void* d_parts, int world, BuildAux* d_aux);
 
+// ---- batched lookups on a trained index (kernels_lookup.cu) -----------------------------------
+// The model groups the lookup kernel is instantiated for (-1: not a top / leaf model): the linear family shares
+// one group, as in compute_leaf_bounds.
+int lookup_top_group(int kind);
+int lookup_leaf_group(int kind);
+// One packed record per leaf: its parameters in Model::params() order, then its error bound.
+__host__ __device__ constexpr int lookup_record_bytes(int leaf_kind) { return leaf_kind == M_CUBIC ? 64 : 32; }
+// N records (N x lookup_record_bytes bytes at `out`, host memory) from N x ppm parameters and N errors.
+void pack_leaf_records(int leaf_kind, const double* params, const u64* errors, u64 N, void* out);
+// One kernel launch on L.stream (none for nq == 0).  lower_bound = false: out = position estimates, out_err (may be
+// null) = the leaves' error bounds.  lower_bound = true: out = exact lower bounds over keys[0, n); *fallbacks (may be
+// null) grows by the number of queries whose error window missed.  `top` is passed by value; its table pointers
+// (t32, pivots, radix_index) are device memory.
+template <class T>
+void lookup_batch(const Launch& L, const TopModel& top, int leaf_kind, const void* d_records, u64 N, const T* keys, u64 n,
+                  const T* d_queries, u64 nq, u64* d_out, u64* d_out_err, u64* d_fallbacks, bool lower_bound);
+
 // ---- range-partitioned build phases (kernels_shard.cu) ---------------------------------------
 size_t shard_scratch_bytes();
 template <class T>

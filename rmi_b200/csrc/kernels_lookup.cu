@@ -1,0 +1,255 @@
+// kernels_lookup.cu — batched lookups on a trained two-layer RMI (DESIGN §11).
+//
+// predict:      t = min(N-1, top(q)),  pos = min(n-1, leaf[t](q)),  err = error bound of leaf t
+//               — the generated code's lookup(key, &err) (codegen.rs:612-718), with NaN -> 0 where the
+//               generated code's FCLAMP is undefined.
+// lower_bound:  the number of keys k with k < q, found by a branchless binary search over the window
+//               [pos-err, pos+err] (clamped to [0, n]) and confirmed by the keys just outside it.  A window
+//               that does not bracket the answer falls back to a galloping search outward from its edge
+//               and is counted.  For every key of the data set the window brackets the answer (the
+//               reference's property, tests/simple_model_wiki/main.cpp:26-42), so the fallback only runs
+//               for queries the index was not trained on.
+//
+// Thread mapping: a block takes a tile of LOOKUP_THREADS * LOOKUP_Q consecutive queries (grid-stride over
+// tiles); thread x owns queries x, x + LOOKUP_THREADS, ... of the tile, so every query load and result store
+// is coalesced.  The thread carries its LOOKUP_Q queries through the dependent chain — top model, leaf record,
+// key probes — in lockstep, which keeps LOOKUP_Q independent loads in flight per step.
+#include <cstring>
+
+#include "kernels.h"
+
+namespace rmi {
+
+namespace {
+
+// Queries per thread and threads per block, measured on an H100 SXM (DESIGN §11) on the headline index
+// (linear,linear 2^20 over 200M uint64 keys, 2^27 random present keys): lower_bound took 27.4 / 34.2 / 36.6 /
+// 37.0 ms at 1 / 2 / 4 / 8 queries per thread with 128 threads (28.4 / 33.9 / 35.2 / 37.2 ms with 256); predict
+// was 2.65-2.72 ms at 1, 2 and 4 and 2.95 ms at 8.  One query per thread needs 32 registers, so 64 warps fit on
+// an SM, and those warps keep more probes in flight than fewer warps carrying several queries each: the lockstep
+// search waits for the longest window of its queries, and the registers it needs cost warps.
+constexpr int LOOKUP_Q = 1;
+constexpr int LOOKUP_THREADS = 128;
+constexpr int LOOKUP_MAX_BLOCKS_PER_SM = 32;   // grid cap; beyond it the blocks stride over the tiles
+
+// The packed leaf record (pack_leaf_records): parameters, then the error bound, in 16-byte vectors.
+//   32 B: {f0, f1}, {f2, err}               linear family, loglinear, normal, lognormal (f2 = 0 for 2 params)
+//   64 B: {f0, f1}, {f2, f3}, {err, 0}, pad  cubic
+template <int LEAF> struct Rec {
+  static constexpr int VECS = LEAF == M_CUBIC ? 4 : 2;   // stride in 16-byte vectors
+  static constexpr int LOADS = LEAF == M_CUBIC ? 3 : 2;  // vectors a lookup reads
+  __device__ __forceinline__ static void unpack(const ulonglong2 (&v)[LOADS], double* f, u64& err) {
+    f[0] = __longlong_as_double((long long)v[0].x);
+    f[1] = __longlong_as_double((long long)v[0].y);
+    f[2] = __longlong_as_double((long long)v[1].x);
+    if (LEAF == M_CUBIC) {
+      f[3] = __longlong_as_double((long long)v[1].y);
+      err = v[LOADS - 1].x;
+    } else {
+      f[3] = 0.0;
+      err = v[1].y;
+    }
+  }
+};
+
+// First index in [lo, hi) whose key is not < q, or hi.
+template <class T> __device__ __forceinline__ u64 search_range(const T* __restrict__ keys, u64 lo, u64 hi, T q) {
+  while (lo < hi) {
+    u64 mid = lo + ((hi - lo) >> 1);
+    if (keys[mid] < q) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+// The window [lo, hi] missed: the answer is below lo (!left_ok: keys[lo-1] is not < q) or above hi
+// (keys[hi] < q).  Gallop outward from that edge until the answer is bracketed, then search the bracket.
+template <class T>
+__device__ __noinline__ u64 lookup_fallback(const T* __restrict__ keys, u64 n, T q, u64 lo, u64 hi, bool left_ok) {
+  if (!left_ok) {
+    u64 R = lo - 1, step = 1, L = 0;   // answer <= R
+    while (true) {
+      if (R < step) { L = 0; break; }
+      u64 c = R - step;
+      if (keys[c] < q) { L = c + 1; break; }
+      R = c;
+      step <<= 1;
+    }
+    return search_range(keys, L, R, q);
+  }
+  u64 L = hi + 1, step = 1, R = n;     // answer >= L
+  while (true) {
+    if (n - L < step) { R = n; break; }
+    u64 c = L + step - 1;
+    if (!(keys[c] < q)) { R = c; break; }
+    L = c + 1;
+    step <<= 1;
+  }
+  return search_range(keys, L, R, q);
+}
+
+template <class T, int TOP, int LEAF>
+__global__ void __launch_bounds__(LOOKUP_THREADS)
+k_lookup(const __grid_constant__ TopModel top, const ulonglong2* __restrict__ recs, const T* __restrict__ keys, u64 n,
+         u64 N, const T* __restrict__ qs, u64 nq, u64* __restrict__ out, u64* __restrict__ out_err, u64* fallbacks,
+         int lower_bound) {
+  using R = Rec<LEAF>;
+  constexpr int Q = LOOKUP_Q;
+  const u64 tile = (u64)LOOKUP_THREADS * Q;
+  unsigned misses = 0;
+  for (u64 base = (u64)blockIdx.x * tile; base < nq; base += (u64)gridDim.x * tile) {
+    T q[Q];
+    bool live[Q];
+    u64 t[Q];
+#pragma unroll
+    for (int j = 0; j < Q; ++j) {
+      u64 i = base + threadIdx.x + (u64)j * LOOKUP_THREADS;
+      live[j] = i < nq;
+      q[j] = live[j] ? __ldcs(qs + i) : T(0);
+    }
+#pragma unroll
+    for (int j = 0; j < Q; ++j) {
+      u64 p = top_predict<TOP>(top, q[j]);
+      t[j] = p < N - 1 ? p : N - 1;
+    }
+    ulonglong2 v[Q][R::LOADS];
+#pragma unroll
+    for (int j = 0; j < Q; ++j)
+#pragma unroll
+      for (int k = 0; k < R::LOADS; ++k) v[j][k] = __ldg(recs + t[j] * R::VECS + k);
+    u64 pos[Q], err[Q];
+#pragma unroll
+    for (int j = 0; j < Q; ++j) {
+      double f[4];
+      R::unpack(v[j], f, err[j]);
+      u64 p = leaf_predict64<LEAF>(f, Key<T>::as_float(q[j]));
+      pos[j] = p < n - 1 ? p : n - 1;
+    }
+    if (!lower_bound) {
+#pragma unroll
+      for (int j = 0; j < Q; ++j) {
+        u64 i = base + threadIdx.x + (u64)j * LOOKUP_THREADS;
+        if (!live[j]) continue;
+        __stcs(out + i, pos[j]);
+        if (out_err) __stcs(out_err + i, err[j]);
+      }
+      continue;
+    }
+    // window [lo, hi] of candidate answers; the search covers keys [lo, hi)
+    u64 lo[Q], hi[Q], b[Q], len[Q];
+    T edge_l[Q], edge_r[Q];
+#pragma unroll
+    for (int j = 0; j < Q; ++j) {
+      lo[j] = pos[j] >= err[j] ? pos[j] - err[j] : 0;
+      hi[j] = err[j] >= n - pos[j] ? n : pos[j] + err[j];
+      b[j] = lo[j];
+      len[j] = live[j] ? hi[j] - lo[j] : 0;
+      // the confirmation probes do not depend on the search: issued with its first probe
+      edge_l[j] = keys[lo[j] > 0 ? lo[j] - 1 : 0];
+      edge_r[j] = keys[hi[j] < n ? hi[j] : n - 1];
+    }
+    while (true) {
+      bool more = false;
+#pragma unroll
+      for (int j = 0; j < Q; ++j) {
+        if (len[j] > 1) {
+          u64 h = len[j] >> 1;
+          b[j] = keys[b[j] + h] < q[j] ? b[j] + h : b[j];
+          len[j] -= h;
+          more |= len[j] > 1;
+        }
+      }
+      if (!more) break;
+    }
+#pragma unroll
+    for (int j = 0; j < Q; ++j) {
+      u64 r = b[j];
+      if (len[j] == 1) r += keys[r] < q[j] ? 1 : 0;
+      bool left_ok = lo[j] == 0 || edge_l[j] < q[j];
+      bool right_ok = hi[j] == n || !(edge_r[j] < q[j]);
+      if (live[j]) {
+        if (!(left_ok && (r < hi[j] || right_ok))) {
+          ++misses;
+          r = lookup_fallback(keys, n, q[j], lo[j], hi[j], left_ok);
+        }
+        __stcs(out + base + threadIdx.x + (u64)j * LOOKUP_THREADS, r);
+      }
+    }
+  }
+  if (fallbacks) {
+    misses = __reduce_add_sync(0xffffffffu, misses);
+    if ((threadIdx.x & 31) == 0 && misses) atomicAdd((unsigned long long*)fallbacks, (unsigned long long)misses);
+  }
+}
+
+template <class T, int TOP, int LEAF>
+void launch_lookup(const Launch& L, const TopModel& top, const void* recs, u64 N, const T* keys, u64 n, const T* q,
+                   u64 nq, u64* out, u64* out_err, u64* fallbacks, bool lower_bound) {
+  const u64 tile = (u64)LOOKUP_THREADS * LOOKUP_Q;
+  u64 blocks = (nq + tile - 1) / tile;
+  const u64 cap = (u64)L.num_sms * LOOKUP_MAX_BLOCKS_PER_SM;
+  if (blocks > cap) blocks = cap;
+  k_lookup<T, TOP, LEAF><<<(unsigned)blocks, LOOKUP_THREADS, 0, L.stream>>>(
+      top, (const ulonglong2*)recs, keys, n, N, q, nq, out, out_err, fallbacks, lower_bound ? 1 : 0);
+  count_launch();
+}
+
+template <class T, int TOP>
+void lookup_leaf(const Launch& L, const TopModel& top, int leaf_kind, const void* recs, u64 N, const T* keys, u64 n,
+                 const T* q, u64 nq, u64* out, u64* out_err, u64* fallbacks, bool lb) {
+  switch (lookup_leaf_group(leaf_kind)) {
+    case M_LINEAR: launch_lookup<T, TOP, M_LINEAR>(L, top, recs, N, keys, n, q, nq, out, out_err, fallbacks, lb); break;
+    case M_CUBIC: launch_lookup<T, TOP, M_CUBIC>(L, top, recs, N, keys, n, q, nq, out, out_err, fallbacks, lb); break;
+    case M_LOGLINEAR: launch_lookup<T, TOP, M_LOGLINEAR>(L, top, recs, N, keys, n, q, nq, out, out_err, fallbacks, lb); break;
+    case M_NORMAL: launch_lookup<T, TOP, M_NORMAL>(L, top, recs, N, keys, n, q, nq, out, out_err, fallbacks, lb); break;
+    default: launch_lookup<T, TOP, M_LOGNORMAL>(L, top, recs, N, keys, n, q, nq, out, out_err, fallbacks, lb); break;
+  }
+}
+
+}  // namespace
+
+int lookup_top_group(int kind) {
+  if (kind == M_LINEAR || kind == M_ROBUST_LINEAR || kind == M_LINEAR_SPLINE) return M_LINEAR;
+  return kind >= M_LINEAR && kind <= M_HISTOGRAM ? kind : -1;
+}
+int lookup_leaf_group(int kind) {
+  if (kind == M_LINEAR || kind == M_ROBUST_LINEAR || kind == M_LINEAR_SPLINE) return M_LINEAR;
+  return kind >= M_CUBIC && kind <= M_LOGNORMAL ? kind : -1;
+}
+
+void pack_leaf_records(int leaf_kind, const double* params, const u64* errors, u64 N, void* out) {
+  const int ppm = leaf_params_per_model(leaf_kind);
+  const u64 words = lookup_record_bytes(leaf_kind) / 8;
+  u64* o = (u64*)out;
+  for (u64 j = 0; j < N; ++j, o += words) {
+    for (u64 w = 0; w < words; ++w) o[w] = 0;
+    for (int p = 0; p < ppm; ++p) memcpy(&o[p], &params[j * ppm + p], 8);
+    o[leaf_kind == M_CUBIC ? 4 : 3] = errors[j];
+  }
+}
+
+template <class T>
+void lookup_batch(const Launch& L, const TopModel& top, int leaf_kind, const void* recs, u64 N, const T* keys, u64 n,
+                  const T* q, u64 nq, u64* out, u64* out_err, u64* fallbacks, bool lb) {
+  if (nq == 0) return;
+  switch (lookup_top_group(top.kind)) {
+    case M_LINEAR: lookup_leaf<T, M_LINEAR>(L, top, leaf_kind, recs, N, keys, n, q, nq, out, out_err, fallbacks, lb); break;
+    case M_CUBIC: lookup_leaf<T, M_CUBIC>(L, top, leaf_kind, recs, N, keys, n, q, nq, out, out_err, fallbacks, lb); break;
+    case M_LOGLINEAR: lookup_leaf<T, M_LOGLINEAR>(L, top, leaf_kind, recs, N, keys, n, q, nq, out, out_err, fallbacks, lb); break;
+    case M_NORMAL: lookup_leaf<T, M_NORMAL>(L, top, leaf_kind, recs, N, keys, n, q, nq, out, out_err, fallbacks, lb); break;
+    case M_LOGNORMAL: lookup_leaf<T, M_LOGNORMAL>(L, top, leaf_kind, recs, N, keys, n, q, nq, out, out_err, fallbacks, lb); break;
+    case M_RADIX: lookup_leaf<T, M_RADIX>(L, top, leaf_kind, recs, N, keys, n, q, nq, out, out_err, fallbacks, lb); break;
+    case M_RADIX_TABLE: lookup_leaf<T, M_RADIX_TABLE>(L, top, leaf_kind, recs, N, keys, n, q, nq, out, out_err, fallbacks, lb); break;
+    case M_BRADIX: lookup_leaf<T, M_BRADIX>(L, top, leaf_kind, recs, N, keys, n, q, nq, out, out_err, fallbacks, lb); break;
+    default: lookup_leaf<T, M_HISTOGRAM>(L, top, leaf_kind, recs, N, keys, n, q, nq, out, out_err, fallbacks, lb); break;
+  }
+}
+
+#define RMI_LOOKUP_INST(T)                                                                                        \
+  template void lookup_batch<T>(const Launch&, const TopModel&, int, const void*, u64, const T*, u64, const T*, u64, \
+                                u64*, u64*, u64*, bool);
+RMI_LOOKUP_INST(u64)
+RMI_LOOKUP_INST(u32)
+RMI_LOOKUP_INST(double)
+#undef RMI_LOOKUP_INST
+
+}  // namespace rmi

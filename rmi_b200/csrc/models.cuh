@@ -101,6 +101,16 @@ template <int KIND, class T> __device__ __forceinline__ u64 top_predict(const To
   }
 }
 
+// Model::predict_to_int (models/mod.rs:735-737) = max(0, floor(p)) as u64 of a float-valued
+// model, as the leaf kernel and the lookup kernel evaluate it.  The float->int conversion with
+// round-toward-minus-infinity saturates like Rust's cast (negative -> 0, too large -> MAX); NaN
+// must be mapped to 0 by hand.
+template <int LEAF> __device__ __forceinline__ u64 leaf_predict64(const double* f, double x) {
+  double p = predict_float<LEAF>(f, x);
+  u64 v = (u64)__double2ull_rd(p);
+  return p != p ? 0ull : v;
+}
+
 // train/two_layer.rs:14-18
 __device__ __forceinline__ u64 error_between(u64 v1, u64 v2, u64 max_pred) {
   u64 p1 = v1 < max_pred ? v1 : max_pred;
