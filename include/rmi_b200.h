@@ -169,10 +169,29 @@ int rmi_train_stats_batch(const rmi_dataset* ds, const char* top_model, const ch
  *                always exact: a binary search over [pos-err, pos+err], confirmed by the keys just outside that
  *                window, and a galloping search outward when the window misses (never, for a key of the data set). */
 typedef struct rmi_index rmi_index;
+/* One knot of a `--bounded` RMI's cache-fix spline (rmi_cache_fix below): a key and its first-occurrence offset. */
+typedef struct { uint64_t key, offset; } rmi_spline_point;
 /* Upload r's top model (incl. radix table / histogram arrays) and its leaf tables, packed, to ds's device and
  * bind them to ds's keys.  r must hold the leaf tables (not RMI_FLAG_STATS_ONLY) and r->num_rmi_rows must equal
  * rmi_dataset_len(ds); ds must outlive the index.  Immutable: concurrent calls on different streams are fine. */
 int rmi_index_create(const rmi_result* r, const rmi_dataset* ds, rmi_index** out);
+/* A `--bounded` RMI (train_bounded, below): r is the RMI over the K knots of the cache-fix spline
+ * (r->num_rmi_rows == num_knots), knots are those K {key, offset} points (the _L2_PARAMETERS layout, keys strictly
+ * increasing, offsets non-decreasing and < n), ds holds the n u64 keys the spline was fitted to.  The knots are
+ * copied to the device (the caller's array need not outlive the call); ds must outlive the index.  Refused (before
+ * any device work): a non-u64 dataset, line_size 0, no knots, knots out of order or past the keys, and every case
+ * rmi_index_create refuses.  The other rmi_index_* calls take either kind of index; on a bounded one:
+ *   predict      the generated spline lookup(q, &err) (codegen.rs:410-437): (start, e) = the RMI's predict over the
+ *                knots; res = the first knot in [start-e, min(start+e, K)) whose key is not < q (that upper end if
+ *                none); res == K: pos = n-1; res == 0: pos = 0 (the generated code reads knots[-1] there);
+ *                otherwise t = (double)(q - knots[res-1].key) / (double)(knots[res].key - knots[res-1].key) (wrapping
+ *                u64 subtraction), pos = (sat_u64(fma(1-t, offset[res-1], t * offset[res])) / line_size) * line_size
+ *                (sat_u64: Rust's saturating `as u64`, NaN -> 0); err = line_size.
+ *   lower_bound  exact, as for a plain index: a search of [pos, pos + line_size] (clamped to [0, n]), confirmed by
+ *                the keys just outside it when the search ends on an edge, and the galloping fallback (counted)
+ *                when it misses — never, for a key of the data set; wrong knots cost fallbacks, not answers. */
+int rmi_index_create_bounded(const rmi_result* r, const rmi_spline_point* knots, uint64_t num_knots,
+                             uint64_t line_size, const rmi_dataset* ds, rmi_index** out);
 void rmi_index_destroy(rmi_index* idx);
 /* n queries (ds's key type) in device memory on the index's device; enqueued on cuda_stream, no host sync.
  * One kernel launch per call (n == 0: none).  d_err may be NULL. */
@@ -291,8 +310,8 @@ int rmi_shard_train(rmi_shard_build* b, rmi_shard_comm* c, uint32_t flags, rmi_r
  *     knots = rmi_cache_fix(keys);  ds = rmi_dataset_create(knot keys);  rmi_train(ds, ...)
  * — the knots' offsets are 0, 1, 2, ..., i.e. the knot keys are an ordinary sorted duplicate-free
  * data set.  host_keys: n sorted u64 keys ("Can only construct a bounded RMI on u64 data",
- * src/main.rs:285-286).  *out_points is owned by the library: release with rmi_spline_free. */
-typedef struct { uint64_t key, offset; } rmi_spline_point;
+ * src/main.rs:285-286).  *out_points (rmi_spline_point, declared with the lookups above) is owned by the library:
+ * release with rmi_spline_free. */
 int rmi_cache_fix(const uint64_t* host_keys, uint64_t n, uint64_t line_size, rmi_spline_point** out_points,
                   uint64_t* out_count);
 void rmi_spline_free(rmi_spline_point* points);

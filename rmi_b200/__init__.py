@@ -10,15 +10,16 @@ The product is the C-ABI shared library ``rmi_b200/lib/librmi_b200.so`` (CUDA, s
     rmi_lib::output_rmi / rmi_size                                      (codegen.rs:757, :375)
     RMITrainingData / load_data                                         (models/mod.rs:233, src/load.rs:132)
 
-plus RMIIndex, batched lookups (position estimates and exact lower bounds) on the GPU.
+plus RMIIndex and BoundedRMIIndex (a train_bounded build), batched lookups (position estimates and exact lower
+bounds) on the GPU.
 
 and does no arithmetic of its own.  There is no CPU fallback: if the CUDA library is missing
 or no device is present, calls raise.
 """
-from .api import (KEY_F64, KEY_U32, KEY_U64, FLAG_LEAF_COUNTS, FLAG_SHARD_ROOT_ONLY, FLAG_STATS_ONLY, FLAG_TOP_FIT_EXACT, RMIError, RMIIndex, RMIPanic,
+from .api import (BoundedRMIIndex, KEY_F64, KEY_U32, KEY_U64, FLAG_LEAF_COUNTS, FLAG_SHARD_ROOT_ONLY, FLAG_STATS_ONLY, FLAG_TOP_FIT_EXACT, RMIError, RMIIndex, RMIPanic,
                   RMITrainingData, TrainedRMI, cache_fix, find_pareto_efficient_configs, kernel_launch_count, lib_path,
                   load_data, load_library, output_rmi, rmi_size, train, train_bounded, train_for_size, train_stats_batch, version)
 
-__all__ = ["KEY_F64", "KEY_U32", "KEY_U64", "FLAG_LEAF_COUNTS", "FLAG_SHARD_ROOT_ONLY", "FLAG_STATS_ONLY", "FLAG_TOP_FIT_EXACT", "RMIError", "RMIIndex", "RMIPanic",
+__all__ = ["BoundedRMIIndex", "KEY_F64", "KEY_U32", "KEY_U64", "FLAG_LEAF_COUNTS", "FLAG_SHARD_ROOT_ONLY", "FLAG_STATS_ONLY", "FLAG_TOP_FIT_EXACT", "RMIError", "RMIIndex", "RMIPanic",
            "RMITrainingData", "TrainedRMI", "cache_fix", "find_pareto_efficient_configs", "kernel_launch_count", "lib_path",
            "load_data", "load_library", "output_rmi", "rmi_size", "train", "train_bounded", "train_for_size", "train_stats_batch", "version"]

@@ -88,6 +88,8 @@ def load_library():
         L.rmi_find_pareto_efficient_configs.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_uint64, C.c_uint32,
                                                         C.POINTER(_ConfigStats), C.c_uint64, C.POINTER(C.c_uint64)]
         L.rmi_index_create.argtypes = [C.POINTER(_Result), C.c_void_p, C.POINTER(C.c_void_p)]
+        L.rmi_index_create_bounded.argtypes = [C.POINTER(_Result), C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p,
+                                               C.POINTER(C.c_void_p)]
         L.rmi_index_destroy.argtypes = [C.c_void_p]
         L.rmi_index_predict.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]
         L.rmi_index_lower_bound.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -460,3 +462,23 @@ class RMIIndex:
             self.close()
         except Exception:
             pass
+
+
+class BoundedRMIIndex(RMIIndex):
+    """A ``--bounded`` RMI bound to its keys: ``trained`` and ``knots`` are the pair ``train_bounded`` returns (the
+    RMI over the cache-fix spline's knots and the ``(K, 2)`` uint64 knot array), ``data`` the uint64 keys the spline
+    was fitted to.  ``predict`` returns the generated spline ``lookup(key, &err)`` (position rounded down to its
+    line, ``err = line_size``); ``lower_bound`` is exact and, for a key of the data set, searches only that key's
+    line.  Everything else is as for ``RMIIndex``; the knots are copied to the device."""
+
+    def __init__(self, trained: TrainedRMI, knots: np.ndarray, line_size: int, data: RMITrainingData):
+        self._h = C.c_void_p()
+        self.data = data
+        self.key_type = data.key_type
+        self._trained = trained
+        self.line_size = int(line_size)
+        k = np.ascontiguousarray(knots, dtype=np.uint64)
+        if k.ndim != 2 or k.shape[1] != 2:
+            raise ValueError(f"knots must be a (K, 2) array of (key, offset), got shape {k.shape}")
+        _check(load_library().rmi_index_create_bounded(_result_ptr(trained), k.ctypes.data_as(C.c_void_p), k.shape[0],
+                                                       self.line_size, data._h, C.byref(self._h)))

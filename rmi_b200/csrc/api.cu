@@ -465,6 +465,10 @@ struct rmi_index {
   u64* d_pivots = nullptr;
   u64* d_radix_index = nullptr;
   int num_sms = 0;
+  // a bounded (cache-fix) index: the RMI above runs over K knots; null / 0 for a plain index
+  void* d_knots = nullptr;   // K x rmi_spline_point
+  uint64_t K = 0;
+  uint64_t line_size = 0;
 };
 
 namespace {
@@ -473,6 +477,7 @@ void index_free_device(rmi_index* idx) {
   cudaFree(idx->d_t32);
   cudaFree(idx->d_pivots);
   cudaFree(idx->d_radix_index);
+  cudaFree(idx->d_knots);
 }
 
 int index_check_call(const rmi_index* idx, const void* d_queries, uint64_t n, const void* d_out, const char* fn) {
@@ -487,6 +492,13 @@ int index_launch(const rmi_index* idx, const void* d_queries, uint64_t n, uint64
   const rmi_dataset* ds = idx->ds;
   CUDA_TRY(cudaSetDevice(ds->device));
   Launch L{(cudaStream_t)cuda_stream, idx->num_sms};
+  if (idx->d_knots) {
+    lookup_bounded_batch(L, idx->top, idx->leaf_kind, idx->d_records, idx->N, idx->d_knots, idx->K, idx->line_size,
+                         (const u64*)ds->d_keys, ds->n, (const u64*)d_queries, n, (u64*)d_out, (u64*)d_err,
+                         (u64*)d_fallbacks, lower_bound);
+    CUDA_TRY(cudaGetLastError());
+    return RMI_OK;
+  }
   switch (ds->key_type) {
     case RMI_KEY_U64:
       lookup_batch<u64>(L, idx->top, idx->leaf_kind, idx->d_records, idx->N, (const u64*)ds->d_keys, ds->n,
@@ -505,29 +517,32 @@ int index_launch(const rmi_index* idx, const void* d_queries, uint64_t n, uint64
   CUDA_TRY(cudaGetLastError());
   return RMI_OK;
 }
-}  // namespace
-
-extern "C" {
-
-int rmi_index_create(const rmi_result* r, const rmi_dataset* ds, rmi_index** out) {
-  if (!r || !ds || !out) return fail(RMI_ERR_INVALID, "rmi_index_create: null argument");
+// The checks and the upload both kinds of index share: r's tables against ds, or against the knots of a bounded index
+// (num_knots > 0: r must have been trained on them).  Messages name `fn`.
+int index_check_tables(const rmi_result* r, const rmi_dataset* ds, uint64_t num_knots, const std::string& fn) {
   if (!r->l1_params || !r->l1_errors)
-    return fail(RMI_ERR_INVALID, "rmi_index_create: the result holds no leaf tables (trained with RMI_FLAG_STATS_ONLY)");
-  if (r->num_rmi_rows != ds->n)
-    return fail(RMI_ERR_INVALID, "rmi_index_create: the result was trained on " + std::to_string(r->num_rmi_rows) +
-                                     " keys, the dataset holds " + std::to_string(ds->n));
-  if (ds->n == 0 || r->branching_factor == 0) return fail(RMI_ERR_INVALID, "rmi_index_create: empty index");
+    return fail(RMI_ERR_INVALID, fn + ": the result holds no leaf tables (trained with RMI_FLAG_STATS_ONLY)");
+  const uint64_t rows = num_knots ? num_knots : ds->n;
+  if (r->num_rmi_rows != rows)
+    return fail(RMI_ERR_INVALID, fn + ": the result was trained on " + std::to_string(r->num_rmi_rows) + " keys, " +
+                                     (num_knots ? "the spline has " : "the dataset holds ") + std::to_string(rows));
+  if (ds->n == 0 || r->branching_factor == 0) return fail(RMI_ERR_INVALID, fn + ": empty index");
   if (lookup_top_group((int)r->l0_model_id) < 0 || lookup_leaf_group((int)r->l1_model_id) < 0)
-    return fail(RMI_ERR_UNSUPPORTED, "rmi_index_create: unsupported model id (top " + std::to_string(r->l0_model_id) +
+    return fail(RMI_ERR_UNSUPPORTED, fn + ": unsupported model id (top " + std::to_string(r->l0_model_id) +
                                          ", leaf " + std::to_string(r->l1_model_id) + ")");
   if (r->l1_params_per_model != (uint32_t)leaf_params_per_model((int)r->l1_model_id))
-    return fail(RMI_ERR_INVALID, "rmi_index_create: wrong number of leaf parameters");
+    return fail(RMI_ERR_INVALID, fn + ": wrong number of leaf parameters");
   if (r->l0_model_id == M_RADIX_TABLE &&
       (!r->l0_table32 || r->l0_table_bits > 32 || r->l0_table32_len != ((uint64_t)1 << r->l0_table_bits)))
-    return fail(RMI_ERR_INVALID, "rmi_index_create: radix table missing or of the wrong size");
+    return fail(RMI_ERR_INVALID, fn + ": radix table missing or of the wrong size");
   if (r->l0_model_id == M_HISTOGRAM && (!r->l0_array2 || !r->l0_array2_len))
-    return fail(RMI_ERR_INVALID, "rmi_index_create: histogram pivots missing");
+    return fail(RMI_ERR_INVALID, fn + ": histogram pivots missing");
+  return RMI_OK;
+}
 
+// Builds the index on ds's device; knots (K of them, may be null) make it a bounded one.
+int index_upload(const rmi_result* r, const rmi_dataset* ds, const rmi_spline_point* knots, uint64_t K,
+                 uint64_t line_size, const std::string& fn, rmi_index** out) {
   CUDA_TRY(cudaSetDevice(ds->device));
   DeviceInfo di;
   if (int rc = device_info(ds->device, &di)) return rc;
@@ -563,13 +578,49 @@ int rmi_index_create(const rmi_result* r, const rmi_dataset* ds, rmi_index** out
     t.radix_index = idx->d_radix_index;
     t.npivots = r->l0_array2_len;
   }
+  if (e == cudaSuccess && knots) {
+    e = cudaMalloc(&idx->d_knots, sizeof(rmi_spline_point) * K);
+    if (e == cudaSuccess) e = cudaMemcpy(idx->d_knots, knots, sizeof(rmi_spline_point) * K, cudaMemcpyHostToDevice);
+    idx->K = K;
+    idx->line_size = line_size;
+  }
   if (e != cudaSuccess) {
     index_free_device(idx);
     delete idx;
-    return fail(RMI_ERR_CUDA, std::string("rmi_index_create: ") + cudaGetErrorString(e));
+    return fail(RMI_ERR_CUDA, fn + ": " + cudaGetErrorString(e));
   }
   *out = idx;
   return RMI_OK;
+}
+
+
+}  // namespace
+
+extern "C" {
+
+int rmi_index_create(const rmi_result* r, const rmi_dataset* ds, rmi_index** out) {
+  if (!r || !ds || !out) return fail(RMI_ERR_INVALID, "rmi_index_create: null argument");
+  if (int rc = index_check_tables(r, ds, 0, "rmi_index_create")) return rc;
+  return index_upload(r, ds, nullptr, 0, 0, "rmi_index_create", out);
+}
+
+int rmi_index_create_bounded(const rmi_result* r, const rmi_spline_point* knots, uint64_t num_knots,
+                             uint64_t line_size, const rmi_dataset* ds, rmi_index** out) {
+  const std::string fn = "rmi_index_create_bounded";
+  if (!r || !knots || !ds || !out) return fail(RMI_ERR_INVALID, fn + ": null argument");
+  if (ds->key_type != RMI_KEY_U64) return fail(RMI_ERR_INVALID, fn + ": Can only construct a bounded RMI on u64 data");
+  if (line_size == 0) return fail(RMI_ERR_INVALID, fn + ": line size 0");
+  if (num_knots == 0) return fail(RMI_ERR_INVALID, fn + ": no spline knots");
+  if (int rc = index_check_tables(r, ds, num_knots, fn)) return rc;
+  for (uint64_t i = 0; i < num_knots; ++i) {
+    if (knots[i].offset >= ds->n)
+      return fail(RMI_ERR_INVALID, fn + ": knot " + std::to_string(i) + " has offset " + std::to_string(knots[i].offset) +
+                                       ", the dataset holds " + std::to_string(ds->n) + " keys");
+    if (i && !(knots[i - 1].key < knots[i].key && knots[i - 1].offset <= knots[i].offset))
+      return fail(RMI_ERR_INVALID, fn + ": knots " + std::to_string(i - 1) + " and " + std::to_string(i) +
+                                       " are out of order (keys must increase strictly, offsets must not decrease)");
+  }
+  return index_upload(r, ds, knots, num_knots, line_size, fn, out);
 }
 
 void rmi_index_destroy(rmi_index* idx) {

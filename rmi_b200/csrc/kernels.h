@@ -157,6 +157,12 @@ void pack_leaf_records(int leaf_kind, const double* params, const u64* errors, u
 template <class T>
 void lookup_batch(const Launch& L, const TopModel& top, int leaf_kind, const void* d_records, u64 N, const T* keys, u64 n,
                   const T* d_queries, u64 nq, u64* d_out, u64* d_out_err, u64* d_fallbacks, bool lower_bound);
+// The same for a bounded (cache-fix) index over u64 keys: the RMI (d_records, N leaves) predicts one of the K knots
+// at d_knots (K x {key, offset}, 16 bytes each), the spline step gives the key's line of line_size keys, and
+// lower_bound searches that line.  out_err receives line_size.
+void lookup_bounded_batch(const Launch& L, const TopModel& top, int leaf_kind, const void* d_records, u64 N,
+                          const void* d_knots, u64 K, u64 line_size, const u64* keys, u64 n, const u64* d_queries,
+                          u64 nq, u64* d_out, u64* d_out_err, u64* d_fallbacks, bool lower_bound);
 
 // ---- range-partitioned build phases (kernels_shard.cu) ---------------------------------------
 size_t shard_scratch_bytes();

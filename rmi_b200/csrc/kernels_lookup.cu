@@ -205,7 +205,140 @@ void lookup_leaf(const Launch& L, const TopModel& top, int leaf_kind, const void
   }
 }
 
+// ---- bounded (`--bounded`, cache-fix) index ------------------------------------------------------------------
+// The RMI runs over the K spline knots.  predict: (start, e) as above with K rows; res = the first knot in
+// [start-e, start+e) ∩ [0, K) whose key is not < q; the spline between knots res-1 and res gives the key's
+// position, rounded down to its line (codegen.rs:410-437).  lower_bound: the answer lies in [pos, pos + line]
+// for every key of the data set (the spline's construction), so the kernel searches that window only.
+//
+// Windows of up to BOUNDED_COUNT_MAX keys are searched by loading every key independently and counting those
+// below q (no dependent probe chain); longer ones by the branchless binary search.  The keys just outside the
+// window are read only when the search ends on that edge, so a present key touches its own line alone unless its
+// lower bound is the line's first index.
+constexpr u64 BOUNDED_COUNT_MAX = 16;
+
+template <int TOP, int LEAF>
+__global__ void __launch_bounds__(LOOKUP_THREADS)
+k_lookup_bounded(const __grid_constant__ TopModel top, const ulonglong2* __restrict__ recs, u64 N,
+                 const ulonglong2* __restrict__ knots, u64 K, u64 line, const u64* __restrict__ keys, u64 n,
+                 const u64* __restrict__ qs, u64 nq, u64* __restrict__ out, u64* __restrict__ out_err, u64* fallbacks,
+                 int lower_bound) {
+  using R = Rec<LEAF>;
+  unsigned misses = 0;
+  for (u64 i = (u64)blockIdx.x * LOOKUP_THREADS + threadIdx.x; i < nq; i += (u64)gridDim.x * LOOKUP_THREADS) {
+    const u64 q = __ldcs(qs + i);
+    u64 t = top_predict<TOP>(top, q);
+    t = t < N - 1 ? t : N - 1;
+    ulonglong2 v[R::LOADS];
+#pragma unroll
+    for (int k = 0; k < R::LOADS; ++k) v[k] = __ldg(recs + t * R::VECS + k);
+    double f[4];
+    u64 e;
+    R::unpack(v, f, e);
+    u64 start = leaf_predict64<LEAF>(f, Key<u64>::as_float(q));
+    start = start < K - 1 ? start : K - 1;
+    // knot window [lower, upper); upper saturates where start + e would pass K
+    const u64 lower = e > start ? 0 : start - e;
+    const u64 upper = e >= K - start ? K : start + e;
+    u64 b = lower, len = upper - lower;
+    while (len > 1) {
+      const u64 h = len >> 1;
+      b = knots[b + h].x < q ? b + h : b;
+      len -= h;
+    }
+    const u64 res = len == 1 && knots[b].x < q ? b + 1 : b;
+    u64 pos;
+    if (res == K) {
+      pos = n - 1;
+    } else if (res == 0) {
+      pos = 0;
+    } else {
+      const ulonglong2 p0 = knots[res - 1], p1 = knots[res];
+      const double tt = __ddiv_rn(__ull2double_rn(q - p0.x), __ull2double_rn(p1.x - p0.x));
+      const double y = __fma_rn(__dsub_rn(1.0, tt), __ull2double_rn(p0.y), __dmul_rn(tt, __ull2double_rn(p1.y)));
+      pos = f64_to_u64_sat(y) / line * line;
+    }
+    if (!lower_bound) {
+      __stcs(out + i, pos);
+      if (out_err) __stcs(out_err + i, line);
+      continue;
+    }
+    const u64 lo = pos < n ? pos : n;
+    const u64 hi = line >= n - lo ? n : lo + line;
+    u64 r = lo;
+    if (line <= BOUNDED_COUNT_MAX) {
+#pragma unroll
+      for (u64 j = 0; j < BOUNDED_COUNT_MAX; ++j)
+        if (lo + j < hi) r += keys[lo + j] < q ? 1 : 0;
+    } else {
+      u64 kb = lo, klen = hi - lo;
+      while (klen > 1) {
+        const u64 h = klen >> 1;
+        kb = keys[kb + h] < q ? kb + h : kb;
+        klen -= h;
+      }
+      r = klen == 1 && keys[kb] < q ? kb + 1 : kb;
+    }
+    const bool left_ok = r > lo || lo == 0 || keys[lo - 1] < q;
+    const bool right_ok = r < hi || hi == n || !(keys[hi] < q);
+    if (!(left_ok && right_ok)) {
+      ++misses;
+      r = lookup_fallback(keys, n, q, lo, hi, left_ok);
+    }
+    __stcs(out + i, r);
+  }
+  if (fallbacks) {
+    misses = __reduce_add_sync(0xffffffffu, misses);
+    if ((threadIdx.x & 31) == 0 && misses) atomicAdd((unsigned long long*)fallbacks, (unsigned long long)misses);
+  }
+}
+
+template <int TOP, int LEAF>
+void launch_lookup_bounded(const Launch& L, const TopModel& top, const void* recs, u64 N, const void* knots, u64 K,
+                           u64 line, const u64* keys, u64 n, const u64* q, u64 nq, u64* out, u64* out_err,
+                           u64* fallbacks, bool lower_bound) {
+  u64 blocks = (nq + LOOKUP_THREADS - 1) / LOOKUP_THREADS;
+  const u64 cap = (u64)L.num_sms * LOOKUP_MAX_BLOCKS_PER_SM;
+  if (blocks > cap) blocks = cap;
+  k_lookup_bounded<TOP, LEAF><<<(unsigned)blocks, LOOKUP_THREADS, 0, L.stream>>>(
+      top, (const ulonglong2*)recs, N, (const ulonglong2*)knots, K, line, keys, n, q, nq, out, out_err, fallbacks,
+      lower_bound ? 1 : 0);
+  count_launch();
+}
+
+#define RMI_BOUNDED_ARGS recs, N, knots, K, line, keys, n, q, nq, out, out_err, fallbacks, lb
+template <int TOP>
+void lookup_bounded_leaf(const Launch& L, const TopModel& top, int leaf_kind, const void* recs, u64 N,
+                         const void* knots, u64 K, u64 line, const u64* keys, u64 n, const u64* q, u64 nq, u64* out,
+                         u64* out_err, u64* fallbacks, bool lb) {
+  switch (lookup_leaf_group(leaf_kind)) {
+    case M_LINEAR: launch_lookup_bounded<TOP, M_LINEAR>(L, top, RMI_BOUNDED_ARGS); break;
+    case M_CUBIC: launch_lookup_bounded<TOP, M_CUBIC>(L, top, RMI_BOUNDED_ARGS); break;
+    case M_LOGLINEAR: launch_lookup_bounded<TOP, M_LOGLINEAR>(L, top, RMI_BOUNDED_ARGS); break;
+    case M_NORMAL: launch_lookup_bounded<TOP, M_NORMAL>(L, top, RMI_BOUNDED_ARGS); break;
+    default: launch_lookup_bounded<TOP, M_LOGNORMAL>(L, top, RMI_BOUNDED_ARGS); break;
+  }
+}
+
 }  // namespace
+
+void lookup_bounded_batch(const Launch& L, const TopModel& top, int leaf_kind, const void* recs, u64 N,
+                          const void* knots, u64 K, u64 line, const u64* keys, u64 n, const u64* q, u64 nq, u64* out,
+                          u64* out_err, u64* fallbacks, bool lb) {
+  if (nq == 0) return;
+  switch (lookup_top_group(top.kind)) {
+    case M_LINEAR: lookup_bounded_leaf<M_LINEAR>(L, top, leaf_kind, RMI_BOUNDED_ARGS); break;
+    case M_CUBIC: lookup_bounded_leaf<M_CUBIC>(L, top, leaf_kind, RMI_BOUNDED_ARGS); break;
+    case M_LOGLINEAR: lookup_bounded_leaf<M_LOGLINEAR>(L, top, leaf_kind, RMI_BOUNDED_ARGS); break;
+    case M_NORMAL: lookup_bounded_leaf<M_NORMAL>(L, top, leaf_kind, RMI_BOUNDED_ARGS); break;
+    case M_LOGNORMAL: lookup_bounded_leaf<M_LOGNORMAL>(L, top, leaf_kind, RMI_BOUNDED_ARGS); break;
+    case M_RADIX: lookup_bounded_leaf<M_RADIX>(L, top, leaf_kind, RMI_BOUNDED_ARGS); break;
+    case M_RADIX_TABLE: lookup_bounded_leaf<M_RADIX_TABLE>(L, top, leaf_kind, RMI_BOUNDED_ARGS); break;
+    case M_BRADIX: lookup_bounded_leaf<M_BRADIX>(L, top, leaf_kind, RMI_BOUNDED_ARGS); break;
+    default: lookup_bounded_leaf<M_HISTOGRAM>(L, top, leaf_kind, RMI_BOUNDED_ARGS); break;
+  }
+}
+#undef RMI_BOUNDED_ARGS
 
 int lookup_top_group(int kind) {
   if (kind == M_LINEAR || kind == M_ROBUST_LINEAR || kind == M_LINEAR_SPLINE) return M_LINEAR;
