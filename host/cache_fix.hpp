@@ -2,10 +2,13 @@
 // key -> offset function whose prediction always lands in the correct cache line
 // (line = offset / line_size).  CPU-side restatement of rmi_lib/src/cache_fix.rs
 // (Spline :5-44, SplineFit :46-104, cache_fix :106-150) and of train_bounded
-// (rmi_lib/src/train/mod.rs:156-184).  The fit is a greedy, strictly serial scan (every
-// accepted point is re-checked against the whole current segment), so — as SURVEY.md 8(f)4
-// says — it stays on the host; its output, the spline's knots, is a sorted duplicate-free
-// key array that then goes through the ordinary GPU build (rmi_train) as the data set.
+// (rmi_lib/src/train/mod.rs:156-184).  The fit is the reference's greedy scan on one host core
+// (every accepted point is re-checked against the whole current segment): rmi_cache_fix's CPU
+// path, and the reference the device scan (kernels_cachefix.cu, rmi_cache_fix_device) is
+// tested against knot for knot.  The device scan rests on a property of this code: the knot
+// after a knot depends on that knot alone (DESIGN.md section 12).  The output, the spline's
+// knots, is a sorted duplicate-free key array that then goes through the ordinary GPU build
+// (rmi_train) as the data set.
 #pragma once
 #include <cmath>
 #include <cstdint>

@@ -7,9 +7,9 @@
 // (--optimize, --max-size), --devices <a,b,...>: the key set is replicated to every listed GPU
 // (device-to-device copies) and the independent configurations are spread over them.
 // The build itself is librmi_b200.so (CUDA); this binary only loads the data set into HBM,
-// calls rmi_train and writes the artefacts (codegen.hpp).  `--bounded` runs the reference's
-// serial cache-fix scan on the host (cache_fix.hpp) and then builds the RMI over the spline's
-// knots on the GPU like any other data set.  There is no CPU training path: without a usable
+// calls rmi_train and writes the artefacts (codegen.hpp).  `--bounded` fits the reference's
+// cache-fix spline on the GPU from the loaded keys (rmi_cache_fix_device) and then builds the RMI
+// over the spline's knots on the GPU like any other data set.  There is no CPU training path: without a usable
 // GPU every build fails with the CUDA error text.
 #include <cerrno>
 #include <chrono>
@@ -216,8 +216,8 @@ int main(int argc, char** argv) {
       bounded_build_ns = (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t0).count();
       sized = true;
     } else if (a.has("--bounded")) {
-      // train_bounded (train/mod.rs:156-184): the serial cache-fix scan on the host, then the
-      // ordinary GPU build with the spline's knots as the data set (their offsets are 0, 1, 2, ...)
+      // train_bounded (train/mod.rs:156-184): the cache-fix spline fitted on the device from the keys already
+      // loaded, then the ordinary GPU build with the spline's knots as the data set (their offsets are 0, 1, 2, ...)
       if (a.pos.size() < 4) die("called `Option::unwrap()` on a `None` value (models and branching factor are required)");
       char* endp = nullptr;
       const std::string ls = a.opt["--bounded"];
@@ -225,16 +225,12 @@ int main(int argc, char** argv) {
       if (ls.empty() || *endp) die("Line size must be a positive integer.");
       if (file_kt != RMI_KEY_U64) die("Can only construct a bounded RMI on u64 data.");
       auto t0 = std::chrono::steady_clock::now();
-      std::vector<uint64_t> host_keys(num_rows);
-      {
-        std::ifstream in(fp, std::ios::binary);
-        uint64_t cnt = 0;
-        in.read(reinterpret_cast<char*>(&cnt), 8);
-        in.read(reinterpret_cast<char*>(host_keys.data()), (std::streamsize)(num_rows * 8));
-        if (!in || cnt != num_rows) die("Unable to read the data file at " + fp);
-      }
-      try { spline = cache_fix(host_keys.data(), num_rows, cf.line_size); } catch (std::exception& e) { die(e.what()); }
-      host_keys.clear(); host_keys.shrink_to_fit();
+      rmi_spline_point* pts = nullptr;
+      uint64_t num_pts = 0;
+      if (rmi_cache_fix_device(ds, cf.line_size, &pts, &num_pts, nullptr) != RMI_OK) die(rmi_last_error());
+      spline.reserve(num_pts);
+      for (uint64_t i = 0; i < num_pts; ++i) spline.emplace_back(pts[i].key, pts[i].offset);
+      rmi_spline_free(pts);
       std::fprintf(stderr, "Bounded spline compressed data to %.0f%% of original (%zu points, constructed from %llu points).\n",
                    std::round((double)spline.size() / (double)num_rows * 100.0), spline.size(), (unsigned long long)num_rows);
       std::vector<uint64_t> knot_keys(spline.size());

@@ -305,15 +305,34 @@ int rmi_shard_train(rmi_shard_build* b, rmi_shard_comm* c, uint32_t flags, rmi_r
 
 /* ---- `--bounded` support: rmi_lib::cache_fix (reference rmi_lib/src/cache_fix.rs:106-150) ----------
  * The error-bounded spline over key -> first-occurrence offset whose interpolation always lands in
- * the key's line (offset / line_size).  A greedy, strictly serial HOST scan (as in the reference;
- * SURVEY.md section 8(f)4): no device work.  train_bounded (train/mod.rs:156-184) is then
- *     knots = rmi_cache_fix(keys);  ds = rmi_dataset_create(knot keys);  rmi_train(ds, ...)
+ * the key's line (offset / line_size).  train_bounded (train/mod.rs:156-184) is then
+ *     knots = rmi_cache_fix_device(ds);  kds = rmi_dataset_create(knot keys);  rmi_train(kds, ...)
  * — the knots' offsets are 0, 1, 2, ..., i.e. the knot keys are an ordinary sorted duplicate-free
- * data set.  host_keys: n sorted u64 keys ("Can only construct a bounded RMI on u64 data",
- * src/main.rs:285-286).  *out_points (rmi_spline_point, declared with the lookups above) is owned by the library:
- * release with rmi_spline_free. */
+ * data set.  Two forms with the same output, knot for knot:
+ *   rmi_cache_fix         the reference's greedy scan on one host core (no device work), over n sorted u64
+ *                         host_keys;
+ *   rmi_cache_fix_device  the same spline fitted on the device from ds's resident keys, with no host copy of the
+ *                         keys (DESIGN.md section 12 gives the method and its speed).
+ * *out_points (rmi_spline_point, declared with the lookups above) is owned by the library: release with
+ * rmi_spline_free.  Both report the reference's panics as RMI_ERR_PANIC with its messages (fewer keys than the
+ * line size, line size 0, a first key of 0). */
 int rmi_cache_fix(const uint64_t* host_keys, uint64_t n, uint64_t line_size, rmi_spline_point** out_points,
                   uint64_t* out_count);
+/* What a device scan did (rmi_cache_fix_device's optional last argument). */
+typedef struct {
+  uint64_t chunk_keys;        /* key indices per speculation chunk */
+  uint64_t chunks;            /* ceil(n / chunk_keys) */
+  uint64_t points;            /* points in the spline's input stream (distinct keys and their key - 1 points) */
+  uint64_t stitch_segments;   /* segments the stitch walked to join neighbouring chunks' chains */
+  uint64_t fallback_points;   /* points the sequential fallback walked where speculation did not join */
+  uint64_t evaluations;       /* spline predictions, all passes */
+} rmi_cache_fix_stats;
+/* ds: a u64 dataset ("Can only construct a bounded RMI on u64 data", src/main.rs:285-286; other key types and null
+ * arguments are RMI_ERR_INVALID, before any device work).  Runs on the calling thread's CUDA stream (as rmi_train),
+ * so concurrent calls from several host threads are safe; its device scratch is O(n / chunk_keys) words plus the
+ * knots, from the stream-ordered pool, released before return.  Five kernel launches.  stats may be NULL. */
+int rmi_cache_fix_device(const rmi_dataset* ds, uint64_t line_size, rmi_spline_point** out_points,
+                         uint64_t* out_count, rmi_cache_fix_stats* stats);
 void rmi_spline_free(rmi_spline_point* points);
 
 /* ---- The rest of rmi_lib's public surface (host-side code, no device work of their own) ---------

@@ -11,7 +11,7 @@ The product is the C-ABI shared library ``rmi_b200/lib/librmi_b200.so`` (CUDA, s
     RMITrainingData / load_data                                         (models/mod.rs:233, src/load.rs:132)
 
 plus RMIIndex and BoundedRMIIndex (a train_bounded build), batched lookups (position estimates and exact lower
-bounds) on the GPU.
+bounds) on the GPU.  cache_fix / train_bounded on an RMITrainingData fit the cache-fix spline on the GPU.
 
 and does no arithmetic of its own.  There is no CPU fallback: if the CUDA library is missing
 or no device is present, calls raise.

@@ -44,6 +44,12 @@ class _Result(C.Structure):
     ]
 
 
+class _CacheFixStats(C.Structure):
+    """struct rmi_cache_fix_stats (include/rmi_b200.h): what a device cache-fix scan did."""
+    _fields_ = [("chunk_keys", C.c_uint64), ("chunks", C.c_uint64), ("points", C.c_uint64),
+                ("stitch_segments", C.c_uint64), ("fallback_points", C.c_uint64), ("evaluations", C.c_uint64)]
+
+
 class _ConfigStats(C.Structure):
     """struct rmi_config_stats (optimizer.rs:153-160 RMIStatistics)."""
     _fields_ = [("models", C.c_char * 64), ("branching_factor", C.c_uint64), ("average_log2_error", C.c_double),
@@ -80,6 +86,8 @@ def load_library():
                                          C.POINTER(C.POINTER(_Result))]
         L.rmi_result_free.argtypes = [C.POINTER(_Result)]
         L.rmi_cache_fix.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
+        L.rmi_cache_fix_device.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64),
+                                           C.POINTER(_CacheFixStats)]
         L.rmi_spline_free.argtypes = [C.c_void_p]
         L.rmi_model_size.restype = C.c_uint64
         L.rmi_model_size.argtypes = [C.POINTER(_Result), C.c_int, C.c_uint64]
@@ -183,36 +191,53 @@ class RMITrainingData:
             pass
 
 
-def cache_fix(keys: np.ndarray, line_size: int) -> np.ndarray:
-    """rmi_lib::cache_fix (cache_fix.rs:106-150): the error-bounded spline over key -> offset whose
-    interpolation always lands in the key's line.  A serial HOST scan (no GPU).  Returns the knots as a
-    (K, 2) uint64 array of (key, offset)."""
-    keys = np.ascontiguousarray(keys)
-    if keys.dtype != np.uint64:
-        raise RMIPanic("Can only construct a bounded RMI on u64 data.")
-    L = load_library()
-    pts, cnt = C.c_void_p(), C.c_uint64(0)
-    _check(L.rmi_cache_fix(keys.ctypes.data_as(C.c_void_p), keys.size, int(line_size), C.byref(pts), C.byref(cnt)))
+def _take_knots(L, pts, cnt) -> np.ndarray:
+    """Copy the library-owned knot array into a (K, 2) uint64 numpy array and release it."""
     try:
         n = int(cnt.value)
-        out = np.frombuffer((C.c_uint64 * (2 * n)).from_address(pts.value), dtype=np.uint64).reshape(n, 2).copy() if n else \
-            np.zeros((0, 2), dtype=np.uint64)
+        return np.frombuffer((C.c_uint64 * (2 * n)).from_address(pts.value), dtype=np.uint64).reshape(n, 2).copy() if n \
+            else np.zeros((0, 2), dtype=np.uint64)
     finally:
         L.rmi_spline_free(pts)
-    return out
 
 
-def train_bounded(keys: np.ndarray, model_spec: str, branch_factor: int, line_size: int, device: int = 0, flags: int = 0):
-    """rmi_lib::train_bounded (train/mod.rs:156-184): cache_fix on the host, then the two-layer RMI over the
-    spline's knots on the GPU.  Returns (TrainedRMI with num_data_rows = len(keys), knots) — the pair the
-    reference keeps in TrainedRMI.cache_fix."""
-    knots = cache_fix(keys, line_size)
+def cache_fix(data, line_size: int, with_stats: bool = False):
+    """rmi_lib::cache_fix (cache_fix.rs:106-150): the error-bounded spline over key -> offset whose
+    interpolation always lands in the key's line.  Returns the knots as a (K, 2) uint64 array of (key, offset).
+
+    ``data`` is a numpy array (the reference's serial scan on one host core, no GPU) or an RMITrainingData (the
+    same knots, fitted on the data's GPU from its resident keys).  with_stats=True returns ``(knots, stats)``:
+    for the device scan a dict of rmi_cache_fix_stats (chunk_keys, chunks, points, stitch_segments,
+    fallback_points, evaluations); None for the host scan."""
+    L = load_library()
+    pts, cnt = C.c_void_p(), C.c_uint64(0)
+    if isinstance(data, RMITrainingData):
+        st = _CacheFixStats()
+        _check(L.rmi_cache_fix_device(data._h, int(line_size), C.byref(pts), C.byref(cnt), C.byref(st)))
+        knots = _take_knots(L, pts, cnt)
+        stats = {name: int(getattr(st, name)) for name, _ in _CacheFixStats._fields_}
+        return (knots, stats) if with_stats else knots
+    keys = np.ascontiguousarray(data)
+    if keys.dtype != np.uint64:
+        raise RMIPanic("Can only construct a bounded RMI on u64 data.")
+    _check(L.rmi_cache_fix(keys.ctypes.data_as(C.c_void_p), keys.size, int(line_size), C.byref(pts), C.byref(cnt)))
+    knots = _take_knots(L, pts, cnt)
+    return (knots, None) if with_stats else knots
+
+
+def train_bounded(data, model_spec: str, branch_factor: int, line_size: int, device: int = 0, flags: int = 0):
+    """rmi_lib::train_bounded (train/mod.rs:156-184): cache_fix, then the two-layer RMI over the spline's knots
+    on the GPU.  ``data``: a numpy array of uint64 keys (the cache-fix scan runs on the host) or an
+    RMITrainingData (it runs on the data's GPU).  ``device`` is the GPU that trains the RMI over the knots.  Returns (TrainedRMI with
+    num_data_rows = the number of keys, knots) — the pair the reference keeps in TrainedRMI.cache_fix."""
+    knots = cache_fix(data, line_size)
+    num_rows = len(data) if isinstance(data, RMITrainingData) else int(np.asarray(data).size)
     ds = RMITrainingData(np.ascontiguousarray(knots[:, 0]), device=device)
     try:
         rmi = train(ds, model_spec, branch_factor, flags)
     finally:
         ds.close()
-    rmi.num_data_rows = int(np.asarray(keys).size)
+    rmi.num_data_rows = num_rows
     return rmi, knots
 
 

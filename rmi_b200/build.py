@@ -12,7 +12,7 @@ LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "librmi_b200.so")
 OBJ_DIR = os.path.join(HERE, "build")
 
-SOURCES = ["kernels_top.cu", "kernels_leaf.cu", "kernels_shard.cu", "kernels_lookup.cu", "api.cu"]
+SOURCES = ["kernels_top.cu", "kernels_leaf.cu", "kernels_shard.cu", "kernels_lookup.cu", "kernels_cachefix.cu", "api.cu"]
 HEADERS = ["rust_math.cuh", "models.cuh", "device_util.cuh", "spline.cuh", "kernels.h",
            os.path.join("..", "..", "include", "rmi_b200.h"), os.path.join("..", "..", "host", "cache_fix.hpp"), os.path.join("..", "..", "host", "codegen.hpp"),
            os.path.join("..", "..", "host", "optimizer.hpp")]

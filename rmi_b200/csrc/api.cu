@@ -1304,6 +1304,93 @@ int rmi_train_with_top(const rmi_dataset* ds, const char* model_spec, uint64_t b
   return train_entry(ds, model_spec, branch_factor, flags, l0_fparams, n_fparams, out);
 }
 
+int rmi_cache_fix_device(const rmi_dataset* ds, uint64_t line_size, rmi_spline_point** out_points, uint64_t* out_count,
+                         rmi_cache_fix_stats* stats) {
+  g_last_error.clear();
+  const std::string fn = "rmi_cache_fix_device";
+  if (!ds || !out_points || !out_count) return fail(RMI_ERR_INVALID, fn + ": null argument");
+  if (ds->key_type != RMI_KEY_U64) return fail(RMI_ERR_INVALID, fn + ": Can only construct a bounded RMI on u64 data");
+  // The host scan's panics, in its order (cache_fix.hpp).  Nothing else can fire on sorted keys: along the point
+  // stream x strictly increases (a key's minus point is emitted only when it differs from the previous key, and
+  // key - 1 >= previous key for distinct sorted keys), so minus_epsilon's and add_point's ordering asserts hold, and
+  // offsets never decrease, so dest.1 >= from_y holds.  The one exception is key 0: its minus point wraps to
+  // 2^64 - 1 and with_new_dest then refuses the following point (0, 0).
+  const uint64_t n = ds->n;
+  if (!(n > line_size)) return fail(RMI_ERR_PANIC, "Cannot apply a cachefix with fewer items than the line size");
+  if (line_size == 0) return fail(RMI_ERR_PANIC, "attempt to divide by zero");
+  if (!ds->sorted) return fail(RMI_ERR_PANIC, "keys are not sorted in ascending order");
+  CUDA_TRY(cudaSetDevice(ds->device));
+  DeviceInfo di;
+  if (int rc = device_info(ds->device, &di)) return rc;
+  BuildContext* bc = t_build_ctx.get(ds->device);
+  if (!bc) return fail(RMI_ERR_CUDA, fn + ": could not create the CUDA stream");
+  cudaStream_t st = bc->st;
+  const u64* keys = (const u64*)ds->d_keys;
+  uint64_t first = 0;
+  CUDA_TRY(cudaMemcpyAsync(&first, keys, sizeof(u64), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  if (first == 0) return fail(RMI_ERR_PANIC, "When source x is 18446744073709551615, cannot set dest x to 0");
+
+  const u64 chunk = CACHEFIX_CHUNK, nch = (n + chunk - 1) / chunk;
+  u64 h_stats[CF_NUM_STATS] = {};
+  rmi_spline_point* host = nullptr;
+  u64 total = 0;
+  cudaError_t e = cudaSuccess;
+  {
+    Arena A(st);
+    CacheFixScratch s;
+    s.targets = A.get<u64>(nch * CACHEFIX_TARGETS);
+    s.spec_count = A.get<u64>(nch);
+    s.spec_exit = A.get<u64>(nch);
+    s.stitch_exit = A.get<u64>(nch);
+    s.stitch_ok = A.get<u32>(nch);
+    s.entry = A.get<u64>(nch);
+    s.count = A.get<u64>(nch);
+    s.offsets = A.get<u64>(nch + 1);
+    s.last_knot = A.get<u64>(2);
+    s.stats = A.get<u64>(CF_NUM_STATS);
+    e = A.err;
+    if (e == cudaSuccess) e = cudaMemsetAsync(s.stats, 0, sizeof(u64) * CF_NUM_STATS, st);
+    Launch L{st, di.num_sms};
+    if (e == cudaSuccess) {
+      cache_fix_scan(L, keys, n, line_size, chunk, s);
+      e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&total, s.offsets + nch, sizeof(u64), cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    ++total;   // finish()'s last point
+    u64* d_out = e == cudaSuccess ? A.get<u64>(2 * total) : nullptr;
+    if (e == cudaSuccess) e = A.err;
+    if (e == cudaSuccess) {
+      cache_fix_emit(L, keys, n, line_size, chunk, s, d_out);
+      e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h_stats, s.stats, sizeof h_stats, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) {
+      host = static_cast<rmi_spline_point*>(std::malloc(total * sizeof(rmi_spline_point)));
+      if (!host) return fail(RMI_ERR_INVALID, fn + ": out of host memory");
+      e = cudaMemcpyAsync(host, d_out, total * sizeof(rmi_spline_point), cudaMemcpyDeviceToHost, st);
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  }
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);   // the scratch is back in the pool
+  if (e != cudaSuccess) {
+    std::free(host);
+    return fail(RMI_ERR_CUDA, fn + ": " + cudaGetErrorString(e));
+  }
+  *out_points = host;
+  *out_count = total;
+  if (stats) {
+    stats->chunk_keys = chunk;
+    stats->chunks = nch;
+    stats->points = h_stats[CF_STAT_POINTS];
+    stats->stitch_segments = h_stats[CF_STAT_STITCH_SEGMENTS];
+    stats->fallback_points = h_stats[CF_STAT_FALLBACK_POINTS];
+    stats->evaluations = h_stats[CF_STAT_EVALS];
+  }
+  return RMI_OK;
+}
+
 }  // extern "C"
 
 // ===========================================================================================

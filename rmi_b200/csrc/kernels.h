@@ -164,6 +164,32 @@ void lookup_bounded_batch(const Launch& L, const TopModel& top, int leaf_kind, c
                           const void* d_knots, u64 K, u64 line_size, const u64* keys, u64 n, const u64* d_queries,
                           u64 nq, u64* d_out, u64* d_out_err, u64* d_fallbacks, bool lower_bound);
 
+// ---- the `--bounded` cache-fix scan (kernels_cachefix.cu, DESIGN.md section 12) ----------------------------------
+// Key indices per speculation chunk, and how many of a chunk's speculative knots the stitch can join.
+// (DESIGN.md section 12.3 gives the sweep.)
+constexpr u64 CACHEFIX_CHUNK = 256;
+constexpr int CACHEFIX_TARGETS = 16;
+enum CacheFixStat { CF_STAT_POINTS = 0, CF_STAT_STITCH_SEGMENTS = 1, CF_STAT_FALLBACK_POINTS = 2, CF_STAT_EVALS = 3,
+                    CF_NUM_STATS = 4 };
+// Device scratch of one scan, nch = ceil(n / chunk) chunks: O(nch) words.
+struct CacheFixScratch {
+  u64* targets;       // nch x CACHEFIX_TARGETS: pids of the first knots of each chunk's speculative chain
+  u64* spec_count;    // nch: knots the speculative chain starts inside its chunk
+  u64* spec_exit;     // nch: its first knot at or past the chunk's end
+  u64* stitch_exit;   // nch: the chunk's exit as the stitch found it
+  u32* stitch_ok;     // nch
+  u64* entry;         // nch: the chunk's first true knot (pid; may lie past the chunk)
+  u64* count;         // nch: true knots inside the chunk
+  u64* offsets;       // nch + 1: exclusive scan of count; offsets[nch] = knots before finish()'s last point
+  u64* last_knot;     // 2: the point finish() appends
+  u64* stats;         // CF_NUM_STATS counters, zeroed by the caller
+};
+// count / speculate / stitch / resolve: four launches on L.stream; s.offsets[nch] then holds the knot count - 1.
+void cache_fix_scan(const Launch& L, const u64* keys, u64 n, u64 line, u64 chunk, const CacheFixScratch& s);
+// One launch: writes the offsets[nch] + 1 knots as {key, offset} pairs to d_out.
+void cache_fix_emit(const Launch& L, const u64* keys, u64 n, u64 line, u64 chunk, const CacheFixScratch& s,
+                    void* d_out);
+
 // ---- range-partitioned build phases (kernels_shard.cu) ---------------------------------------
 size_t shard_scratch_bytes();
 template <class T>

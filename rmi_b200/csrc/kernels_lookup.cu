@@ -17,6 +17,7 @@
 #include <cstring>
 
 #include "kernels.h"
+#include "spline.cuh"
 
 namespace rmi {
 
@@ -254,9 +255,7 @@ k_lookup_bounded(const __grid_constant__ TopModel top, const ulonglong2* __restr
       pos = 0;
     } else {
       const ulonglong2 p0 = knots[res - 1], p1 = knots[res];
-      const double tt = __ddiv_rn(__ull2double_rn(q - p0.x), __ull2double_rn(p1.x - p0.x));
-      const double y = __fma_rn(__dsub_rn(1.0, tt), __ull2double_rn(p0.y), __dmul_rn(tt, __ull2double_rn(p1.y)));
-      pos = f64_to_u64_sat(y) / line * line;
+      pos = cache_fix_interp(q, p0.x, p0.y, p1.x, p1.y) / line * line;
     }
     if (!lower_bound) {
       __stcs(out + i, pos);

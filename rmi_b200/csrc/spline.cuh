@@ -54,4 +54,13 @@ __device__ __forceinline__ void cubic_from_points(double xmin, double ymin, doub
   d = __dadd_rn(d, ymin);
 }
 
+// The cache-fix spline's interpolation between (x0, y0) and (x1, y1) at x (cache_fix.rs:36-43, and the generated
+// spline lookup, codegen.rs:410-437): t = (x - x0) / (x1 - x0) with wrapping u64 subtractions,
+// fma(1 - t, y0, t * y1), then Rust's saturating `as u64` (NaN -> 0).  Shared by the bounded lookup
+// (kernels_lookup.cu) and the device cache-fix scan (kernels_cachefix.cu), which must agree with the host bit for bit.
+__device__ __forceinline__ u64 cache_fix_interp(u64 x, u64 x0, u64 y0, u64 x1, u64 y1) {
+  const double t = __ddiv_rn(__ull2double_rn(x - x0), __ull2double_rn(x1 - x0));
+  return f64_to_u64_sat(__fma_rn(__dsub_rn(1.0, t), __ull2double_rn(y0), __dmul_rn(t, __ull2double_rn(y1))));
+}
+
 }  // namespace rmi
