@@ -925,6 +925,9 @@ int train_typed(const rmi_dataset* ds, const ModelName& top, const ModelName& le
     u64* d_counts = A.get<u64>(N);
     void* d_scratch = A.get<char>(top_scratch_bytes(N));
     void* d_stats = A.get<char>(stats_scratch_bytes(N));
+    // the key sample the top fit leaves for the boundary search (kernels.h); not with injected top parameters
+    T* d_sample = !l0_over && top_fit_writes_sample(top.kind, (flags & RMI_FLAG_TOP_FIT_EXACT) != 0)
+                      ? bounds_sample_at<T>(A.get<char>(bounds_sample_bytes(n, sizeof(T)))) : nullptr;
     u32* d_table = nullptr;
     u64 *d_pivots = nullptr, *d_ri = nullptr;
     u64 hist_bins = 0, hist_ipb = 0;
@@ -973,11 +976,11 @@ int train_typed(const rmi_dataset* ds, const ModelName& top, const ModelName& le
       bool leaf_results_copied = false;
       if (!l0_over && !host_top && rc == RMI_OK)
         host_status |= fit_top_model<T>(L, keys, n, top.kind, top.table_bits, N, exact, d_top, d_aux, d_scratch, d_table,
-                                        d_pivots, d_ri);
+                                        d_pivots, d_ri, d_sample);
       cudaEventRecord(evp[0], st);
       if (host_status == 0 && rc == RMI_OK) {
         // injected top parameters are not known to be monotone: take the streaming pass, which checks
-        compute_leaf_bounds<T>(L, keys, n, top.kind, d_top, N, d_S, d_aux, /*allow_search=*/l0_over == nullptr);
+        compute_leaf_bounds<T>(L, keys, n, top.kind, d_top, N, d_S, d_aux, /*allow_search=*/l0_over == nullptr, d_sample);
         cudaEventRecord(evp[1], st);
         {
           Shard<T> whole = whole_array<T>(n);
@@ -1117,6 +1120,8 @@ int train_batch_typed(const rmi_dataset* ds, const ModelName& top, const std::ve
     u64* d_counts = A.get<u64>(N);
     void* d_scratch = A.get<char>(top_scratch_bytes(N));
     void* d_stats = A.get<char>(stats_scratch_bytes(N));
+    T* d_sample = top_fit_writes_sample(top.kind, (flags & RMI_FLAG_TOP_FIT_EXACT) != 0)
+                      ? bounds_sample_at<T>(A.get<char>(bounds_sample_bytes(n, sizeof(T)))) : nullptr;
     u32* d_table = nullptr;
     u64 *d_pivots = nullptr, *d_ri = nullptr;
     u64 hist_bins = 0, hist_ipb = 0;
@@ -1144,9 +1149,9 @@ int train_batch_typed(const rmi_dataset* ds, const ModelName& top, const std::ve
       cudaMemsetAsync(d_aux0, 0, sizeof(BuildAux), st);
       const bool exact = (flags & RMI_FLAG_TOP_FIT_EXACT) != 0;
       unsigned host_status = fit_top_model<T>(L, keys, n, top.kind, top.table_bits, N, exact, d_top, d_aux0, d_scratch, d_table,
-                                              d_pivots, d_ri);
+                                              d_pivots, d_ri, d_sample);
       if (host_status == 0) {
-        compute_leaf_bounds<T>(L, keys, n, top.kind, d_top, N, d_S, d_aux0, /*allow_search=*/true);
+        compute_leaf_bounds<T>(L, keys, n, top.kind, d_top, N, d_S, d_aux0, /*allow_search=*/true, d_sample);
         Shard<T> whole = whole_array<T>(n);
         whole.no_dups = ds->no_dups ? 1 : 0;
         for (size_t k = 0; k < K; ++k) {

@@ -62,6 +62,55 @@ __device__ __forceinline__ int load_keys4(const T* __restrict__ keys, u64 base, 
 }
 __device__ __forceinline__ bool is_aligned16(const void* p) { return (reinterpret_cast<unsigned long long>(p) & 15ull) == 0; }
 
+// createpolicy for an L2 eviction priority: 0 evict_normal, 1 evict_first, 2 evict_last.
+__device__ __forceinline__ u64 l2_policy_of(int kind) {
+  u64 p;
+  if (kind == 1) asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+  else if (kind == 2) asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
+  else asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+
+// load_keys4 with an L2 eviction policy (l2_policy_of) on the 128-bit loads.
+template <class T>
+__device__ __forceinline__ int load_keys4_hint(const T* __restrict__ keys, u64 base, u64 n, bool aligned16, T (&k)[4],
+                                               u64 policy) {
+  int cnt = (n - base) < 4ull ? (int)(n - base) : 4;
+  if (cnt == 4 && aligned16) {
+    u64 raw8[4];
+    u32 raw4[4];
+    if (sizeof(T) == 8) {
+      const T* p = keys + base;
+      asm("ld.global.nc.L2::cache_hint.v2.u64 {%0, %1}, [%2], %3;" : "=l"(raw8[0]), "=l"(raw8[1]) : "l"(p), "l"(policy));
+      asm("ld.global.nc.L2::cache_hint.v2.u64 {%0, %1}, [%2], %3;" : "=l"(raw8[2]), "=l"(raw8[3]) : "l"(p + 2), "l"(policy));
+#pragma unroll
+      for (int e = 0; e < 4; ++e) memcpy(&k[e], &raw8[e], sizeof(T));
+    } else {
+      asm("ld.global.nc.L2::cache_hint.v4.u32 {%0, %1, %2, %3}, [%4], %5;"
+          : "=r"(raw4[0]), "=r"(raw4[1]), "=r"(raw4[2]), "=r"(raw4[3]) : "l"(keys + base), "l"(policy));
+#pragma unroll
+      for (int e = 0; e < 4; ++e) memcpy(&k[e], &raw4[e], sizeof(T));
+    }
+  } else {
+#pragma unroll
+    for (int e = 0; e < 4; ++e) k[e] = keys[base + (u64)(e < cnt ? e : cnt - 1)];
+  }
+  return cnt;
+}
+
+// One key stored with an L2 eviction policy (l2_policy_of).
+template <class T> __device__ __forceinline__ void store_key_hint(T* p, T v, u64 policy) {
+  if (sizeof(T) == 8) {
+    u64 b;
+    memcpy(&b, &v, 8);
+    asm volatile("st.global.L2::cache_hint.b64 [%0], %1, %2;" ::"l"(p), "l"(b), "l"(policy) : "memory");
+  } else {
+    u32 b;
+    memcpy(&b, &v, 4);
+    asm volatile("st.global.L2::cache_hint.b32 [%0], %1, %2;" ::"l"(p), "r"(b), "l"(policy) : "memory");
+  }
+}
+
 // map_scale! (reference models/mod.rs:238-250): (offset as f64 * sf) as usize when the
 // scale differs from 1.0 by more than f64::EPSILON.
 __device__ __forceinline__ u64 scale_offset(u64 off, double sf, int use_sf) {

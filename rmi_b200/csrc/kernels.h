@@ -97,16 +97,31 @@ constexpr u32 LONG_LEAF_CAP = 16;    // more long leaves than this: no separate 
 
 void count_launch();   // bumps the process-wide kernel launch counter (api.cu)
 
+// ---- key sample for the leaf-boundary search --------------------------------------------------
+// The parallel linear / robust_linear top fit streams every key anyway; on the way it leaves
+// sample[s] = keys[s * BOUNDS_SAMPLE_R] for s < bounds_sample_len(n) (25 MB at 200M u64 keys) with an L2 evict_last
+// policy, and compute_leaf_bounds() then finds each leaf boundary in the sample (from L2) before it touches the keys
+// (DESIGN.md section 4 gives the sweep of R).
+constexpr u64 BOUNDS_SAMPLE_R = 64;
+__host__ __device__ inline u64 bounds_sample_len(u64 n) { return (n + BOUNDS_SAMPLE_R - 1) / BOUNDS_SAMPLE_R; }
+// The sample occupies whole 128-byte L2 lines of its own (compute_leaf_bounds discards them once the search is done):
+// allocate bounds_sample_bytes() and place the sample at bounds_sample_at() of that allocation.
+inline size_t bounds_sample_bytes(u64 n, size_t key_bytes) { return (bounds_sample_len(n) * key_bytes + 127) / 128 * 128 + 128; }
+template <class T> inline T* bounds_sample_at(void* raw) { return (T*)(((uintptr_t)raw + 127) & ~(uintptr_t)127); }
+// The top fits that stream the keys on the device and leave the sample behind.
+inline bool top_fit_writes_sample(int kind, bool exact) { return (kind == M_LINEAR || kind == M_ROBUST_LINEAR) && !exact; }
+
 // ---- top-model fits (kernels_top.cu) -------------------------------------------------------
 // All write the fitted model into *d_top (device) and OR failure bits into d_aux->status.
 // `scratch` must hold at least top_scratch_bytes() bytes.
 size_t top_scratch_bytes(u64 num_leaves);
 // Returns host-detected StatusBits (0 = launched); device-detected ones land in d_aux->status.
+// d_sample: null, or where the key sample goes when top_fit_writes_sample(kind, exact).
 void histogram_bins(u64 n, u64 num_leaves, u64* num_bins, u64* items_per_bin);
 template <class T>
 unsigned fit_top_model(const Launch& L, const T* keys, u64 n, int kind, int table_bits, u64 num_leaves, bool exact,
                        TopModel* d_top, BuildAux* d_aux, void* scratch, u32* d_table32, u64* d_pivots,
-                       u64* d_radix_index);
+                       u64* d_radix_index, T* d_sample);
 
 // Sortedness of a key array (verified once per dataset): *d_flag |= 1 if out of order.
 template <class T> void check_sorted(const Launch& L, const T* keys, u64 n, u64 i0, u64 i1, unsigned* d_flag);
@@ -114,9 +129,11 @@ template <class T> void check_sorted(const Launch& L, const T* keys, u64 n, u64 
 // ---- leaf layer (kernels_leaf.cu) ----------------------------------------------------------
 // S[j] = first index whose clamped top prediction is >= j, for j in [0, N]; also verifies
 // sortedness and monotonicity and derives the split (two_layer.rs:131-175).
+// d_sample: the key sample fit_top_model left (null if none); when the boundaries are searched, the search starts in
+// it, and afterwards its L2 lines are discarded (its contents are undefined from then on).
 template <class T>
 void compute_leaf_bounds(const Launch& L, const T* keys, u64 n, int top_kind, const TopModel* d_top, u64 num_leaves,
-                         u64* d_S, BuildAux* d_aux, bool allow_search);
+                         u64* d_S, BuildAux* d_aux, bool allow_search, const T* d_sample);
 // Fused per-leaf pass: closed-form fit (build_models_from), empty-leaf constants, forward
 // pass / max error, lower-bound widening (two_layer.rs:20-99, :186-259,
 // lower_bound_correction.rs:91-137).  Writes N x ppm params, N errors, N counts.

@@ -97,27 +97,75 @@ k_bounds(const T* __restrict__ keys, u64 n, const TopModel* __restrict__ top_ptr
 // keys.  ~28 probes per leaf instead of a pass over all n keys; neighbouring leaves share
 // the upper levels of the search in L1/L2.  Sortedness (and with it monotonicity of the
 // targets) is verified by k_leaf, which visits every consecutive key pair anyway.
+//
+// With a key sample (sample[s] = keys[s * BOUNDS_SAMPLE_R], s < ns, left in L2 by the linear top fit) the search runs
+// in two steps: the first sample point whose prediction reaches j, from L2, then the at most R - 1 keys between that
+// point and the one before it (512 B at R = 64), whose first two probes are placed by interpolation.  The predicate is
+// evaluated on the same keys, so S is the same.
+// Without the sample the lower levels of every search are separate DRAM sectors of the 1.6 GB key array, and the phase
+// is bound by them: a two-level search over the boundaries (every 32nd first, the others in their brackets), a gallop
+// from j*n/N and a 4-ary search all probe the key array itself and were no faster.  With the sample, the DRAM sectors
+// of the last step set the cost, so R and the interpolated first probes matter.  Measured on the headline build:
+// 0.238 ms without the sample; with it, bisecting the last step, 0.140 / 0.153 / 0.181 / 0.203 ms at R = 32 / 64 /
+// 128 / 256 (H100 SXM, 700 W limit); with the interpolated probes 0.120 ms at R = 64 and 0.122 ms at R = 32, against
+// 0.235 ms without the sample (400 W limit).  DESIGN.md section 4.
 template <class T, int TOP>
 __global__ void __launch_bounds__(BOUNDS_THREADS)
 k_bounds_search(const T* __restrict__ keys, u64 n, const TopModel* __restrict__ top_ptr, u64 N,
-                u64* __restrict__ S) {
+                u64* __restrict__ S, const T* __restrict__ sample) {
   TopModel m = *top_ptr;
   u64 j = (u64)blockIdx.x * blockDim.x + threadIdx.x;
   if (j > N) return;
   u64 lo = 0, hi = n;
   if (j == N) lo = n;
   else if (j > 0) {
-    // (alternatives tried and dropped: a two-level search — every 32nd boundary first, the others between their
-    //  brackets, ~13 probes in a 48 KB window — no faster; galloping outwards from the interpolated index j*n/N
-    //  — slower, the divergent gallop loops cost more than the saved probes — and a 4-ary search with three
-    //  independent probes per level — no change: the phase is bound by DRAM sectors per boundary, not by levels
-    //  of latency)
+    if (sample) {
+      const u64 ns = bounds_sample_len(n);
+      u64 a = 0, b = ns;
+      while (a < b) {
+        u64 mid = a + ((b - a) >> 1);
+        if (top_predict<TOP>(m, sample[mid]) >= j) b = mid; else a = mid + 1;
+      }
+      // keys[(a - 1) * R] predicts below j, keys[a * R] (if a < ns) reaches it
+      if (a == 0) hi = 0;
+      else {
+        lo = (a - 1) * BOUNDS_SAMPLE_R + 1;
+        hi = a * BOUNDS_SAMPLE_R < n ? a * BOUNDS_SAMPLE_R : n;
+        if (TOP == M_LINEAR && a < ns && lo < hi) {
+          // First probes: the index where the line between the two sample points reaches the key at which the top
+          // model predicts j, then one 32-byte sector further towards the answer.  Within a sector of that guess the
+          // bracket is then down to two sectors, and the binary search below finishes it from L1.
+          constexpr u64 SK = 32 / sizeof(T);
+          const double k0 = Key<T>::as_float(sample[a - 1]), k1 = Key<T>::as_float(sample[a]);
+          double t = (__dadd_rn((double)j, -m.f[0]) / m.f[1] - k0) / (k1 - k0);
+          if (!(t >= 0.0)) t = 0.0;
+          if (t > 1.0) t = 1.0;
+          u64 g = lo + (u64)(t * (double)(hi - lo));
+          if (g >= hi) g = hi - 1;
+          const bool below = top_predict<TOP>(m, keys[g]) >= j;   // the answer is at or below g
+          if (below) hi = g; else lo = g + 1;
+          if (lo < hi) {
+            const u64 g2 = below ? (g >= lo + SK ? g - SK : lo) : (g + SK < hi ? g + SK : hi - 1);
+            if (top_predict<TOP>(m, keys[g2]) >= j) hi = g2; else lo = g2 + 1;
+          }
+        }
+      }
+    }
     while (lo < hi) {
       u64 mid = lo + ((hi - lo) >> 1);
       if (top_predict<TOP>(m, keys[mid]) >= j) hi = mid; else lo = mid + 1;
     }
   }
   S[j] = lo;
+}
+
+// Drops the key sample's lines from L2 without writing them back: k_leaf's forward pass lives on the L2 lines its fit
+// pass left behind (DESIGN.md section 4), and evict_last lines of a sample nobody reads again would take their place.
+// `lines` whole 128-byte lines from the 128-byte aligned `p` (bounds_sample_at).
+__global__ void k_discard_l2(const char* p, u64 lines) {
+  u64 stride = (u64)gridDim.x * blockDim.x;
+  for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < lines; i += stride)
+    asm volatile("discard.global.L2 [%0], 128;" ::"l"(p + i * 128) : "memory");
 }
 __host__ __device__ constexpr bool top_is_monotone_by_construction(int kind) {
   return kind == M_LINEAR || kind == M_ROBUST_LINEAR || kind == M_LINEAR_SPLINE || kind == M_RADIX ||
@@ -168,14 +216,6 @@ constexpr int PIECE_STRIDE = 16;   // bytes between a row's consecutive pieces
 constexpr int SSTAGES = 2;
 constexpr int WARP_STREAM_BYTES = SSTAGES * STAGE_BYTES + 32 * 4 + 32 * 4;
 
-// createpolicy for an L2 eviction priority: 0 evict_normal, 1 evict_first, 2 evict_last.
-__device__ __forceinline__ u64 l2_policy_of(int kind) {
-  u64 p;
-  if (kind == 1) asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-  else if (kind == 2) asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
-  else asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(p));
-  return p;
-}
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src, int src_bytes) {
   unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(d), "l"(gmem_src), "r"(src_bytes) : "memory");
@@ -1649,13 +1689,18 @@ int grid_cap(u64 n, int threads, int cap) {
 
 template <class T, int TOP>
 void launch_bounds_impl(const Launch& L, const T* keys, u64 n, const TopModel* d_top, u64 N, u64* d_S, BuildAux* d_aux,
-                   bool allow_search) {
+                   bool allow_search, const T* d_sample) {
   if (allow_search && top_is_monotone_by_construction(TOP)) {
     k_bounds_search<T, TOP><<<(unsigned)((N + 1 + BOUNDS_THREADS - 1) / BOUNDS_THREADS), BOUNDS_THREADS, 0, L.stream>>>(
-        keys, n, d_top, N, d_S);
+        keys, n, d_top, N, d_S, d_sample);
     count_launch();
     k_split<T, TOP><<<1, 32, 0, L.stream>>>(keys, n, d_top, N, d_S, d_aux, 1);
     count_launch();
+    const u64 lines = (bounds_sample_len(n) * sizeof(T) + 127) / 128;
+    if (d_sample && lines) {
+      k_discard_l2<<<grid_cap(lines, BOUNDS_THREADS, L.num_sms * 8), BOUNDS_THREADS, 0, L.stream>>>((const char*)d_sample, lines);
+      count_launch();
+    }
     return;
   }
   k_fill<<<grid_cap(N + 1, BOUNDS_THREADS, L.num_sms * 8), BOUNDS_THREADS, 0, L.stream>>>(d_S, N + 1, n);
@@ -1810,19 +1855,19 @@ void launch_leaf(const Launch& L, const T* keys, const Shard<T>& sh, u64 N, cons
 
 template <class T>
 void compute_leaf_bounds(const Launch& L, const T* keys, u64 n, int top_kind, const TopModel* d_top, u64 N, u64* d_S,
-                         BuildAux* d_aux, bool allow_search) {
+                         BuildAux* d_aux, bool allow_search, const T* d_sample) {
   switch (top_kind) {
     case M_LINEAR:
     case M_ROBUST_LINEAR:
-    case M_LINEAR_SPLINE: launch_bounds_impl<T, M_LINEAR>(L, keys, n, d_top, N, d_S, d_aux, allow_search); break;
-    case M_CUBIC: launch_bounds_impl<T, M_CUBIC>(L, keys, n, d_top, N, d_S, d_aux, allow_search); break;
-    case M_LOGLINEAR: launch_bounds_impl<T, M_LOGLINEAR>(L, keys, n, d_top, N, d_S, d_aux, allow_search); break;
-    case M_NORMAL: launch_bounds_impl<T, M_NORMAL>(L, keys, n, d_top, N, d_S, d_aux, allow_search); break;
-    case M_LOGNORMAL: launch_bounds_impl<T, M_LOGNORMAL>(L, keys, n, d_top, N, d_S, d_aux, allow_search); break;
-    case M_RADIX: launch_bounds_impl<T, M_RADIX>(L, keys, n, d_top, N, d_S, d_aux, allow_search); break;
-    case M_RADIX_TABLE: launch_bounds_impl<T, M_RADIX_TABLE>(L, keys, n, d_top, N, d_S, d_aux, allow_search); break;
-    case M_BRADIX: launch_bounds_impl<T, M_BRADIX>(L, keys, n, d_top, N, d_S, d_aux, allow_search); break;
-    case M_HISTOGRAM: launch_bounds_impl<T, M_HISTOGRAM>(L, keys, n, d_top, N, d_S, d_aux, allow_search); break;
+    case M_LINEAR_SPLINE: launch_bounds_impl<T, M_LINEAR>(L, keys, n, d_top, N, d_S, d_aux, allow_search, d_sample); break;
+    case M_CUBIC: launch_bounds_impl<T, M_CUBIC>(L, keys, n, d_top, N, d_S, d_aux, allow_search, nullptr); break;
+    case M_LOGLINEAR: launch_bounds_impl<T, M_LOGLINEAR>(L, keys, n, d_top, N, d_S, d_aux, allow_search, nullptr); break;
+    case M_NORMAL: launch_bounds_impl<T, M_NORMAL>(L, keys, n, d_top, N, d_S, d_aux, allow_search, nullptr); break;
+    case M_LOGNORMAL: launch_bounds_impl<T, M_LOGNORMAL>(L, keys, n, d_top, N, d_S, d_aux, allow_search, nullptr); break;
+    case M_RADIX: launch_bounds_impl<T, M_RADIX>(L, keys, n, d_top, N, d_S, d_aux, allow_search, nullptr); break;
+    case M_RADIX_TABLE: launch_bounds_impl<T, M_RADIX_TABLE>(L, keys, n, d_top, N, d_S, d_aux, allow_search, nullptr); break;
+    case M_BRADIX: launch_bounds_impl<T, M_BRADIX>(L, keys, n, d_top, N, d_S, d_aux, allow_search, nullptr); break;
+    case M_HISTOGRAM: launch_bounds_impl<T, M_HISTOGRAM>(L, keys, n, d_top, N, d_S, d_aux, allow_search, nullptr); break;
     default: break;
   }
 }
@@ -1909,7 +1954,7 @@ void leaf_statistics_merge(const Launch& L, const void* d_parts, int world, Buil
 }
 
 #define INST(T)                                                                                                  \
-  template void compute_leaf_bounds<T>(const Launch&, const T*, u64, int, const TopModel*, u64, u64*, BuildAux*, bool); \
+  template void compute_leaf_bounds<T>(const Launch&, const T*, u64, int, const TopModel*, u64, u64*, BuildAux*, bool, const T*); \
   template void fit_leaves<T>(const Launch&, const T*, const Shard<T>&, int, u64, const u64*, BuildAux*, double*, u64*, u64*);
 INST(u64)
 INST(u32)

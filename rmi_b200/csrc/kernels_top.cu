@@ -38,27 +38,42 @@ __device__ __forceinline__ void stream_item(const T* __restrict__ keys, u64 i, d
 // slr()'s closing formulas (linear.rs:36-58).  MODE 0: y;  MODE 1: ln(y), non-finite dropped
 // (loglinear_slr, linear.rs:61-72).
 // partial layout per block: {Sx, Sy, Sxx, Sxy, count}
+// sample (MODE 0, may be null): receives keys[s * BOUNDS_SAMPLE_R] for every s < bounds_sample_len(n), stored
+// evict_last so that the sample is still in L2 when the boundary search reads it; the keys themselves are loaded
+// evict_first, so that this 1.6 GB stream does not push the sample out.
 // ------------------------------------------------------------------------------------------
 template <class T, int MODE>
 __global__ void __launch_bounds__(TOP_THREADS)
 k_slr_partial(const T* __restrict__ keys, u64 n, u64 i0, u64 i1, double sf, int use_sf,
-              double* __restrict__ partials) {
+              double* __restrict__ partials, T* __restrict__ sample) {
   __shared__ double sm[32];
   u64 mid = i0 + ((i1 - i0) >> 1);
   double px = Key<T>::as_float(keys[mid]);
   double py = MODE == 0 ? __ull2double_rn(scale_offset(mid, sf, use_sf)) : 0.0;
   double sx = 0, sy = 0, sxx = 0, sxy = 0, cnt = 0;
   const bool aligned = is_aligned16(keys);
+  const u64 ld_policy = l2_policy_of(1), st_policy = l2_policy_of(2);
   // each thread owns 4 consecutive keys per trip (128-bit loads); [i0, i1) is covered from the
   // 4-aligned index at or below i0
+  const u64 tid = (u64)blockIdx.x * blockDim.x + threadIdx.x;
   u64 stride = (u64)gridDim.x * blockDim.x * 4;
   unsigned icnt = 0;
-  for (u64 base = (i0 & ~3ull) + ((u64)blockIdx.x * blockDim.x + threadIdx.x) * 4; base < i1; base += stride) {
-    T k[4];
-    int c = load_keys4(keys, base, n, aligned, k);
+  if (MODE == 0 && sample) {
+    // sample points the loop below does not visit: robust_linear sums [i0, i1) only, the sample covers [0, n)
+    const u64 lo_pts = ((i0 & ~3ull) + BOUNDS_SAMPLE_R - 1) / BOUNDS_SAMPLE_R;   // s * R < (i0 & ~3)
+    const u64 hi_first = (i1 + BOUNDS_SAMPLE_R - 1) / BOUNDS_SAMPLE_R;           // s * R >= i1
+    const u64 extra = lo_pts + (bounds_sample_len(n) - hi_first);
+    for (u64 q = tid; q < extra; q += stride / 4) {
+      const u64 s = q < lo_pts ? q : hi_first + (q - lo_pts);
+      store_key_hint(sample + s, keys[s * BOUNDS_SAMPLE_R], st_policy);
+    }
+  }
+  // One trip: the 4 keys at `base` (c of them valid), kprev = keys[base - 1].
+  auto trip = [&](u64 base, const T (&k)[4], int c, T kprev) {
+    if (MODE == 0 && sample && base % BOUNDS_SAMPLE_R == 0) store_key_hint(sample + base / BOUNDS_SAMPLE_R, k[0], st_policy);
     bool interior = MODE == 0 && c == 4 && base >= i0 && base + 4 <= i1;
     if (interior) {
-      bool dup = (base > 0 && keys[base - 1] == k[0]) || k[1] == k[0] || k[2] == k[1] || k[3] == k[2];
+      bool dup = (base > 0 && kprev == k[0]) || k[1] == k[0] || k[2] == k[1] || k[3] == k[2];
       if (!dup) {
         // fast path: every key starts its own run, so the offset of key e is base + e and the
         // scaled target floor(offset * sf) is taken with the 2^52 trick (0 <= value < 2^51)
@@ -72,7 +87,7 @@ k_slr_partial(const T* __restrict__ keys, u64 n, u64 i0, u64 i1, double sf, int 
           sx += dx; sy += dy; sxx = fma(dx, dx, sxx); sxy = fma(dx, dy, sxy);
         }
         icnt += 4;
-        continue;
+        return;
       }
     }
     // general path: duplicates, range edges, log targets
@@ -90,6 +105,24 @@ k_slr_partial(const T* __restrict__ keys, u64 n, u64 i0, u64 i1, double sf, int 
       sx += dx; sy += dy; sxx = fma(dx, dx, sxx); sxy = fma(dx, dy, sxy);
       icnt += 1;
     }
+  };
+  // Two trips per iteration, both loaded before either is summed, in the order a one-trip loop takes them (the sums do
+  // not change).  The loop runs while the warp's first lane has keys, so every lane takes part in the shuffles: lane l
+  // gets keys[base - 1] (lane l - 1's last key) from below, only lane 0 loads it.
+  const unsigned FULL = 0xffffffffu;
+  const unsigned lane = threadIdx.x & 31u;
+  for (u64 wb = (i0 & ~3ull) + (tid - lane) * 4; wb < i1; wb += 2 * stride) {
+    const u64 b0 = wb + lane * 4, b1 = b0 + stride;
+    T k0[4] = {}, k1[4] = {};
+    const int c0 = b0 < i1 ? load_keys4_hint(keys, b0, n, aligned, k0, ld_policy) : 0;
+    const int c1 = b1 < i1 ? load_keys4_hint(keys, b1, n, aligned, k1, ld_policy) : 0;
+    T p0 = __shfl_up_sync(FULL, k0[3], 1), p1 = __shfl_up_sync(FULL, k1[3], 1);
+    if (lane == 0) {
+      if (c0 && b0 > 0) p0 = keys[b0 - 1];
+      if (c1) p1 = keys[b1 - 1];
+    }
+    if (c0) trip(b0, k0, c0, p0);
+    if (c1) trip(b1, k1, c1, p1);
   }
   cnt = (double)icnt;
   double r0 = block_sum(sx, sm), r1 = block_sum(sy, sm), r2 = block_sum(sxx, sm), r3 = block_sum(sxy, sm),
@@ -608,7 +641,7 @@ void histogram_bins(u64 n, u64 num_leaves, u64* num_bins, u64* items_per_bin) {
 template <class T>
 unsigned fit_top_model(const Launch& L, const T* keys, u64 n, int kind, int table_bits, u64 num_leaves, bool exact,
                        TopModel* d_top, BuildAux* d_aux, void* scratch, u32* d_table32, u64* d_pivots,
-                       u64* d_radix_index) {
+                       u64* d_radix_index, T* d_sample) {
   cudaStream_t st = L.stream;
   // two_layer.rs:109: scale = N / n, applied per models/mod.rs:238-250
   double sf = (double)num_leaves / (double)n;
@@ -639,7 +672,7 @@ unsigned fit_top_model(const Launch& L, const T* keys, u64 n, int kind, int tabl
         if (exact) { k_slr_exact<T, 1><<<1, 32, 0, st>>>(keys, i0, i1, repeat, sf, use_sf, d_top, d_aux); count_launch(); }
         else {
           int gg = i1 > i0 ? grid_for((i1 - i0 + 3) / 4 + 1, L.num_sms) : 1;
-          if (i1 > i0) { k_slr_partial<T, 1><<<gg, TOP_THREADS, 0, st>>>(keys, n, i0, i1, sf, use_sf, partials); count_launch(); }
+          if (i1 > i0) { k_slr_partial<T, 1><<<gg, TOP_THREADS, 0, st>>>(keys, n, i0, i1, sf, use_sf, partials, nullptr); count_launch(); }
           k_slr_finish<T, 1><<<1, TOP_THREADS, 0, st>>>(keys, i0, i1, repeat, sf, use_sf, partials, i1 > i0 ? gg : 0, d_top, d_aux);
           count_launch();
         }
@@ -648,7 +681,10 @@ unsigned fit_top_model(const Launch& L, const T* keys, u64 n, int kind, int tabl
         count_launch();
       } else {
         int gg = i1 > i0 ? grid_for((i1 - i0 + 3) / 4 + 1, L.num_sms) : 1;
-        if (i1 > i0) { k_slr_partial<T, 0><<<gg, TOP_THREADS, 0, st>>>(keys, n, i0, i1, sf, use_sf, partials); count_launch(); }
+        if (i1 > i0) {
+          k_slr_partial<T, 0><<<gg, TOP_THREADS, 0, st>>>(keys, n, i0, i1, sf, use_sf, partials, d_sample);
+          count_launch();
+        }
         k_slr_finish<T, 0><<<1, TOP_THREADS, 0, st>>>(keys, i0, i1, repeat, sf, use_sf, partials, i1 > i0 ? gg : 0, d_top, d_aux);
         count_launch();
       }
@@ -727,8 +763,8 @@ unsigned fit_top_model(const Launch& L, const T* keys, u64 n, int kind, int tabl
   return 0;
 }
 
-template unsigned fit_top_model<u64>(const Launch&, const u64*, u64, int, int, u64, bool, TopModel*, BuildAux*, void*, u32*, u64*, u64*);
-template unsigned fit_top_model<u32>(const Launch&, const u32*, u64, int, int, u64, bool, TopModel*, BuildAux*, void*, u32*, u64*, u64*);
-template unsigned fit_top_model<double>(const Launch&, const double*, u64, int, int, u64, bool, TopModel*, BuildAux*, void*, u32*, u64*, u64*);
+template unsigned fit_top_model<u64>(const Launch&, const u64*, u64, int, int, u64, bool, TopModel*, BuildAux*, void*, u32*, u64*, u64*, u64*);
+template unsigned fit_top_model<u32>(const Launch&, const u32*, u64, int, int, u64, bool, TopModel*, BuildAux*, void*, u32*, u64*, u64*, u32*);
+template unsigned fit_top_model<double>(const Launch&, const double*, u64, int, int, u64, bool, TopModel*, BuildAux*, void*, u32*, u64*, u64*, double*);
 
 }  // namespace rmi
