@@ -68,17 +68,73 @@ int device_info(int device, DeviceInfo* out) {
   return RMI_OK;
 }
 
-struct ModelName { const char* name; int kind; int table_bits; };
+// fparams / iparams: how many of TopModel::f / ::ip the model uses as a top model (models.cuh: TopModel).
+// root_only: the model may only be the root (train/mod.rs:59-85).
+// shard_rounds: rmi_shard_top_rounds (include/rmi_b200.h); -1 where range-partitioned builds do not offer the top.
+struct ModelName { const char* name; int kind; int table_bits; int fparams, iparams; bool root_only; int shard_rounds; };
 const ModelName kModels[] = {   // reference train/mod.rs:37-54
-    {"linear", M_LINEAR, 0},          {"robust_linear", M_ROBUST_LINEAR, 0}, {"linear_spline", M_LINEAR_SPLINE, 0},
-    {"cubic", M_CUBIC, 0},            {"loglinear", M_LOGLINEAR, 0},         {"normal", M_NORMAL, 0},
-    {"lognormal", M_LOGNORMAL, 0},    {"radix", M_RADIX, 0},                 {"radix8", M_RADIX_TABLE, 8},
-    {"radix18", M_RADIX_TABLE, 18},   {"radix22", M_RADIX_TABLE, 22},        {"radix26", M_RADIX_TABLE, 26},
-    {"radix28", M_RADIX_TABLE, 28},   {"bradix", M_BRADIX, 0},               {"histogram", M_HISTOGRAM, 0}};
+    {"linear", M_LINEAR, 0, 2, 0, false, 1},          {"robust_linear", M_ROBUST_LINEAR, 0, 2, 0, false, 1},
+    {"linear_spline", M_LINEAR_SPLINE, 0, 2, 0, false, 0}, {"cubic", M_CUBIC, 0, 4, 0, false, 3},
+    {"loglinear", M_LOGLINEAR, 0, 2, 0, false, -1},   {"normal", M_NORMAL, 0, 3, 0, false, 2},
+    {"lognormal", M_LOGNORMAL, 0, 3, 0, false, 2},    {"radix", M_RADIX, 0, 0, 2, true, 0},
+    {"radix8", M_RADIX_TABLE, 8, 0, 1, false, 4},     {"radix18", M_RADIX_TABLE, 18, 0, 1, false, 4},
+    {"radix22", M_RADIX_TABLE, 22, 0, 1, false, 4},   {"radix26", M_RADIX_TABLE, 26, 0, 1, false, 4},
+    {"radix28", M_RADIX_TABLE, 28, 0, 1, false, 4},   {"bradix", M_BRADIX, 0, 0, 3, true, -1},
+    {"histogram", M_HISTOGRAM, 0, 0, 1, true, 4}};
 
 const ModelName* find_model(const std::string& s) {
   for (const auto& m : kModels) if (s == m.name) return &m;
   return nullptr;
+}
+
+// ---- the reference's checks of a model spec and of a build's arguments, in rmi_train's order ----------------
+int find_layer(const std::string& name, bool is_root, const ModelName** out) {
+  const ModelName* m = find_model(name);
+  if (!m) return fail(RMI_ERR_PANIC, "Unknown model type: " + name);
+  if (m->root_only && !is_root) return fail(RMI_ERR_PANIC, "if used, model type " + name + " must be the root model");
+  *out = m;
+  return RMI_OK;
+}
+
+int check_leaf(const ModelName* leaf) {
+  if (leaf->kind == M_RADIX_TABLE)
+    return fail(RMI_ERR_UNSUPPORTED, "radix tables are only offered as the top model in this build");
+  return RMI_OK;
+}
+
+// train/mod.rs:104-125: split the spec on ',', validate every layer, then insist on two layers
+int parse_two_layer(const char* spec, const ModelName** top, const ModelName** leaf) {
+  std::vector<const ModelName*> models;
+  std::string s(spec);
+  for (size_t pos = 0;;) {
+    const size_t c = s.find(',', pos);
+    const ModelName* m = nullptr;
+    if (int rc = find_layer(s.substr(pos, c == std::string::npos ? std::string::npos : c - pos), models.empty(), &m)) return rc;
+    models.push_back(m);
+    if (c == std::string::npos) break;
+    pos = c + 1;
+  }
+  if (models.size() != 2)   // train/mod.rs:123-125 panic!() for anything but two layers
+    return fail(RMI_ERR_PANIC, "only two-layer RMIs can be trained (the reference panics on other depths)");
+  *top = models[0];
+  *leaf = models[1];
+  return check_leaf(*leaf);
+}
+
+int check_build(uint64_t n, uint64_t N, bool sorted) {
+  if (N < 1) return fail(RMI_ERR_PANIC, "branching factor must be at least 1");
+  if (n == 0) return fail(RMI_ERR_PANIC, "start index was 0 but end index was 0");
+  if (!sorted) return fail(RMI_ERR_PANIC, "keys are not sorted in ascending order");
+  return RMI_OK;
+}
+
+// f(T()) with T the C++ type of an rmi_key_type
+template <class F> auto with_key_type(int key_type, F&& f) {
+  switch (key_type) {
+    case RMI_KEY_U64: return f(u64());
+    case RMI_KEY_U32: return f(u32());
+    default: return f(double());
+  }
 }
 
 std::string status_text(unsigned st) {
@@ -132,11 +188,10 @@ int verify_sorted(rmi_dataset* ds) {
   CUDA_TRY(cudaMalloc(&d_flag, sizeof(unsigned)));
   cudaMemset(d_flag, 0, sizeof(unsigned));
   Launch L{nullptr, di.num_sms};
-  switch (ds->key_type) {
-    case RMI_KEY_U64: check_sorted<u64>(L, (const u64*)ds->d_keys, ds->n, 0, ds->n, d_flag); break;
-    case RMI_KEY_U32: check_sorted<u32>(L, (const u32*)ds->d_keys, ds->n, 0, ds->n, d_flag); break;
-    default: check_sorted<double>(L, (const double*)ds->d_keys, ds->n, 0, ds->n, d_flag); break;
-  }
+  with_key_type(ds->key_type, [&](auto k) {
+    using T = decltype(k);
+    check_sorted<T>(L, (const T*)ds->d_keys, ds->n, 0, ds->n, d_flag);
+  });
   unsigned h = 0;
   cudaError_t e = cudaMemcpy(&h, d_flag, sizeof(unsigned), cudaMemcpyDeviceToHost);
   cudaFree(d_flag);
@@ -222,6 +277,128 @@ struct ResultBox {
   PinnedArray<char> scalars;   // BuildAux + TopModel read-back
 };
 
+namespace {
+
+// The device tables of a table top: radix8..28's hint table, the histogram's pivots and radix index.
+struct TopTables {
+  u32* t32 = nullptr;
+  u64* pivots = nullptr;        // hist_bins + 1
+  u64* radix_index = nullptr;   // ri_len
+  u64 t32_len = 0, ri_len = 0;
+  u64 hist_bins = 0, hist_ipb = 0;
+
+  // alloc(bytes) returns device memory or null; false if an allocation failed
+  template <class Alloc> bool allocate(const ModelName& top, uint64_t n, uint64_t N, Alloc&& alloc) {
+    if (top.kind == M_RADIX_TABLE) {
+      t32_len = (u64)1 << top.table_bits;
+      t32 = (u32*)alloc(sizeof(u32) * t32_len);
+      return t32 != nullptr;
+    }
+    if (top.kind == M_HISTOGRAM) {
+      histogram_bins(n, N, &hist_bins, &hist_ipb);
+      ri_len = ((u64)1 << 20) + 1;
+      pivots = (u64*)alloc(sizeof(u64) * (hist_bins + 1));
+      radix_index = (u64*)alloc(sizeof(u64) * ri_len);
+      return pivots && radix_index;
+    }
+    return true;
+  }
+
+  // The TopModel a build starts from; f: nf injected top parameters, or null.
+  TopModel initial(const ModelName& top, const double* f = nullptr, uint32_t nf = 0) const {
+    TopModel h;
+    memset(&h, 0, sizeof(h));
+    h.kind = top.kind;
+    h.high = 1;
+    h.table_bits = top.table_bits;
+    h.t32 = t32;
+    h.pivots = pivots;
+    h.radix_index = radix_index;
+    h.npivots = hist_bins;
+    if (top.kind == M_HISTOGRAM) h.ip[0] = hist_bins;
+    for (uint32_t q = 0; f && q < nf && q < 4; ++q) h.f[q] = f[q];
+    return h;
+  }
+};
+
+// Takes the pinned buffers a build's result is copied into: the scalars, the leaf tables if `leaves` (and the key
+// counts if `counts`), and the top model's tables if `tables` is given.  False if page-locked memory ran out.
+bool reserve_result(ResultBox* box, const TopTables* tables, uint64_t N, int ppm, bool leaves, bool counts) {
+  bool ok = box->scalars.resize(sizeof(BuildAux) + sizeof(TopModel));
+  if (ok) memset(box->scalars.data(), 0, sizeof(BuildAux) + sizeof(TopModel));
+  if (leaves) ok = ok && box->l1_params.resize((size_t)N * ppm) && box->l1_errors.resize(N);
+  if (leaves && counts) ok = ok && box->l1_counts.resize(N);
+  if (tables && tables->t32_len) ok = ok && box->table32.resize(tables->t32_len);
+  if (tables && tables->ri_len) ok = ok && box->arr1.resize(tables->ri_len) && box->arr2.resize(tables->hist_bins);
+  return ok;
+}
+const char* const kPinnedFailed = "pinned host allocation for the results failed";
+
+// Issues the copies into the buffers reserve_result took: BuildAux and TopModel, then the leaf tables (params null:
+// none, or already copied; counts null: none), then the top model's tables (tables null: none).
+void copy_result_to_host(ResultBox* box, const TopTables* tables, const BuildAux* d_aux, const TopModel* d_top,
+                         const double* params, const u64* errors, const u64* counts, cudaStream_t st) {
+  cudaMemcpyAsync(box->scalars.data(), d_aux, sizeof(BuildAux), cudaMemcpyDeviceToHost, st);
+  cudaMemcpyAsync(box->scalars.data() + sizeof(BuildAux), d_top, sizeof(TopModel), cudaMemcpyDeviceToHost, st);
+  if (params) {
+    cudaMemcpyAsync(box->l1_params.data(), params, sizeof(double) * box->l1_params.size(), cudaMemcpyDeviceToHost, st);
+    cudaMemcpyAsync(box->l1_errors.data(), errors, sizeof(u64) * box->l1_errors.size(), cudaMemcpyDeviceToHost, st);
+    if (counts) cudaMemcpyAsync(box->l1_counts.data(), counts, sizeof(u64) * box->l1_counts.size(), cudaMemcpyDeviceToHost, st);
+  }
+  if (tables && tables->t32_len)
+    cudaMemcpyAsync(box->table32.data(), tables->t32, sizeof(u32) * tables->t32_len, cudaMemcpyDeviceToHost, st);
+  if (tables && tables->ri_len) {
+    cudaMemcpyAsync(box->arr1.data(), tables->radix_index, sizeof(u64) * tables->ri_len, cudaMemcpyDeviceToHost, st);
+    cudaMemcpyAsync(box->arr2.data(), tables->pivots, sizeof(u64) * tables->hist_bins, cudaMemcpyDeviceToHost, st);
+  }
+}
+
+const BuildAux& result_aux(const ResultBox* box) { return *reinterpret_cast<const BuildAux*>(box->scalars.ptr); }
+
+// The public struct from what copy_result_to_host brought back (the stream synchronised): the statistics
+// (two_layer.rs:267-284), the top model, the leaf model and the tables the box holds.  The top tables' lengths are
+// filled in even where the tables stay on the device: rmi_model_size reads them.
+void fill_result(ResultBox* box, const ModelName& top, const ModelName& leaf, const TopTables& tables, uint64_t n,
+                 uint64_t N) {
+  const BuildAux& a = result_aux(box);
+  const TopModel& t = *reinterpret_cast<const TopModel*>(box->scalars.ptr + sizeof(BuildAux));
+  rmi_result& R = box->pub;
+  memset(&R, 0, sizeof(R));
+  R.num_rmi_rows = n; R.num_data_rows = n; R.branching_factor = N;
+  R.model_max_error = a.max_error;
+  R.model_max_error_idx = a.max_error_idx;
+  R.model_avg_error = (double)a.sum_n_err / (double)n;
+  R.model_avg_l2_error = a.sum_l2;
+  R.model_avg_log2_error = a.sum_log2 / (double)n;
+  R.model_max_log2_error = std::log2((double)a.max_error);
+  R.l0_model_id = top.kind;
+  R.l0_bradix_high = t.high;
+  R.l0_table_bits = top.table_bits;
+  R.l0_num_fparams = top.fparams;
+  R.l0_num_iparams = top.iparams;
+  for (int q = 0; q < 4; ++q) { R.l0_fparams[q] = t.f[q]; R.l0_iparams[q] = t.ip[q]; }
+  R.l0_table32_len = tables.t32_len;
+  R.l0_table32 = box->table32.empty() ? nullptr : box->table32.data();
+  R.l0_array1_len = tables.ri_len;
+  R.l0_array1 = box->arr1.empty() ? nullptr : box->arr1.data();
+  R.l0_array2_len = tables.hist_bins;
+  R.l0_array2 = box->arr2.empty() ? nullptr : box->arr2.data();
+  R.l1_model_id = leaf.kind;
+  R.l1_params_per_model = leaf_params_per_model(leaf.kind);
+  R.l1_params = box->l1_params.empty() ? nullptr : box->l1_params.data();
+  R.l1_errors = box->l1_errors.empty() ? nullptr : box->l1_errors.data();
+  R.l1_counts = box->l1_counts.empty() ? nullptr : box->l1_counts.data();
+  R.could_not_replace = a.could_not_replace ? 1 : 0;
+}
+
+uint64_t elapsed_ns(cudaEvent_t a, cudaEvent_t b) {
+  float ms = 0.f;
+  cudaEventElapsedTime(&ms, a, b);
+  return (uint64_t)((double)ms * 1e6);
+}
+
+}  // namespace
+
 extern "C" {
 
 const char* rmi_last_error(void) { return g_last_error.c_str(); }
@@ -255,11 +432,10 @@ int rmi_dataset_create(const void* host_keys, uint64_t n, rmi_key_type key_type,
       const uint64_t i1 = std::min<uint64_t>(n, i0 + CH);
       e = cudaMemcpyAsync((char*)ds->d_keys + i0 * kb, (const char*)host_keys + i0 * kb, (i1 - i0) * kb,
                           cudaMemcpyHostToDevice, st);
-      switch (key_type) {
-        case RMI_KEY_U64: check_sorted<u64>(L, (const u64*)ds->d_keys, i1, i0, i1, d_flag); break;
-        case RMI_KEY_U32: check_sorted<u32>(L, (const u32*)ds->d_keys, i1, i0, i1, d_flag); break;
-        default: check_sorted<double>(L, (const double*)ds->d_keys, i1, i0, i1, d_flag); break;
-      }
+      with_key_type(key_type, [&](auto k) {
+        using T = decltype(k);
+        check_sorted<T>(L, (const T*)ds->d_keys, i1, i0, i1, d_flag);
+      });
     }
     if (e == cudaSuccess) e = cudaMemcpyAsync(&h_flag, d_flag, sizeof(unsigned), cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
@@ -499,21 +675,11 @@ int index_launch(const rmi_index* idx, const void* d_queries, uint64_t n, uint64
     CUDA_TRY(cudaGetLastError());
     return RMI_OK;
   }
-  switch (ds->key_type) {
-    case RMI_KEY_U64:
-      lookup_batch<u64>(L, idx->top, idx->leaf_kind, idx->d_records, idx->N, (const u64*)ds->d_keys, ds->n,
-                        (const u64*)d_queries, n, (u64*)d_out, (u64*)d_err, (u64*)d_fallbacks, lower_bound);
-      break;
-    case RMI_KEY_U32:
-      lookup_batch<u32>(L, idx->top, idx->leaf_kind, idx->d_records, idx->N, (const u32*)ds->d_keys, ds->n,
-                        (const u32*)d_queries, n, (u64*)d_out, (u64*)d_err, (u64*)d_fallbacks, lower_bound);
-      break;
-    default:
-      lookup_batch<double>(L, idx->top, idx->leaf_kind, idx->d_records, idx->N, (const double*)ds->d_keys, ds->n,
-                           (const double*)d_queries, n, (u64*)d_out, (u64*)d_err, (u64*)d_fallbacks,
-                           lower_bound);
-      break;
-  }
+  with_key_type(ds->key_type, [&](auto k) {
+    using T = decltype(k);
+    lookup_batch<T>(L, idx->top, idx->leaf_kind, idx->d_records, idx->N, (const T*)ds->d_keys, ds->n,
+                    (const T*)d_queries, n, (u64*)d_out, (u64*)d_err, (u64*)d_fallbacks, lower_bound);
+  });
   CUDA_TRY(cudaGetLastError());
   return RMI_OK;
 }
@@ -907,14 +1073,12 @@ int train_typed(const rmi_dataset* ds, const ModelName& top, const ModelName& le
   if (!bc) return fail(RMI_ERR_CUDA, "could not create the build's CUDA streams / events");
   cudaStream_t st = bc->st;
   cudaEvent_t ev0 = bc->ev0, ev1 = bc->ev1, *evp = bc->evp;
-  cudaStream_t side = bc->side;
-  cudaEvent_t ev_fork = bc->ev_fork, ev_join = bc->ev_join;
   int rc = RMI_OK;
   auto box = new ResultBox();
   {
     Arena A(st);
     Launch L{st, di.num_sms};
-    L.side = side; L.ev_fork = ev_fork; L.ev_join = ev_join;
+    L.side = bc->side; L.ev_fork = bc->ev_fork; L.ev_join = bc->ev_join;
     L.d_long = A.get<u32>(LONG_LEAF_CAP + 1);
     const int ppm = leaf_params_per_model(leaf.kind);
     TopModel* d_top = A.get<TopModel>(1);
@@ -928,39 +1092,18 @@ int train_typed(const rmi_dataset* ds, const ModelName& top, const ModelName& le
     // the key sample the top fit leaves for the boundary search (kernels.h); not with injected top parameters
     T* d_sample = !l0_over && top_fit_writes_sample(top.kind, (flags & RMI_FLAG_TOP_FIT_EXACT) != 0)
                       ? bounds_sample_at<T>(A.get<char>(bounds_sample_bytes(n, sizeof(T)))) : nullptr;
-    u32* d_table = nullptr;
-    u64 *d_pivots = nullptr, *d_ri = nullptr;
-    u64 hist_bins = 0, hist_ipb = 0;
-    if (top.kind == M_RADIX_TABLE) d_table = A.get<u32>((size_t)1 << top.table_bits);
-    if (top.kind == M_HISTOGRAM) {
-      histogram_bins(n, N, &hist_bins, &hist_ipb);
-      d_pivots = A.get<u64>(hist_bins + 1);
-      d_ri = A.get<u64>(((size_t)1 << 20) + 1);
-    }
+    TopTables tables;
+    tables.allocate(top, n, N, [&](size_t bytes) -> void* { return A.get<char>(bytes); });
     // pinned host buffers the results are copied into (and that the caller then reads)
     const bool stats_only = (flags & RMI_FLAG_STATS_ONLY) != 0;
-    bool host_ok = box->scalars.resize(sizeof(BuildAux) + sizeof(TopModel));
     const bool want_counts = !stats_only && (flags & RMI_FLAG_LEAF_COUNTS) != 0;
-    if (!stats_only) host_ok = host_ok && box->l1_params.resize((size_t)N * ppm) && box->l1_errors.resize(N);
-    if (want_counts) host_ok = host_ok && box->l1_counts.resize(N);
-    if (top.kind == M_RADIX_TABLE) host_ok = host_ok && box->table32.resize((size_t)1 << top.table_bits);
-    if (top.kind == M_HISTOGRAM) host_ok = host_ok && box->arr1.resize(((size_t)1 << 20) + 1) && box->arr2.resize(hist_bins);
+    const bool host_ok = reserve_result(box, &tables, N, ppm, !stats_only, want_counts);
     if (A.err != cudaSuccess) {
       rc = fail(RMI_ERR_CUDA, std::string("scratch allocation: ") + cudaGetErrorString(A.err));
     } else if (!host_ok) {
-      rc = fail(RMI_ERR_CUDA, "pinned host allocation for the results failed");
+      rc = fail(RMI_ERR_CUDA, kPinnedFailed);
     } else {
-      TopModel h_top;
-      memset(&h_top, 0, sizeof(h_top));
-      h_top.kind = top.kind;
-      h_top.high = 1;
-      h_top.table_bits = top.table_bits;
-      h_top.t32 = d_table;
-      h_top.pivots = d_pivots;
-      h_top.radix_index = d_ri;
-      h_top.npivots = hist_bins;
-      if (top.kind == M_HISTOGRAM) h_top.ip[0] = hist_bins;
-      if (l0_over) for (uint32_t q = 0; q < n_over && q < 4; ++q) h_top.f[q] = l0_over[q];
+      TopModel h_top = tables.initial(top, l0_over, n_over);
       cudaEventRecord(ev0, st);
       unsigned host_status = 0;
       bool exact = (flags & RMI_FLAG_TOP_FIT_EXACT) != 0;
@@ -975,8 +1118,8 @@ int train_typed(const rmi_dataset* ds, const ModelName& top, const ModelName& le
       cudaMemsetAsync(d_aux, 0, sizeof(BuildAux), st);
       bool leaf_results_copied = false;
       if (!l0_over && !host_top && rc == RMI_OK)
-        host_status |= fit_top_model<T>(L, keys, n, top.kind, top.table_bits, N, exact, d_top, d_aux, d_scratch, d_table,
-                                        d_pivots, d_ri, d_sample);
+        host_status |= fit_top_model<T>(L, keys, n, top.kind, top.table_bits, N, exact, d_top, d_aux, d_scratch, tables.t32,
+                                        tables.pivots, tables.radix_index, d_sample);
       cudaEventRecord(evp[0], st);
       if (host_status == 0 && rc == RMI_OK) {
         // injected top parameters are not known to be monotone: take the streaming pass, which checks
@@ -1004,76 +1147,24 @@ int train_typed(const rmi_dataset* ds, const ModelName& top, const ModelName& le
       }
       cudaEventRecord(ev1, st);
       // ---- results to the host --------------------------------------------------------------
-      BuildAux& h_aux = *reinterpret_cast<BuildAux*>(box->scalars.data());
-      TopModel& h_top_back = *reinterpret_cast<TopModel*>(box->scalars.data() + sizeof(BuildAux));
-      memset(&h_aux, 0, sizeof(h_aux));
-      cudaMemcpyAsync(&h_aux, d_aux, sizeof(h_aux), cudaMemcpyDeviceToHost, st);
-      cudaMemcpyAsync(&h_top_back, d_top, sizeof(h_top), cudaMemcpyDeviceToHost, st);
       leaf_copy_join(L);   // slice copies issued by fit_leaves
-      if (host_status == 0 && !stats_only && !leaf_results_copied) {
-        cudaMemcpyAsync(box->l1_params.data(), d_params, sizeof(double) * N * ppm, cudaMemcpyDeviceToHost, st);
-        cudaMemcpyAsync(box->l1_errors.data(), d_errors, sizeof(u64) * N, cudaMemcpyDeviceToHost, st);
-        if (want_counts) cudaMemcpyAsync(box->l1_counts.data(), d_counts, sizeof(u64) * N, cudaMemcpyDeviceToHost, st);
-      }
-      if (host_status == 0 && top.kind == M_RADIX_TABLE) {
-        cudaMemcpyAsync(box->table32.data(), d_table, sizeof(u32) * box->table32.size(), cudaMemcpyDeviceToHost, st);
-      }
-      if (host_status == 0 && top.kind == M_HISTOGRAM) {
-        cudaMemcpyAsync(box->arr1.data(), d_ri, sizeof(u64) * box->arr1.size(), cudaMemcpyDeviceToHost, st);
-        cudaMemcpyAsync(box->arr2.data(), d_pivots, sizeof(u64) * hist_bins, cudaMemcpyDeviceToHost, st);
-      }
+      const bool fitted = host_status == 0;
+      copy_result_to_host(box, fitted ? &tables : nullptr, d_aux, d_top,
+                          fitted && !stats_only && !leaf_results_copied ? d_params : nullptr, d_errors,
+                          want_counts ? d_counts : nullptr, st);
       cudaError_t e = cudaStreamSynchronize(st);
       if (rc != RMI_OK) {
         // (the exact top fit's key read-back failed: reported above)
       } else if (e != cudaSuccess) {
         rc = fail(RMI_ERR_CUDA, std::string("rmi_train: ") + cudaGetErrorString(e));
-      } else if (host_status | h_aux.status) {
-        rc = fail(RMI_ERR_PANIC, status_text(host_status | h_aux.status));
+      } else if (host_status | result_aux(box).status) {
+        rc = fail(RMI_ERR_PANIC, status_text(host_status | result_aux(box).status));
       } else {
+        fill_result(box, top, leaf, tables, n, N);
         rmi_result& R = box->pub;
-        memset(&R, 0, sizeof(R));
-        R.num_rmi_rows = n; R.num_data_rows = n; R.branching_factor = N;
-        // two_layer.rs:267-284
-        R.model_max_error = h_aux.max_error;
-        R.model_max_error_idx = h_aux.max_error_idx;
-        R.model_avg_error = (double)h_aux.sum_n_err / (double)n;
-        R.model_avg_l2_error = h_aux.sum_l2;
-        R.model_avg_log2_error = h_aux.sum_log2 / (double)n;
-        R.model_max_log2_error = std::log2((double)h_aux.max_error);
-        float ms = 0.f;
-        cudaEventElapsedTime(&ms, ev0, ev1);
-        R.device_time_ns = (uint64_t)((double)ms * 1e6);
+        R.device_time_ns = elapsed_ns(ev0, ev1);
         cudaEvent_t seq[5] = {ev0, evp[0], evp[1], evp[2], ev1};
-        for (int q = 0; q < 4; ++q) {
-          cudaEventElapsedTime(&ms, seq[q], seq[q + 1]);
-          R.phase_device_ns[q] = (uint64_t)((double)ms * 1e6);
-        }
-        R.l0_model_id = top.kind;
-        h_top = h_top_back;
-        R.l0_bradix_high = h_top.high;
-        R.l0_table_bits = top.table_bits;
-        switch (top.kind) {
-          case M_CUBIC: R.l0_num_fparams = 4; break;
-          case M_NORMAL: case M_LOGNORMAL: R.l0_num_fparams = 3; break;
-          case M_LINEAR: case M_ROBUST_LINEAR: case M_LINEAR_SPLINE: case M_LOGLINEAR: R.l0_num_fparams = 2; break;
-          case M_RADIX: R.l0_num_iparams = 2; break;
-          case M_BRADIX: R.l0_num_iparams = 3; break;
-          case M_RADIX_TABLE: R.l0_num_iparams = 1; break;   // prefix (the table itself is l0_table32)
-          case M_HISTOGRAM: R.l0_num_iparams = 1; break;
-        }
-        for (int q = 0; q < 4; ++q) { R.l0_fparams[q] = h_top.f[q]; R.l0_iparams[q] = h_top.ip[q]; }
-        R.l0_table32_len = box->table32.size();
-        R.l0_table32 = box->table32.empty() ? nullptr : box->table32.data();
-        R.l0_array1_len = box->arr1.size();
-        R.l0_array1 = box->arr1.empty() ? nullptr : box->arr1.data();
-        R.l0_array2_len = box->arr2.size();
-        R.l0_array2 = box->arr2.empty() ? nullptr : box->arr2.data();
-        R.l1_model_id = leaf.kind;
-        R.l1_params_per_model = ppm;
-        R.l1_params = stats_only ? nullptr : box->l1_params.data();
-        R.l1_errors = stats_only ? nullptr : box->l1_errors.data();
-        R.l1_counts = want_counts ? box->l1_counts.data() : nullptr;
-        R.could_not_replace = h_aux.could_not_replace ? 1 : 0;
+        for (int q = 0; q < 4; ++q) R.phase_device_ns[q] = elapsed_ns(seq[q], seq[q + 1]);
         R.top_fit_exact = (exact && !l0_over) ? 1 : 0;
       }
     }
@@ -1122,34 +1213,23 @@ int train_batch_typed(const rmi_dataset* ds, const ModelName& top, const std::ve
     void* d_stats = A.get<char>(stats_scratch_bytes(N));
     T* d_sample = top_fit_writes_sample(top.kind, (flags & RMI_FLAG_TOP_FIT_EXACT) != 0)
                       ? bounds_sample_at<T>(A.get<char>(bounds_sample_bytes(n, sizeof(T)))) : nullptr;
-    u32* d_table = nullptr;
-    u64 *d_pivots = nullptr, *d_ri = nullptr;
-    u64 hist_bins = 0, hist_ipb = 0;
-    if (top.kind == M_RADIX_TABLE) d_table = A.get<u32>((size_t)1 << top.table_bits);
-    if (top.kind == M_HISTOGRAM) {
-      histogram_bins(n, N, &hist_bins, &hist_ipb);
-      d_pivots = A.get<u64>(hist_bins + 1);
-      d_ri = A.get<u64>(((size_t)1 << 20) + 1);
-    }
+    TopTables tables;
+    tables.allocate(top, n, N, [&](size_t bytes) -> void* { return A.get<char>(bytes); });
     bool host_ok = true;
     for (size_t k = 0; k < K; ++k) {
       boxes[k] = new ResultBox();
-      host_ok = host_ok && boxes[k]->scalars.resize(sizeof(BuildAux) + sizeof(TopModel));
+      host_ok = host_ok && reserve_result(boxes[k], nullptr, N, 0, false, false);
     }
     if (A.err != cudaSuccess) rc = fail(RMI_ERR_CUDA, std::string("scratch allocation: ") + cudaGetErrorString(A.err));
-    else if (!host_ok) rc = fail(RMI_ERR_CUDA, "pinned host allocation for the results failed");
+    else if (!host_ok) rc = fail(RMI_ERR_CUDA, kPinnedFailed);
     else {
-      TopModel h_top;
-      memset(&h_top, 0, sizeof(h_top));
-      h_top.kind = top.kind; h_top.high = 1; h_top.table_bits = top.table_bits;
-      h_top.t32 = d_table; h_top.pivots = d_pivots; h_top.radix_index = d_ri; h_top.npivots = hist_bins;
-      if (top.kind == M_HISTOGRAM) h_top.ip[0] = hist_bins;
+      const TopModel h_top = tables.initial(top);
       cudaEventRecord(bc->ev0, st);
       cudaMemcpyAsync(d_top, &h_top, sizeof(h_top), cudaMemcpyHostToDevice, st);
       cudaMemsetAsync(d_aux0, 0, sizeof(BuildAux), st);
       const bool exact = (flags & RMI_FLAG_TOP_FIT_EXACT) != 0;
-      unsigned host_status = fit_top_model<T>(L, keys, n, top.kind, top.table_bits, N, exact, d_top, d_aux0, d_scratch, d_table,
-                                              d_pivots, d_ri, d_sample);
+      unsigned host_status = fit_top_model<T>(L, keys, n, top.kind, top.table_bits, N, exact, d_top, d_aux0, d_scratch,
+                                              tables.t32, tables.pivots, tables.radix_index, d_sample);
       if (host_status == 0) {
         compute_leaf_bounds<T>(L, keys, n, top.kind, d_top, N, d_S, d_aux0, /*allow_search=*/true, d_sample);
         Shard<T> whole = whole_array<T>(n);
@@ -1159,8 +1239,7 @@ int train_batch_typed(const rmi_dataset* ds, const ModelName& top, const std::ve
           cudaMemcpyAsync(d_aux, d_aux0, sizeof(BuildAux), cudaMemcpyDeviceToDevice, st);
           fit_leaves<T>(L, keys, whole, leaves[k]->kind, N, d_S, d_aux, d_params, d_errors, d_counts);
           leaf_statistics(L, n, N, d_errors, d_counts, d_aux, d_stats);
-          cudaMemcpyAsync(boxes[k]->scalars.data(), d_aux, sizeof(BuildAux), cudaMemcpyDeviceToHost, st);
-          cudaMemcpyAsync(boxes[k]->scalars.data() + sizeof(BuildAux), d_top, sizeof(TopModel), cudaMemcpyDeviceToHost, st);
+          copy_result_to_host(boxes[k], nullptr, d_aux, d_top, nullptr, nullptr, nullptr, st);
         }
       }
       cudaEventRecord(bc->ev1, st);
@@ -1171,40 +1250,12 @@ int train_batch_typed(const rmi_dataset* ds, const ModelName& top, const std::ve
         float ms = 0.f;
         cudaEventElapsedTime(&ms, bc->ev0, bc->ev1);
         for (size_t k = 0; k < K && rc == RMI_OK; ++k) {
-          const BuildAux& h_aux = *reinterpret_cast<const BuildAux*>(boxes[k]->scalars.data());
-          const TopModel& tb = *reinterpret_cast<const TopModel*>(boxes[k]->scalars.data() + sizeof(BuildAux));
-          if (h_aux.status) { rc = fail(RMI_ERR_PANIC, std::string(top.name) + "," + leaves[k]->name + ": " + status_text(h_aux.status)); break; }
-          rmi_result& R = boxes[k]->pub;
-          memset(&R, 0, sizeof(R));
-          R.num_rmi_rows = n; R.num_data_rows = n; R.branching_factor = N;
-          R.model_max_error = h_aux.max_error;
-          R.model_max_error_idx = h_aux.max_error_idx;
-          R.model_avg_error = (double)h_aux.sum_n_err / (double)n;
-          R.model_avg_l2_error = h_aux.sum_l2;
-          R.model_avg_log2_error = h_aux.sum_log2 / (double)n;
-          R.model_max_log2_error = std::log2((double)h_aux.max_error);
-          R.device_time_ns = (uint64_t)((double)ms * 1e6 / (double)K);   // the batch's device time, shared out evenly
-          R.l0_model_id = top.kind;
-          R.l0_bradix_high = tb.high;
-          R.l0_table_bits = top.table_bits;
-          switch (top.kind) {
-            case M_CUBIC: R.l0_num_fparams = 4; break;
-            case M_NORMAL: case M_LOGNORMAL: R.l0_num_fparams = 3; break;
-            case M_LINEAR: case M_ROBUST_LINEAR: case M_LINEAR_SPLINE: case M_LOGLINEAR: R.l0_num_fparams = 2; break;
-            case M_RADIX: R.l0_num_iparams = 2; break;
-            case M_BRADIX: R.l0_num_iparams = 3; break;
-            case M_RADIX_TABLE: R.l0_num_iparams = 1; break;
-            case M_HISTOGRAM: R.l0_num_iparams = 1; break;
-          }
-          for (int q = 0; q < 4; ++q) { R.l0_fparams[q] = tb.f[q]; R.l0_iparams[q] = tb.ip[q]; }
-          // sizes of the top model's tables (rmi_model_size needs them; the tables themselves stay on the device)
-          R.l0_table32_len = top.kind == M_RADIX_TABLE ? ((uint64_t)1 << top.table_bits) : 0;
-          R.l0_array1_len = top.kind == M_HISTOGRAM ? (((uint64_t)1 << 20) + 1) : 0;
-          R.l0_array2_len = top.kind == M_HISTOGRAM ? hist_bins : 0;
-          R.l1_model_id = leaves[k]->kind;
-          R.l1_params_per_model = leaf_params_per_model(leaves[k]->kind);
-          R.could_not_replace = h_aux.could_not_replace ? 1 : 0;
-          R.top_fit_exact = exact ? 1 : 0;
+          const unsigned status = result_aux(boxes[k]).status;
+          if (status) { rc = fail(RMI_ERR_PANIC, std::string(top.name) + "," + leaves[k]->name + ": " + status_text(status)); break; }
+          // the top tables stay on the device: the result holds their lengths (rmi_model_size) without them
+          fill_result(boxes[k], top, *leaves[k], tables, n, N);
+          boxes[k]->pub.device_time_ns = (uint64_t)((double)ms * 1e6 / (double)K);   // the batch's device time, shared out evenly
+          boxes[k]->pub.top_fit_exact = exact ? 1 : 0;
         }
       }
     }
@@ -1220,48 +1271,14 @@ int train_entry(const rmi_dataset* ds, const char* model_spec, uint64_t N, uint3
                 uint32_t n_over, rmi_result** out) {
   g_last_error.clear();
   if (!ds || !model_spec || !out) return fail(RMI_ERR_INVALID, "rmi_train: null argument");
-  // train/mod.rs:104-109: split the spec on ',', validate, last = leaf type
-  std::vector<std::string> layers;
-  {
-    std::string s(model_spec);
-    size_t pos = 0;
-    for (;;) {
-      size_t c = s.find(',', pos);
-      if (c == std::string::npos) { layers.push_back(s.substr(pos)); break; }
-      layers.push_back(s.substr(pos, c - pos));
-      pos = c + 1;
-    }
-  }
-  std::vector<const ModelName*> models;
-  for (size_t i = 0; i < layers.size(); ++i) {
-    const ModelName* m = find_model(layers[i]);
-    if (!m) return fail(RMI_ERR_PANIC, "Unknown model type: " + layers[i]);
-    // train/mod.rs:59-85 validate: radix / bradix / histogram must be the root model
-    bool must_be_top = m->kind == M_RADIX || m->kind == M_BRADIX || m->kind == M_HISTOGRAM;
-    if (must_be_top && i != 0)
-      return fail(RMI_ERR_PANIC, "if used, model type " + layers[i] + " must be the root model");
-    models.push_back(m);
-  }
-  if (models.size() != 2)   // train/mod.rs:123-125 panic!() for anything but two layers
-    return fail(RMI_ERR_PANIC, "only two-layer RMIs can be trained (the reference panics on other depths)");
-  const ModelName& top = *models[0];
-  const ModelName& leaf = *models[1];
-  if (leaf.kind == M_RADIX_TABLE)
-    return fail(RMI_ERR_UNSUPPORTED, "radix tables are only offered as the top model in this build");
-  if (N < 1) return fail(RMI_ERR_PANIC, "branching factor must be at least 1");
-  if (ds->n == 0) return fail(RMI_ERR_PANIC, "start index was 0 but end index was 0");
-  if (!ds->sorted) return fail(RMI_ERR_PANIC, "keys are not sorted in ascending order");
-  if (l0_over) {
-    uint32_t need = top.kind == M_CUBIC ? 4 : (top.kind == M_NORMAL || top.kind == M_LOGNORMAL) ? 3 : 2;
-    if (top.kind > M_LOGNORMAL || n_over != need)
-      return fail(RMI_ERR_INVALID, "rmi_train_with_top: top model has no float parameters or wrong count");
-  }
-  switch (ds->key_type) {
-    case RMI_KEY_U64: return train_typed<u64>(ds, top, leaf, N, flags, l0_over, n_over, out);
-    case RMI_KEY_U32: return train_typed<u32>(ds, top, leaf, N, flags, l0_over, n_over, out);
-    case RMI_KEY_F64: return train_typed<double>(ds, top, leaf, N, flags, l0_over, n_over, out);
-  }
-  return fail(RMI_ERR_INVALID, "bad key type");
+  const ModelName *top = nullptr, *leaf = nullptr;
+  if (int rc = parse_two_layer(model_spec, &top, &leaf)) return rc;
+  if (int rc = check_build(ds->n, N, ds->sorted)) return rc;
+  if (l0_over && (top->fparams == 0 || n_over != (uint32_t)top->fparams))
+    return fail(RMI_ERR_INVALID, "rmi_train_with_top: top model has no float parameters or wrong count");
+  return with_key_type(ds->key_type, [&](auto k) {
+    return train_typed<decltype(k)>(ds, *top, *leaf, N, flags, l0_over, n_over, out);
+  });
 }
 
 }  // namespace
@@ -1282,26 +1299,17 @@ int rmi_train_stats_batch(const rmi_dataset* ds, const char* top_model, const ch
                           uint64_t branch_factor, uint32_t flags, rmi_result** out) {
   g_last_error.clear();
   if (!ds || !top_model || !leaf_models || num_leaf_models < 1 || !out) return fail(RMI_ERR_INVALID, "rmi_train_stats_batch: bad argument");
-  const ModelName* top = find_model(top_model);
-  if (!top) return fail(RMI_ERR_PANIC, std::string("Unknown model type: ") + top_model);
-  std::vector<const ModelName*> leaves;
+  const ModelName* top = nullptr;
+  if (int rc = find_layer(top_model, true, &top)) return rc;
+  std::vector<const ModelName*> leaves(num_leaf_models);
   for (int k = 0; k < num_leaf_models; ++k) {
-    const ModelName* m = leaf_models[k] ? find_model(leaf_models[k]) : nullptr;
-    if (!m) return fail(RMI_ERR_PANIC, std::string("Unknown model type: ") + (leaf_models[k] ? leaf_models[k] : "(null)"));
-    if (m->kind == M_RADIX || m->kind == M_BRADIX || m->kind == M_HISTOGRAM)   // train/mod.rs:59-85
-      return fail(RMI_ERR_PANIC, std::string("if used, model type ") + m->name + " must be the root model");
-    if (m->kind == M_RADIX_TABLE) return fail(RMI_ERR_UNSUPPORTED, "radix tables are only offered as the top model in this build");
-    leaves.push_back(m);
+    if (int rc = find_layer(leaf_models[k] ? leaf_models[k] : "(null)", false, &leaves[k])) return rc;
+    if (int rc = check_leaf(leaves[k])) return rc;
   }
-  if (branch_factor < 1) return fail(RMI_ERR_PANIC, "branching factor must be at least 1");
-  if (ds->n == 0) return fail(RMI_ERR_PANIC, "start index was 0 but end index was 0");
-  if (!ds->sorted) return fail(RMI_ERR_PANIC, "keys are not sorted in ascending order");
-  switch (ds->key_type) {
-    case RMI_KEY_U64: return train_batch_typed<u64>(ds, *top, leaves, branch_factor, flags, out);
-    case RMI_KEY_U32: return train_batch_typed<u32>(ds, *top, leaves, branch_factor, flags, out);
-    case RMI_KEY_F64: return train_batch_typed<double>(ds, *top, leaves, branch_factor, flags, out);
-  }
-  return fail(RMI_ERR_INVALID, "bad key type");
+  if (int rc = check_build(ds->n, branch_factor, ds->sorted)) return rc;
+  return with_key_type(ds->key_type, [&](auto k) {
+    return train_batch_typed<decltype(k)>(ds, *top, leaves, branch_factor, flags, out);
+  });
 }
 int rmi_train_with_top(const rmi_dataset* ds, const char* model_spec, uint64_t branch_factor, uint32_t flags,
                        const double* l0_fparams, uint32_t n_fparams, rmi_result** out) {
@@ -1437,10 +1445,7 @@ struct rmi_shard_build {
   const LeafCopyOut* leaf_copy = nullptr;   // rmi_shard_train with a shared result region: sliced launch of the owned leaf window,
   u64 leaf_lo = 0, leaf_hi = 0;             //   each slice's records copied to the host while the next slice computes
   // table tops (radix8..28, histogram): the table every rank fills its part of, merged by an all-reduce MAX
-  u32* d_table32 = nullptr;             // 2^table_bits hints
-  u64* d_pivots = nullptr;              // hist_bins + 1
-  u64* d_ri = nullptr;                  // 2^20 + 1
-  u64 hist_bins = 0, hist_ipb = 0;
+  TopTables tables;
   cudaEvent_t ev_off = nullptr, ev_t0 = nullptr, ev_t1 = nullptr, ev_leaf0 = nullptr, ev_leaf1 = nullptr;
 };
 
@@ -1526,24 +1531,20 @@ template <class T> int shard_phase_typed(rmi_shard_build* b, int phase) {
     for (int q = 1; q < RMI_NUM_PHASES; ++q) b->ran[q] = false;
   }
   const T first_key = key_from_bits<T>(b->info.first_key_bits), last_key = key_from_bits<T>(b->info.last_key_bits);
+  const TopTables& tt = b->tables;
   switch (phase) {
     case RMI_PHASE_TOP_LOCAL:
       cudaMemsetAsync(b->d_aux, 0, sizeof(BuildAux), b->st);
       {
-        TopModel h;
-        memset(&h, 0, sizeof(h));
-        h.kind = b->top->kind; h.high = 1;
-        h.table_bits = b->top->table_bits;
-        h.t32 = b->d_table32; h.pivots = b->d_pivots; h.radix_index = b->d_ri; h.npivots = b->hist_bins;
-        if (b->top->kind == M_HISTOGRAM) h.ip[0] = b->hist_bins;
+        const TopModel h = tt.initial(*b->top);
         cudaMemcpyAsync(b->d_top, &h, sizeof(h), cudaMemcpyHostToDevice, b->st);
       }
-      if (b->top->kind == M_HISTOGRAM && (b->hist_bins == 0 || b->hist_ipb < 1)) b->host_status |= ST_HIST_BINS;   // histogram.rs:25-27
+      if (b->top->kind == M_HISTOGRAM && (tt.hist_bins == 0 || tt.hist_ipb < 1)) b->host_status |= ST_HIST_BINS;   // histogram.rs:25-27
       b->host_status |= shard_top_local<T>(L, keys, sh, b->top->kind, b->N, b->info.pivot_x, b->info.pivot_y, first_key,
                                            last_key, b->d_scratch, (double*)b->buf.sums);
       if ((b->top->kind == M_RADIX_TABLE || b->top->kind == M_HISTOGRAM) && b->host_status == 0)
-        shard_table_local<T>(L, keys, sh, b->top->kind, b->top->table_bits, b->N, first_key, last_key, b->d_aux, b->d_table32,
-                             b->d_pivots, b->hist_bins, b->hist_ipb);
+        shard_table_local<T>(L, keys, sh, b->top->kind, b->top->table_bits, b->N, first_key, last_key, b->d_aux, tt.t32,
+                             tt.pivots, tt.hist_bins, tt.hist_ipb);
       break;
     case RMI_PHASE_TOP_MID:
       shard_top_mid<T>(L, keys, sh, b->top->kind, b->N, first_key, last_key, b->d_scratch, (double*)b->buf.sums, b->d_aux);
@@ -1551,8 +1552,8 @@ template <class T> int shard_phase_typed(rmi_shard_build* b, int phase) {
     case RMI_PHASE_TOP_FINISH:
       shard_top_finish<T>(L, sh, b->top->kind, b->N, b->info.pivot_x, b->info.pivot_y, (const double*)b->buf.sums,
                           first_key, last_key, b->info.last_F, b->d_scratch, b->d_top, b->d_aux);
-      if (b->top->kind == M_RADIX_TABLE && b->host_status == 0) shard_table_decode(L, b->top->table_bits, b->d_table32);
-      if (b->top->kind == M_HISTOGRAM && b->host_status == 0) hist_radix_index(L, b->d_pivots, b->hist_bins, b->d_ri);
+      if (b->top->kind == M_RADIX_TABLE && b->host_status == 0) shard_table_decode(L, b->top->table_bits, tt.t32);
+      if (b->top->kind == M_HISTOGRAM && b->host_status == 0) hist_radix_index(L, tt.pivots, tt.hist_bins, tt.radix_index);
       break;
     case RMI_PHASE_BOUNDS:
       shard_bounds<T>(L, keys, sh, b->top->kind, b->d_top, b->N, (u64*)b->buf.S, b->d_aux);
@@ -1595,25 +1596,13 @@ uint32_t rmi_params_per_model(const char* leaf_model_name) {
 
 int rmi_shard_top_rounds(const char* top_model_name) {
   const ModelName* m = top_model_name ? find_model(top_model_name) : nullptr;
-  if (!m) return -1;
-  switch (m->kind) {
-    case M_LINEAR_SPLINE: case M_RADIX: return 0;
-    case M_LINEAR: case M_ROBUST_LINEAR: return 1;
-    case M_NORMAL: case M_LOGNORMAL: return 2;
-    case M_CUBIC: return 3;
-    case M_RADIX_TABLE: case M_HISTOGRAM: return 4;
-    default: return -1;
-  }
+  return m ? m->shard_rounds : -1;
 }
 
 int rmi_shard_ends_get(const rmi_dataset* ds, rmi_shard_ends* out) {
   if (!ds || !out) return fail(RMI_ERR_INVALID, "rmi_shard_ends_get: null argument");
   CUDA_TRY(cudaSetDevice(ds->device));
-  switch (ds->key_type) {
-    case RMI_KEY_U64: return shard_ends_typed<u64>(ds, out);
-    case RMI_KEY_U32: return shard_ends_typed<u32>(ds, out);
-    default: return shard_ends_typed<double>(ds, out);
-  }
+  return with_key_type(ds->key_type, [&](auto k) { return shard_ends_typed<decltype(k)>(ds, out); });
 }
 
 int rmi_shard_build_create(const rmi_dataset* local, const rmi_shard_info* info, const char* model_spec,
@@ -1621,23 +1610,12 @@ int rmi_shard_build_create(const rmi_dataset* local, const rmi_shard_info* info,
                            rmi_shard_build** out) {
   g_last_error.clear();
   if (!local || !info || !model_spec || !buffers || !out) return fail(RMI_ERR_INVALID, "rmi_shard_build_create: null argument");
-  std::string s(model_spec);
-  size_t c = s.find(',');
-  if (c == std::string::npos || s.find(',', c + 1) != std::string::npos)
-    return fail(RMI_ERR_PANIC, "only two-layer RMIs can be trained (the reference panics on other depths)");
-  const ModelName* top = find_model(s.substr(0, c));
-  const ModelName* leaf = find_model(s.substr(c + 1));
-  if (!top) return fail(RMI_ERR_PANIC, "Unknown model type: " + s.substr(0, c));
-  if (!leaf) return fail(RMI_ERR_PANIC, "Unknown model type: " + s.substr(c + 1));
-  if (leaf->kind == M_RADIX || leaf->kind == M_BRADIX || leaf->kind == M_HISTOGRAM)
-    return fail(RMI_ERR_PANIC, "if used, model type " + s.substr(c + 1) + " must be the root model");
-  if (rmi_shard_top_rounds(top->name) < 0)
+  const ModelName *top = nullptr, *leaf = nullptr;
+  if (int rc = parse_two_layer(model_spec, &top, &leaf)) return rc;
+  if (top->shard_rounds < 0)
     return fail(RMI_ERR_UNSUPPORTED, "range-partitioned builds offer the top models linear, robust_linear, linear_spline, "
                                      "cubic, normal, lognormal, radix, radix8..28, histogram");
-  if (leaf->kind == M_RADIX_TABLE) return fail(RMI_ERR_UNSUPPORTED, "radix tables are only offered as the top model");
-  if (branch_factor < 1) return fail(RMI_ERR_PANIC, "branching factor must be at least 1");
-  if (info->n_global == 0) return fail(RMI_ERR_PANIC, "start index was 0 but end index was 0");
-  if (!local->sorted) return fail(RMI_ERR_PANIC, "keys are not sorted in ascending order");
+  if (int rc = check_build(info->n_global, branch_factor, local->sorted)) return rc;
   CUDA_TRY(cudaSetDevice(local->device));
   DeviceInfo di;
   if (int rc = device_info(local->device, &di)) return rc;
@@ -1657,12 +1635,10 @@ int rmi_shard_build_create(const rmi_dataset* local, const rmi_shard_info* info,
          cudaEventCreateWithFlags(&b->ev_join, cudaEventDisableTiming) == cudaSuccess &&
          cudaMalloc((void**)&b->d_long, sizeof(u32) * (LONG_LEAF_CAP + 1)) == cudaSuccess;
   }
-  if (ok && top->kind == M_RADIX_TABLE) ok = cudaMalloc((void**)&b->d_table32, sizeof(u32) << top->table_bits) == cudaSuccess;
-  if (ok && top->kind == M_HISTOGRAM) {
-    histogram_bins(info->n_global, branch_factor, &b->hist_bins, &b->hist_ipb);
-    ok = cudaMalloc((void**)&b->d_pivots, sizeof(u64) * (b->hist_bins + 1)) == cudaSuccess &&
-         cudaMalloc((void**)&b->d_ri, sizeof(u64) * (((size_t)1 << 20) + 1)) == cudaSuccess;
-  }
+  ok = ok && b->tables.allocate(*top, info->n_global, branch_factor, [](size_t bytes) -> void* {
+    void* p = nullptr;
+    return cudaMalloc(&p, bytes) == cudaSuccess ? p : nullptr;
+  });
   if (!ok) { rmi_shard_build_destroy(b); return fail(RMI_ERR_CUDA, "rmi_shard_build_create: device allocation failed"); }
   *out = b;
   return RMI_OK;
@@ -1670,8 +1646,9 @@ int rmi_shard_build_create(const rmi_dataset* local, const rmi_shard_info* info,
 
 int rmi_shard_top_table(rmi_shard_build* b, void** device_ptr, uint64_t* count, int* elem_bytes) {
   if (!b || !device_ptr || !count || !elem_bytes) return fail(RMI_ERR_INVALID, "rmi_shard_top_table: null argument");
-  if (b->top->kind == M_RADIX_TABLE) { *device_ptr = b->d_table32; *count = (uint64_t)1 << b->top->table_bits; *elem_bytes = 4; return RMI_OK; }
-  if (b->top->kind == M_HISTOGRAM) { *device_ptr = b->d_pivots; *count = b->hist_bins; *elem_bytes = 8; return RMI_OK; }
+  const TopTables& tt = b->tables;
+  if (tt.t32) { *device_ptr = tt.t32; *count = tt.t32_len; *elem_bytes = 4; return RMI_OK; }
+  if (tt.pivots) { *device_ptr = tt.pivots; *count = tt.hist_bins; *elem_bytes = 8; return RMI_OK; }
   *device_ptr = nullptr; *count = 0; *elem_bytes = 0;
   return RMI_OK;
 }
@@ -1680,11 +1657,7 @@ int rmi_shard_phase(rmi_shard_build* b, int phase) {
   if (!b) return fail(RMI_ERR_INVALID, "rmi_shard_phase: null build");
   b->gather_mode = false;   // host-driven flow: the caller combines the leaf records with an all-reduce SUM of zero-filled arrays
   CUDA_TRY(cudaSetDevice(b->ds->device));
-  switch (b->ds->key_type) {
-    case RMI_KEY_U64: return shard_phase_typed<u64>(b, phase);
-    case RMI_KEY_U32: return shard_phase_typed<u32>(b, phase);
-    default: return shard_phase_typed<double>(b, phase);
-  }
+  return with_key_type(b->ds->key_type, [&](auto k) { return shard_phase_typed<decltype(k)>(b, phase); });
 }
 
 int rmi_shard_set_halo(rmi_shard_build* b, uint64_t halo_keys) {
@@ -1696,59 +1669,26 @@ int rmi_shard_set_halo(rmi_shard_build* b, uint64_t halo_keys) {
 
 }  // extern "C"
 
-// Fills the public result from the scalars / tables already copied into `box` (after the stream has been
-// synchronised).  st_all: OR of every rank's status word; cnr: some rank could not replace an empty leaf.
-static int shard_fill_result(rmi_shard_build* b, ResultBox* box, uint32_t flags, unsigned st_all, bool cnr, bool have_leaves,
-                             const uint64_t* total_device_ns, rmi_result** out) {
-  const uint64_t N = b->N, n = b->info.n_global;
-  const int ppm = leaf_params_per_model(b->leaf->kind);
-  const bool stats_only = (flags & RMI_FLAG_STATS_ONLY) != 0 || !have_leaves;
-  const bool want_counts = !stats_only && (flags & RMI_FLAG_LEAF_COUNTS) != 0;
-  BuildAux& h_aux = *reinterpret_cast<BuildAux*>(box->scalars.data());
-  TopModel& h_top = *reinterpret_cast<TopModel*>(box->scalars.data() + sizeof(BuildAux));
+// The public result from what copy_result_to_host brought back (after the stream has been synchronised).
+// st_all: OR of every rank's status word; cnr: some rank could not replace an empty leaf.
+static int shard_result(rmi_shard_build* b, ResultBox* box, unsigned st_all, bool cnr, const uint64_t* total_device_ns,
+                        rmi_result** out) {
   if (st_all) {
-    std::string msg = status_text((b->host_status | h_aux.status | st_all) & ~ST_HALO_TOO_SMALL);
+    std::string msg = status_text((b->host_status | result_aux(box).status | st_all) & ~ST_HALO_TOO_SMALL);
     if (st_all & ST_HALO_TOO_SMALL) msg += (msg.empty() ? "" : "; ") + std::string("a leaf reaches past the halo copied from the next rank");
     if (msg.empty()) msg = "another rank reported a failure";
     delete box;
     return fail(RMI_ERR_PANIC, msg);
   }
+  fill_result(box, *b->top, *b->leaf, b->tables, b->info.n_global, b->N);
   rmi_result& R = box->pub;
-  memset(&R, 0, sizeof(R));
-  R.num_rmi_rows = n; R.num_data_rows = n; R.branching_factor = N;
-  R.model_max_error = h_aux.max_error;
-  R.model_max_error_idx = h_aux.max_error_idx;
-  R.model_avg_error = (double)h_aux.sum_n_err / (double)n;
-  R.model_avg_l2_error = h_aux.sum_l2;
-  R.model_avg_log2_error = h_aux.sum_log2 / (double)n;
-  R.model_max_log2_error = std::log2((double)h_aux.max_error);
-  R.l0_model_id = b->top->kind;
-  R.l0_bradix_high = 1;
-  R.l0_table_bits = b->top->table_bits;
-  if (b->top->kind == M_RADIX) R.l0_num_iparams = 2;
-  else if (b->top->kind == M_RADIX_TABLE || b->top->kind == M_HISTOGRAM) R.l0_num_iparams = 1;
-  else R.l0_num_fparams = b->top->kind == M_CUBIC ? 4 : ((b->top->kind == M_NORMAL || b->top->kind == M_LOGNORMAL) ? 3 : 2);
-  R.l0_table32_len = box->table32.size();
-  R.l0_table32 = box->table32.empty() ? nullptr : box->table32.data();
-  R.l0_array1_len = box->arr1.size();
-  R.l0_array1 = box->arr1.empty() ? nullptr : box->arr1.data();
-  R.l0_array2_len = box->arr2.size();
-  R.l0_array2 = box->arr2.empty() ? nullptr : box->arr2.data();
-  for (int q = 0; q < 4; ++q) { R.l0_fparams[q] = h_top.f[q]; R.l0_iparams[q] = h_top.ip[q]; }
-  R.l1_model_id = b->leaf->kind;
-  R.l1_params_per_model = ppm;
-  R.l1_params = stats_only ? nullptr : box->l1_params.data();
-  R.l1_errors = stats_only ? nullptr : box->l1_errors.data();
-  R.l1_counts = want_counts ? box->l1_counts.data() : nullptr;
   {   // device time of this rank's phases (collectives between them are not included)
     const int map[RMI_NUM_PHASES] = {0, 0, 1, 1, 2, 3, 0};
     for (int q = 0; q < RMI_NUM_PHASES; ++q) {
       if (!b->ran[q]) continue;
-      float ms = 0.f;
-      if (cudaEventElapsedTime(&ms, b->ev_begin[q], b->ev_end[q]) == cudaSuccess) {
-        R.phase_device_ns[map[q]] += (uint64_t)((double)ms * 1e6);
-        R.device_time_ns += (uint64_t)((double)ms * 1e6);
-      }
+      const uint64_t ns = elapsed_ns(b->ev_begin[q], b->ev_end[q]);
+      R.phase_device_ns[map[q]] += ns;
+      R.device_time_ns += ns;
     }
   }
   if (total_device_ns) R.device_time_ns = *total_device_ns;   // whole build on the stream, collectives included
@@ -1763,37 +1703,22 @@ extern "C" {
 int rmi_shard_finish(rmi_shard_build* b, uint32_t flags, rmi_result** out) {
   if (!b || !out) return fail(RMI_ERR_INVALID, "rmi_shard_finish: null argument");
   CUDA_TRY(cudaSetDevice(b->ds->device));
-  const uint64_t N = b->N;
-  const int ppm = leaf_params_per_model(b->leaf->kind);
   const bool stats_only = (flags & RMI_FLAG_STATS_ONLY) != 0;
-  auto box = new ResultBox();
-  bool host_ok = box->scalars.resize(sizeof(BuildAux) + sizeof(TopModel));
   const bool want_counts = !stats_only && (flags & RMI_FLAG_LEAF_COUNTS) != 0;
-  if (!stats_only) host_ok = host_ok && box->l1_params.resize((size_t)N * ppm) && box->l1_errors.resize(N);
-  if (want_counts) host_ok = host_ok && box->l1_counts.resize(N);
-  if (!host_ok) { delete box; return fail(RMI_ERR_CUDA, "pinned host allocation for the results failed"); }
-  BuildAux& h_aux = *reinterpret_cast<BuildAux*>(box->scalars.data());
-  TopModel& h_top = *reinterpret_cast<TopModel*>(box->scalars.data() + sizeof(BuildAux));
+  auto box = new ResultBox();
+  if (!reserve_result(box, &b->tables, b->N, leaf_params_per_model(b->leaf->kind), !stats_only, want_counts)) {
+    delete box;
+    return fail(RMI_ERR_CUDA, kPinnedFailed);
+  }
+  copy_result_to_host(box, &b->tables, b->d_aux, b->d_top, stats_only ? nullptr : (const double*)b->buf.params,
+                      (const u64*)b->buf.errors, want_counts ? (const u64*)b->buf.counts : nullptr, b->st);
   unsigned h_status = 0;
-  cudaMemcpyAsync(&h_aux, b->d_aux, sizeof(BuildAux), cudaMemcpyDeviceToHost, b->st);
-  cudaMemcpyAsync(&h_top, b->d_top, sizeof(TopModel), cudaMemcpyDeviceToHost, b->st);
-  if (b->top->kind == M_RADIX_TABLE && box->table32.resize((size_t)1 << b->top->table_bits))
-    cudaMemcpyAsync(box->table32.data(), b->d_table32, sizeof(u32) << b->top->table_bits, cudaMemcpyDeviceToHost, b->st);
-  if (b->top->kind == M_HISTOGRAM && box->arr1.resize(((size_t)1 << 20) + 1) && box->arr2.resize(b->hist_bins)) {
-    cudaMemcpyAsync(box->arr1.data(), b->d_ri, sizeof(u64) * box->arr1.size(), cudaMemcpyDeviceToHost, b->st);
-    cudaMemcpyAsync(box->arr2.data(), b->d_pivots, sizeof(u64) * b->hist_bins, cudaMemcpyDeviceToHost, b->st);
-  }
-  if (!stats_only) {
-    cudaMemcpyAsync(box->l1_params.data(), b->buf.params, sizeof(double) * N * ppm, cudaMemcpyDeviceToHost, b->st);
-    cudaMemcpyAsync(box->l1_errors.data(), b->buf.errors, sizeof(u64) * N, cudaMemcpyDeviceToHost, b->st);
-    if (want_counts) cudaMemcpyAsync(box->l1_counts.data(), b->buf.counts, sizeof(u64) * N, cudaMemcpyDeviceToHost, b->st);
-  }
   cudaError_t e = cudaStreamSynchronize(b->st);
   if (e == cudaSuccess) e = cudaMemcpy(&h_status, b->buf.status, sizeof(unsigned), cudaMemcpyDeviceToHost);
   if (e != cudaSuccess) { delete box; return fail(RMI_ERR_CUDA, std::string("rmi_shard_finish: ") + cudaGetErrorString(e)); }
   // host-driven flow: buffers.status holds whatever the caller combined over the ranks (sharded.py: a bitwise OR)
-  unsigned st_all = b->host_status | h_aux.status | h_status;
-  return shard_fill_result(b, box, flags, st_all, h_aux.could_not_replace != 0, true, nullptr, out);
+  const BuildAux& h_aux = result_aux(box);
+  return shard_result(b, box, b->host_status | h_aux.status | h_status, h_aux.could_not_replace != 0, nullptr, out);
 }
 
 // ---- the whole range-partitioned build in one call, collectives issued on the build's stream ----------
@@ -1987,10 +1912,7 @@ static int shard_train_typed(rmi_shard_build* b, rmi_shard_comm* c, uint32_t fla
   double* sums = (double*)b->buf.sums;
   // pinned host memory for the results first (nothing below waits for the host except the owner offsets)
   auto box = new ResultBox();
-  bool host_ok = box->scalars.resize(sizeof(BuildAux) + sizeof(TopModel));
-  if (leaves_to_host) host_ok = host_ok && box->l1_params.resize((size_t)N * ppm) && box->l1_errors.resize(N);
-  if (leaves_to_host && want_counts) host_ok = host_ok && box->l1_counts.resize(N);
-  if (!host_ok) { delete box; return fail(RMI_ERR_CUDA, "pinned host allocation for the results failed"); }
+  if (!reserve_result(box, &b->tables, N, ppm, leaves_to_host, want_counts)) { delete box; return fail(RMI_ERR_CUDA, kPinnedFailed); }
   b->gather_mode = true;
   int rc = RMI_OK;
   auto phase = [&](int ph) { if (rc == RMI_OK) rc = shard_phase_typed<T>(b, ph); };
@@ -2013,15 +1935,16 @@ static int shard_train_typed(rmi_shard_build* b, rmi_shard_comm* c, uint32_t fla
   // ---- top model: local part, 0-2 tiny all-reduces, closed form (identical on every rank) -----------------
   phase(RMI_PHASE_TOP_LOCAL);
   mark("top local");
-  const int rounds = rmi_shard_top_rounds(b->top->name);
+  const int rounds = b->top->shard_rounds;
   if (W > 1 && rc == RMI_OK) {
     if (rounds == 1 || rounds == 2) nccl(nc.AllReduce(sums, sums, 8, ncclFloat64, ncclSum, comm, st), "ncclAllReduce(top sums)");
     if (rounds == 3) nccl(nc.AllReduce(sums + 8, sums + 8, 4, ncclInt64, ncclMin, comm, st), "ncclAllReduce(cubic interior points)");
     if (rounds == 4 && b->host_status == 0) {   // table tops: merge the ranks' partial tables (one writer per entry, zero elsewhere)
+      const TopTables& tt = b->tables;
       if (b->top->kind == M_RADIX_TABLE)
-        nccl(nc.AllReduce(b->d_table32, b->d_table32, (size_t)1 << b->top->table_bits, ncclUint32, ncclMax, comm, st), "ncclAllReduce(radix table)");
+        nccl(nc.AllReduce(tt.t32, tt.t32, tt.t32_len, ncclUint32, ncclMax, comm, st), "ncclAllReduce(radix table)");
       else
-        nccl(nc.AllReduce(b->d_pivots, b->d_pivots, b->hist_bins, ncclUint64, ncclMax, comm, st), "ncclAllReduce(histogram pivots)");
+        nccl(nc.AllReduce(tt.pivots, tt.pivots, tt.hist_bins, ncclUint64, ncclMax, comm, st), "ncclAllReduce(histogram pivots)");
     }
   }
   if (rounds >= 2) {
@@ -2128,22 +2051,9 @@ static int shard_train_typed(rmi_shard_build* b, rmi_shard_comm* c, uint32_t fla
   cudaEventRecord(b->ev_t1, st);
   if (rc != RMI_OK) { cudaStreamSynchronize(st); delete box; return rc; }
   // ---- results to the host ------------------------------------------------------------------------------------
-  BuildAux& h_aux = *reinterpret_cast<BuildAux*>(box->scalars.data());
-  TopModel& h_top = *reinterpret_cast<TopModel*>(box->scalars.data() + sizeof(BuildAux));
-  cudaMemcpyAsync(&h_aux, b->d_aux, sizeof(BuildAux), cudaMemcpyDeviceToHost, st);
-  cudaMemcpyAsync(&h_top, b->d_top, sizeof(TopModel), cudaMemcpyDeviceToHost, st);
+  copy_result_to_host(box, &b->tables, b->d_aux, b->d_top, leaves_to_host ? (const double*)b->buf.params : nullptr,
+                      (const u64*)b->buf.errors, want_counts ? (const u64*)b->buf.counts : nullptr, st);
   cudaMemcpyAsync(b->h_flags_all, b->d_flags_all, 2 * sizeof(unsigned) * W, cudaMemcpyDeviceToHost, st);
-  if (b->top->kind == M_RADIX_TABLE && box->table32.resize((size_t)1 << b->top->table_bits))
-    cudaMemcpyAsync(box->table32.data(), b->d_table32, sizeof(u32) << b->top->table_bits, cudaMemcpyDeviceToHost, st);
-  if (b->top->kind == M_HISTOGRAM && box->arr1.resize(((size_t)1 << 20) + 1) && box->arr2.resize(b->hist_bins)) {
-    cudaMemcpyAsync(box->arr1.data(), b->d_ri, sizeof(u64) * box->arr1.size(), cudaMemcpyDeviceToHost, st);
-    cudaMemcpyAsync(box->arr2.data(), b->d_pivots, sizeof(u64) * b->hist_bins, cudaMemcpyDeviceToHost, st);
-  }
-  if (leaves_to_host) {
-    cudaMemcpyAsync(box->l1_params.data(), b->buf.params, sizeof(double) * N * ppm, cudaMemcpyDeviceToHost, st);
-    cudaMemcpyAsync(box->l1_errors.data(), b->buf.errors, sizeof(u64) * N, cudaMemcpyDeviceToHost, st);
-    if (want_counts) cudaMemcpyAsync(box->l1_counts.data(), b->buf.counts, sizeof(u64) * N, cudaMemcpyDeviceToHost, st);
-  }
   cudaError_t e = cudaStreamSynchronize(st);
   if (e != cudaSuccess) { delete box; return fail(RMI_ERR_CUDA, std::string("rmi_shard_train: ") + cudaGetErrorString(e)); }
   if (trace && n_marks > 1) {
@@ -2163,7 +2073,7 @@ static int shard_train_typed(rmi_shard_build* b, rmi_shard_comm* c, uint32_t fla
   float ms = 0.f;
   cudaEventElapsedTime(&ms, b->ev_t0, b->ev_t1);
   const uint64_t total_ns = (uint64_t)((double)ms * 1e6);
-  int rcf = shard_fill_result(b, box, flags, st_all, cnr, leaves_to_host, &total_ns, out);
+  int rcf = shard_result(b, box, st_all, cnr, &total_ns, out);
   if (rcf == RMI_OK && shared) {
     if (rank == 0) {   // the leaf tables live in the shared region (valid until the next-but-one call, see the header)
       rmi_result* R = *out;
@@ -2185,11 +2095,7 @@ int rmi_shard_train(rmi_shard_build* b, rmi_shard_comm* c, uint32_t flags, rmi_r
     return fail(RMI_ERR_INVALID, "rmi_shard_train: call rmi_shard_set_partition with the communicator's world size and rank first");
   if (!nccl_api().ok) return fail(RMI_ERR_UNSUPPORTED, nccl_api().error);
   CUDA_TRY(cudaSetDevice(b->ds->device));
-  switch (b->ds->key_type) {
-    case RMI_KEY_U64: return shard_train_typed<u64>(b, c, flags, out);
-    case RMI_KEY_U32: return shard_train_typed<u32>(b, c, flags, out);
-    default: return shard_train_typed<double>(b, c, flags, out);
-  }
+  return with_key_type(b->ds->key_type, [&](auto k) { return shard_train_typed<decltype(k)>(b, c, flags, out); });
 }
 
 void rmi_shard_build_destroy(rmi_shard_build* b) {
@@ -2200,7 +2106,7 @@ void rmi_shard_build_destroy(rmi_shard_build* b) {
   if (b->ev_join) cudaEventDestroy(b->ev_join);
   if (b->side) cudaStreamDestroy(b->side);
   cudaFree(b->d_long);
-  cudaFree(b->d_table32); cudaFree(b->d_pivots); cudaFree(b->d_ri);
+  cudaFree(b->tables.t32); cudaFree(b->tables.pivots); cudaFree(b->tables.radix_index);
   cudaFree(b->d_bases); cudaFree(b->d_off); cudaFree(b->d_parts); cudaFree(b->d_flags_mine); cudaFree(b->d_flags_all);
   if (b->h_off) cudaFreeHost(b->h_off);
   if (b->h_flags_all) cudaFreeHost(b->h_flags_all);
