@@ -172,15 +172,7 @@ def test_other_leaf_models_given_top(rmi, oracle, leaf, dname):
     g = rmi.train(dataset(rmi, dname), spec, bf)
     parity.assert_top_equal(g, o)
     if leaf == "cubic":
-        # pow(x, 3.0) in libm vs the double-double cube on the device: equal to 1e-9, and
-        # almost always bit-equal; error bounds are compared where the parameters are.
-        assert g.l1_params.shape == o.l1_params.shape
-        same = (parity.bits(g.l1_params) == parity.bits(o.l1_params)).all(axis=1)
-        assert same.mean() > 0.99
-        for j in np.flatnonzero(~same):
-            parity.assert_coef_close("cubic", g.l1_params[j], o.l1_params[j], len(keys))
-        assert np.array_equal(g.last_layer_max_l1s[same], o.l1_errors[same])
-        assert np.array_equal(g.l1_counts, o.l1_counts)
+        parity.assert_cubic_leaves_close(g, o, len(keys))
     else:
         parity.assert_same_rmi(g, o)
 

@@ -22,7 +22,38 @@ def _free_port():
     return p
 
 
+def _designed_counts(n, N=1024):
+    """Leaf counts (radix top, N leaves, 2^15 values per leaf) that put long leaves at the ranks' cuts (0.31 n for
+    two ranks, n/3 and 2n/3 for three): leaf 300 (long-leaf kernel for linear leaves) holds 0.31 n, leaf 311
+    (solo chain, cooperative walk) starts at n/3, and a warp of 28 long leaves (cubic: the all-long cooperative
+    walk) has leaf 366 start at 2n/3.  A leaf that starts at a cut is trained with the previous rank's last key."""
+    c1, c2 = int(n * 0.31), n // 3
+    c3 = 2 * n // 3
+    counts = []
+
+    def fill(k, keys):
+        counts.extend(keys // k + (i < keys % k) for i in range(k))
+
+    fill(300, c1 - 1500)
+    counts.append(3000)                                   # [c1 - 1500, c1 + 1500)
+    fill(10, c2 - (c1 + 1500))
+    counts.append(2000)                                   # [c2, c2 + 2000)
+    long28 = 14 * 1100
+    fill(40, c3 - long28 - (c2 + 2000))
+    counts.extend([1100] * 28)                            # leaves 352 .. 379; leaf 366 starts at c3
+    fill(N - len(counts), n - c3 - long28)
+    assert len(counts) == N and sum(counts) == n and counts[366] == 1100 and sum(counts[:366]) == c3
+    return counts
+
+
 def _keys(kind, n):
+    if kind == "designed":
+        counts = _designed_counts(n)
+        S = np.cumsum([0] + counts)
+        runs = [(int(n * 0.31) - 20, 40),                 # across the two-rank cut, inside leaf 300
+                (int(S[366]) - 20, 20),                   # ending on leaf 365's last key, at the cut 2n/3
+                (int(S[311]) + 15, 5), (int(S[311]) + 31, 5)]   # around the solo hand-off of leaf 311
+        return datasets.designed_leaves(counts, 15, np.uint64, runs=runs)
     if kind == "uniform":
         return datasets.uniform_u64(n, seed=31)
     if kind == "dups":
@@ -103,7 +134,9 @@ CASES = [("uniform", "linear,linear", 1024), ("uniform", "radix,linear", 4096), 
          ("uniform", "radix18,linear", 2048), ("dups", "radix8,linear", 200), ("lognormal", "histogram,linear", 512),
          ("uniform", "histogram,linear_spline", 1000),
          # enough leaves per rank for the sliced launch of the owned leaf window (shared result region, one-call path)
-         ("uniform", "linear,linear", 131072), ("dups", "linear_spline,linear", 98304)]
+         ("uniform", "linear,linear", 131072), ("dups", "linear_spline,linear", 98304),
+         # long leaves, a warp of 28 long leaves and runs of equal keys at the cuts (_designed_counts)
+         ("designed", "radix,linear", 1024), ("designed", "radix,cubic", 1024)]
 
 
 @pytest.mark.parametrize("kind,spec,N", CASES, ids=[f"{c[0]}-{c[1]}-{c[2]}" for c in CASES])
