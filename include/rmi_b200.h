@@ -151,6 +151,13 @@ int rmi_train(const rmi_dataset* ds, const char* model_spec, uint64_t branch_fac
 int rmi_train_with_top(const rmi_dataset* ds, const char* model_spec, uint64_t branch_factor, uint32_t flags,
                        const double* l0_fparams, uint32_t n_fparams, rmi_result** out);
 void rmi_result_free(rmi_result* r);
+/* The reference's error pass, lower-bound widening and statistics (two_layer.rs:205-284) of r's top and leaf tables
+ * over ds's keys.  Parameters are never refitted or replaced: the returned result holds r's tables bit for bit,
+ * with l1_errors, (with RMI_FLAG_LEAF_COUNTS) l1_counts and the summary statistics measured on ds, and
+ * num_rmi_rows = num_data_rows = rmi_dataset_len(ds).  Flags: RMI_FLAG_STATS_ONLY, RMI_FLAG_LEAF_COUNTS.
+ * A top model that is not monotone on ds is RMI_ERR_PANIC with the training's message (two_layer.rs:50).
+ * phase_device_ns: [0] upload of the tables, [1] leaf boundaries, [2] error pass, [3] statistics. */
+int rmi_evaluate(const rmi_dataset* ds, const rmi_result* r, uint32_t flags, rmi_result** out);
 
 /* The optimizer's unit of work (optimizer.rs:110-125 enumerates every leaf type for each (top, branching factor)):
  * `num_leaf_models` configurations "top,leaf_k" with the SAME top model and branching factor in one call.  The top
@@ -349,6 +356,26 @@ uint64_t rmi_model_size(const rmi_result* r, int include_errors, uint64_t num_sp
 int rmi_output_rmi(const char* ns, const rmi_result* r, const char* data_dir, const char* out_dir, int key_type,
                    int include_errors, uint64_t build_time_ns, const rmi_spline_point* knots, uint64_t num_knots,
                    uint64_t line_size, uint64_t num_data_rows);
+
+/* What rmi_load_rmi found in an artefact besides the model. */
+typedef struct {
+  int key_type;            /* RMI_KEY_U64 or RMI_KEY_F64: the lookup signature's key type */
+  int has_errors;          /* 0: a --no-errors artefact; the result's l1_errors is NULL */
+  uint64_t line_size;      /* --bounded: the cache-fix line size; 0 otherwise */
+  uint64_t num_knots;      /* --bounded: knots returned in *knots (free with rmi_spline_free); 0 otherwise */
+  uint64_t num_data_rows;  /* --bounded: total_keys; otherwise num_rmi_rows */
+  uint64_t build_time_ns;  /* BUILD_TIME_NS */
+} rmi_artefact_info;
+/* The inverse of rmi_output_rmi (host code, no device work): reads <out_dir>/<ns>.cpp, <ns>.h, <ns>_data.h and the
+ * blobs under data_dir, in the forms the reference's code generator writes, and rebuilds the two-layer model as a
+ * result (release with rmi_result_free).  linear, robust_linear and linear_spline generate the same code and load as
+ * RMI_MODEL_LINEAR.  The artefact holds no statistics: the model_avg_* / model_max_log2_error fields are NaN and
+ * model_max_error(_idx) 0; rmi_evaluate measures them.  build_time_ns = BUILD_TIME_NS, the timings are 0.  *knots is
+ * NULL unless the artefact is --bounded.  A malformed artefact (missing or truncated blob, wrong namespace, unknown
+ * function, bad constant, sizes that disagree, RMI_SIZE included) is RMI_ERR_INVALID with the file named in
+ * rmi_last_error(); a --bounded artefact without errors, whose generated code does not compile, RMI_ERR_UNSUPPORTED. */
+int rmi_load_rmi(const char* ns, const char* out_dir, const char* data_dir, rmi_result** out, rmi_spline_point** knots,
+                 rmi_artefact_info* info);
 
 /* optimizer::find_pareto_efficient_configs (optimizer.rs:233-249): the two-phase search over
  * (models, branching factor); every candidate is one stats-only build.  `replicas` are

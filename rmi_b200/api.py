@@ -50,6 +50,12 @@ class _CacheFixStats(C.Structure):
                 ("stitch_segments", C.c_uint64), ("fallback_points", C.c_uint64), ("evaluations", C.c_uint64)]
 
 
+class _ArtefactInfo(C.Structure):
+    """struct rmi_artefact_info (include/rmi_b200.h): what rmi_load_rmi found besides the model."""
+    _fields_ = [("key_type", C.c_int), ("has_errors", C.c_int), ("line_size", C.c_uint64), ("num_knots", C.c_uint64),
+                ("num_data_rows", C.c_uint64), ("build_time_ns", C.c_uint64)]
+
+
 class _ConfigStats(C.Structure):
     """struct rmi_config_stats (optimizer.rs:153-160 RMIStatistics)."""
     _fields_ = [("models", C.c_char * 64), ("branching_factor", C.c_uint64), ("average_log2_error", C.c_double),
@@ -93,6 +99,9 @@ def load_library():
         L.rmi_model_size.argtypes = [C.POINTER(_Result), C.c_int, C.c_uint64]
         L.rmi_output_rmi.argtypes = [C.c_char_p, C.POINTER(_Result), C.c_char_p, C.c_char_p, C.c_int, C.c_int, C.c_uint64,
                                      C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64]
+        L.rmi_load_rmi.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.POINTER(C.POINTER(_Result)), C.POINTER(C.c_void_p),
+                                   C.POINTER(_ArtefactInfo)]
+        L.rmi_evaluate.argtypes = [C.c_void_p, C.POINTER(_Result), C.c_uint32, C.POINTER(C.POINTER(_Result))]
         L.rmi_find_pareto_efficient_configs.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_uint64, C.c_uint32,
                                                         C.POINTER(_ConfigStats), C.c_uint64, C.POINTER(C.c_uint64)]
         L.rmi_index_create.argtypes = [C.POINTER(_Result), C.c_void_p, C.POINTER(C.c_void_p)]
@@ -272,6 +281,40 @@ def output_rmi(namespace: str, rmi, data_dir: str, key_type: int = KEY_U64, incl
         int(num_data_rows)))
 
 
+def load_rmi(namespace: str, out_dir: str = ".", data_dir: str = "rmi_data"):
+    """The inverse of output_rmi (host code, no GPU): reads <out_dir>/<ns>.cpp/.h/_data.h and the blobs under data_dir
+    as the reference's code generator writes them.  Returns ``(TrainedRMI, cache_fix)``, cache_fix ``None`` or
+    ``(line_size, knots)`` with knots a (K, 2) uint64 array (the reference's TrainedRMI.cache_fix).  The artefact holds
+    no statistics (NaN / 0 here; ``evaluate`` measures them); ``last_layer_max_l1s`` is None for a --no-errors
+    artefact.  linear, robust_linear and linear_spline generate the same code and load as linear.  ``key_type`` on
+    the returned TrainedRMI is the lookup signature's (KEY_U64 or KEY_F64)."""
+    L = load_library()
+    res, pts, info = C.POINTER(_Result)(), C.c_void_p(), _ArtefactInfo()
+    _check(L.rmi_load_rmi(namespace.encode(), out_dir.encode(), data_dir.encode(), C.byref(res), C.byref(pts), C.byref(info)))
+    r = res.contents
+    spec = f"{MODEL_NAMES[int(r.l0_model_id)]},{MODEL_NAMES[int(r.l1_model_id)]}"
+    trained = result_from_pointer(res, spec)
+    trained.num_data_rows = int(info.num_data_rows)
+    trained.build_time = int(info.build_time_ns)
+    trained.key_type = int(info.key_type)
+    cf = None
+    if pts.value:
+        cf = (int(info.line_size), _take_knots(L, pts, C.c_uint64(info.num_knots)))
+    return trained, cf
+
+
+def evaluate(trained: TrainedRMI, data: RMITrainingData, counts: bool = True, flags: int = 0) -> TrainedRMI:
+    """The reference's error pass, lower-bound widening and statistics (two_layer.rs:205-284) of ``trained``'s top and
+    leaf tables over ``data``'s keys, on the GPU.  The tables are returned unchanged, bit for bit; the error bounds,
+    the key counts (counts=True) and the statistics are those of ``data``, and num_rmi_rows = num_data_rows =
+    len(data).  Raises RMIPanic where the top model is not monotone on ``data`` (two_layer.rs:50)."""
+    if counts:
+        flags = int(flags) | FLAG_LEAF_COUNTS
+    res = C.POINTER(_Result)()
+    _check(load_library().rmi_evaluate(data._h, _result_ptr(trained), int(flags), C.byref(res)))
+    return result_from_pointer(res, trained.models)
+
+
 def find_pareto_efficient_configs(replicas, restrict_to: int = 10, flags: int = 0) -> list[dict]:
     """optimizer::find_pareto_efficient_configs (optimizer.rs:233-249).  `replicas`: one RMITrainingData or a
     list holding the same keys on several devices (RMITrainingData.replicate); the independent stats-only
@@ -338,6 +381,7 @@ class TrainedRMI:
     could_not_replace: bool
     top_fit_exact: bool
     _res: object = None            # keeps the underlying struct rmi_result alive
+    key_type: int | None = None    # load_rmi: the key type of the artefact's lookup signature
 
 
 class _ResultOwner:
@@ -442,6 +486,26 @@ class RMIIndex:
         self.key_type = data.key_type
         self._trained = trained
         _check(load_library().rmi_index_create(_result_ptr(trained), data._h, C.byref(self._h)))
+
+    @classmethod
+    def load(cls, namespace: str, data: RMITrainingData, out_dir: str = ".", data_dir: str = "rmi_data") -> "RMIIndex":
+        """An index from generated artefacts (load_rmi) over ``data``: an RMIIndex, or a BoundedRMIIndex for a
+        --bounded artefact.  An f64 artefact needs f64 data; a u64 artefact takes u64 or u32 data (the rmi CLI writes
+        uint64_t code for uint32 key files).  A --no-errors artefact gets its bounds from ``evaluate`` on ``data``.
+        Keys that differ in number from the ones the artefact was built on fail in rmi_index_create; an index over
+        the new keys is then ``RMIIndex(evaluate(trained, data), data)``."""
+        trained, cf = load_rmi(namespace, out_dir, data_dir)
+        want = (KEY_F64,) if trained.key_type == KEY_F64 else (KEY_U64, KEY_U32)
+        if data.key_type not in want:
+            raise RMIError(f"the artefact's lookup takes {'double' if trained.key_type == KEY_F64 else 'uint64_t'} keys, "
+                           f"the data holds {np.dtype(_NP_OF_KEY[data.key_type])}")
+        if cf is not None:
+            if trained.last_layer_max_l1s is None:
+                raise RMIError("a --bounded artefact without errors cannot be served")
+            return BoundedRMIIndex(trained, cf[1], cf[0], data)
+        if trained.last_layer_max_l1s is None:
+            trained = evaluate(trained, data, counts=False)
+        return cls(trained, data)
 
     def _queries(self, q) -> np.ndarray:
         if not isinstance(q, np.ndarray) or q.dtype != np.dtype(_NP_OF_KEY[self.key_type]):

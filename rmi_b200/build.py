@@ -12,10 +12,11 @@ LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "librmi_b200.so")
 OBJ_DIR = os.path.join(HERE, "build")
 
-SOURCES = ["kernels_top.cu", "kernels_leaf.cu", "kernels_shard.cu", "kernels_lookup.cu", "kernels_cachefix.cu", "api.cu"]
+SOURCES = ["kernels_top.cu", "kernels_leaf.cu", "kernels_shard.cu", "kernels_lookup.cu", "kernels_cachefix.cu", "kernels_eval.cu",
+           "api.cu"]
 HEADERS = ["rust_math.cuh", "models.cuh", "device_util.cuh", "spline.cuh", "kernels.h",
            os.path.join("..", "..", "include", "rmi_b200.h"), os.path.join("..", "..", "host", "cache_fix.hpp"), os.path.join("..", "..", "host", "codegen.hpp"),
-           os.path.join("..", "..", "host", "optimizer.hpp")]
+           os.path.join("..", "..", "host", "optimizer.hpp"), os.path.join("..", "..", "host", "artefact_load.hpp")]
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 # -fmad=false: the reference fuses a multiply-add only where it writes mul_add; everything

@@ -15,6 +15,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -23,6 +24,7 @@
 #include "kernels.h"
 #include "nccl_dl.h"
 #include "../../host/cache_fix.hpp"
+#include "../../host/artefact_load.hpp"
 #include "../../host/codegen.hpp"
 #include "../../host/optimizer.hpp"
 
@@ -275,6 +277,7 @@ struct ResultBox {
   PinnedArray<uint32_t> table32;
   PinnedArray<uint64_t> arr1, arr2;
   PinnedArray<char> scalars;   // BuildAux + TopModel read-back
+  std::unique_ptr<rmihost::LoadedArtefact> loaded;   // rmi_load_rmi: owns the tables (host memory, no device needed)
 };
 
 namespace {
@@ -302,6 +305,41 @@ struct TopTables {
       return pivots && radix_index;
     }
     return true;
+  }
+
+  // The tables of a given result's top model (rmi_evaluate): allocated with alloc and uploaded on st.
+  template <class Alloc> bool upload(const rmi_result& r, cudaStream_t st, Alloc&& alloc) {
+    if (r.l0_model_id == M_RADIX_TABLE) {
+      t32_len = r.l0_table32_len;
+      t32 = (u32*)alloc(sizeof(u32) * t32_len);
+      if (!t32) return false;
+      cudaMemcpyAsync(t32, r.l0_table32, sizeof(u32) * t32_len, cudaMemcpyHostToDevice, st);
+    }
+    if (r.l0_model_id == M_HISTOGRAM) {
+      hist_bins = r.l0_array2_len;
+      ri_len = r.l0_array1_len;
+      pivots = (u64*)alloc(sizeof(u64) * hist_bins);
+      radix_index = (u64*)alloc(sizeof(u64) * ri_len);
+      if (!pivots || !radix_index) return false;
+      cudaMemcpyAsync(pivots, r.l0_array2, sizeof(u64) * hist_bins, cudaMemcpyHostToDevice, st);
+      cudaMemcpyAsync(radix_index, r.l0_array1, sizeof(u64) * ri_len, cudaMemcpyHostToDevice, st);
+    }
+    return true;
+  }
+
+  // The TopModel of a given result, pointing at the tables upload() placed.
+  TopModel given(const rmi_result& r) const {
+    TopModel h;
+    memset(&h, 0, sizeof(h));
+    h.kind = (int)r.l0_model_id;
+    h.high = (int)r.l0_bradix_high;
+    h.table_bits = (int)r.l0_table_bits;
+    for (int q = 0; q < 4; ++q) { h.f[q] = r.l0_fparams[q]; h.ip[q] = r.l0_iparams[q]; }
+    h.t32 = t32;
+    h.pivots = pivots;
+    h.radix_index = radix_index;
+    h.npivots = hist_bins;
+    return h;
   }
 
   // The TopModel a build starts from; f: nf injected top parameters, or null.
@@ -564,6 +602,38 @@ int rmi_output_rmi(const char* ns, const rmi_result* r, const char* data_dir, co
   } catch (const std::exception& e) {
     return fail(RMI_ERR_PANIC, e.what());
   }
+}
+
+int rmi_load_rmi(const char* ns, const char* out_dir, const char* data_dir, rmi_result** out, rmi_spline_point** knots,
+                 rmi_artefact_info* info) {
+  g_last_error.clear();
+  if (!ns || !out_dir || !data_dir || !out || !knots || !info) return fail(RMI_ERR_INVALID, "rmi_load_rmi: null argument");
+  auto a = std::make_unique<rmihost::LoadedArtefact>();
+  try {
+    rmihost::load_rmi(ns, out_dir, data_dir, a.get());
+  } catch (const rmihost::LoadError& e) {
+    return fail(e.code, e.what());
+  } catch (const std::exception& e) {
+    return fail(RMI_ERR_INVALID, std::string("rmi_load_rmi: ") + e.what());
+  }
+  rmi_spline_point* pts = nullptr;
+  if (!a->knots.empty()) {
+    pts = static_cast<rmi_spline_point*>(std::malloc(a->knots.size() * sizeof(rmi_spline_point)));
+    if (!pts) return fail(RMI_ERR_INVALID, "rmi_load_rmi: out of host memory");
+    for (size_t k = 0; k < a->knots.size(); ++k) { pts[k].key = a->knots[k].first; pts[k].offset = a->knots[k].second; }
+  }
+  auto box = new ResultBox();
+  box->pub = a->r;
+  *out = &box->pub;
+  *knots = pts;
+  info->key_type = a->key_type;
+  info->has_errors = a->has_errors ? 1 : 0;
+  info->line_size = a->line_size;
+  info->num_knots = a->knots.size();
+  info->num_data_rows = a->r.num_data_rows;
+  info->build_time_ns = a->build_time_ns;
+  box->loaded = std::move(a);   // the result's tables live in the loaded artefact
+  return RMI_OK;
 }
 
 int rmi_find_pareto_efficient_configs(const rmi_dataset* const* replicas, int num_replicas, uint64_t restrict_to,
@@ -1281,6 +1351,111 @@ int train_entry(const rmi_dataset* ds, const char* model_spec, uint64_t N, uint3
   });
 }
 
+// The model table entry of a result's top / leaf model id (radix tables by their table bits).
+const ModelName* model_of(uint32_t kind, uint32_t table_bits) {
+  for (const auto& m : kModels)
+    if (m.kind == (int)kind && (kind != M_RADIX_TABLE || m.table_bits == (int)table_bits)) return &m;
+  return nullptr;
+}
+
+// The statuses of the boundary pass that concern a given top model: the error pass clamps the top's prediction to
+// N - 1 (two_layer.rs:210-211) and fits nothing, so only the order checks of two_layer.rs:50 remain.
+constexpr unsigned kEvaluateStatus = ST_NOT_SORTED | ST_NON_MONOTONE;
+
+template <class T>
+int evaluate_typed(const rmi_dataset* ds, const rmi_result* r, const ModelName& top, const ModelName& leaf, uint32_t flags,
+                   rmi_result** out) {
+  auto t_start = std::chrono::steady_clock::now();
+  const uint64_t n = ds->n, N = r->branching_factor;
+  const T* keys = (const T*)ds->d_keys;
+  CUDA_TRY(cudaSetDevice(ds->device));
+  DeviceInfo di;
+  if (int rc = device_info(ds->device, &di)) return rc;
+  BuildContext* bc = t_build_ctx.get(ds->device);
+  if (!bc) return fail(RMI_ERR_CUDA, "could not create the build's CUDA streams / events");
+  cudaStream_t st = bc->st;
+  cudaEvent_t ev0 = bc->ev0, ev1 = bc->ev1, *evp = bc->evp;
+  const int ppm = leaf_params_per_model(leaf.kind);
+  const bool stats_only = (flags & RMI_FLAG_STATS_ONLY) != 0;
+  const bool want_counts = !stats_only && (flags & RMI_FLAG_LEAF_COUNTS) != 0;
+  int rc = RMI_OK;
+  auto box = new ResultBox();
+  {
+    Arena A(st);
+    Launch L{st, di.num_sms};
+    TopModel* d_top = A.get<TopModel>(1);
+    BuildAux* d_aux = A.get<BuildAux>(1);
+    u64* d_S = A.get<u64>(N + 1);
+    double* d_params = A.get<double>(N * ppm);
+    u64* d_errors = A.get<u64>(N);
+    u64* d_counts = A.get<u64>(N);
+    u64* d_scratch = A.get<u64>(2 * N);
+    void* d_stats = A.get<char>(stats_scratch_bytes(N));
+    TopTables tables;
+    const bool host_ok = reserve_result(box, nullptr, N, ppm, !stats_only, want_counts) &&
+                         (r->l0_table32_len == 0 || box->table32.resize(r->l0_table32_len)) &&
+                         (r->l0_model_id != M_HISTOGRAM ||
+                          (box->arr1.resize(r->l0_array1_len) && box->arr2.resize(r->l0_array2_len)));
+    cudaEventRecord(ev0, st);
+    const bool tables_ok = tables.upload(*r, st, [&](size_t bytes) -> void* { return A.get<char>(bytes); });
+    if (A.err != cudaSuccess || !tables_ok) {
+      rc = fail(RMI_ERR_CUDA, std::string("scratch allocation: ") + cudaGetErrorString(A.err));
+    } else if (!host_ok) {
+      rc = fail(RMI_ERR_CUDA, kPinnedFailed);
+    } else {
+      const TopModel h_top = tables.given(*r);
+      cudaMemcpyAsync(d_top, &h_top, sizeof(h_top), cudaMemcpyHostToDevice, st);
+      cudaMemcpyAsync(d_params, r->l1_params, sizeof(double) * N * ppm, cudaMemcpyHostToDevice, st);
+      cudaMemsetAsync(d_aux, 0, sizeof(BuildAux), st);
+      cudaEventRecord(evp[0], st);
+      // the streaming pass: the given top is not known to be monotone on these keys
+      compute_leaf_bounds<T>(L, keys, n, top.kind, d_top, N, d_S, d_aux, /*allow_search=*/false, nullptr);
+      cudaEventRecord(evp[1], st);
+      evaluate_leaves<T>(L, keys, n, ds->no_dups, leaf.kind, N, d_S, d_params, d_scratch, d_errors, d_counts);
+      cudaEventRecord(evp[2], st);
+      leaf_statistics(L, n, N, d_errors, d_counts, d_aux, d_stats);
+      cudaEventRecord(ev1, st);
+      copy_result_to_host(box, nullptr, d_aux, d_top, nullptr, nullptr, nullptr, st);
+      if (!stats_only) {
+        cudaMemcpyAsync(box->l1_errors.data(), d_errors, sizeof(u64) * N, cudaMemcpyDeviceToHost, st);
+        if (want_counts) cudaMemcpyAsync(box->l1_counts.data(), d_counts, sizeof(u64) * N, cudaMemcpyDeviceToHost, st);
+      }
+      cudaError_t e = cudaStreamSynchronize(st);
+      const unsigned status = e == cudaSuccess ? result_aux(box).status & kEvaluateStatus : 0;
+      if (e != cudaSuccess) {
+        rc = fail(RMI_ERR_CUDA, std::string("rmi_evaluate: ") + cudaGetErrorString(e));
+      } else if (status) {
+        rc = fail(RMI_ERR_PANIC, status_text(status));
+      } else {
+        // r's tables, as given (the device copies were only read)
+        if (!stats_only) memcpy(box->l1_params.data(), r->l1_params, sizeof(double) * N * ppm);
+        if (r->l0_table32_len) memcpy(box->table32.data(), r->l0_table32, sizeof(u32) * r->l0_table32_len);
+        if (r->l0_model_id == M_HISTOGRAM) {
+          memcpy(box->arr1.data(), r->l0_array1, sizeof(u64) * r->l0_array1_len);
+          memcpy(box->arr2.data(), r->l0_array2, sizeof(u64) * r->l0_array2_len);
+        }
+        tables.t32_len = r->l0_table32_len;
+        tables.ri_len = r->l0_model_id == M_HISTOGRAM ? r->l0_array1_len : 0;
+        tables.hist_bins = r->l0_model_id == M_HISTOGRAM ? r->l0_array2_len : 0;
+        fill_result(box, top, leaf, tables, n, N);
+        rmi_result& R = box->pub;
+        R.l0_num_fparams = r->l0_num_fparams;
+        R.l0_num_iparams = r->l0_num_iparams;
+        R.device_time_ns = elapsed_ns(ev0, ev1);
+        cudaEvent_t seq[5] = {ev0, evp[0], evp[1], evp[2], ev1};
+        for (int q = 0; q < 4; ++q) R.phase_device_ns[q] = elapsed_ns(seq[q], seq[q + 1]);
+        R.top_fit_exact = r->top_fit_exact;
+      }
+    }
+  }   // arena frees (stream-ordered)
+  cudaStreamSynchronize(st);
+  if (rc != RMI_OK) { delete box; return rc; }
+  box->pub.build_time_ns =
+      (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t_start).count();
+  *out = &box->pub;
+  return RMI_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1315,6 +1490,27 @@ int rmi_train_with_top(const rmi_dataset* ds, const char* model_spec, uint64_t b
                        const double* l0_fparams, uint32_t n_fparams, rmi_result** out) {
   if (!l0_fparams) return fail(RMI_ERR_INVALID, "rmi_train_with_top: null parameters");
   return train_entry(ds, model_spec, branch_factor, flags, l0_fparams, n_fparams, out);
+}
+
+int rmi_evaluate(const rmi_dataset* ds, const rmi_result* r, uint32_t flags, rmi_result** out) {
+  g_last_error.clear();
+  const std::string fn = "rmi_evaluate";
+  if (!ds || !r || !out) return fail(RMI_ERR_INVALID, fn + ": null argument");
+  const ModelName* top = model_of(r->l0_model_id, r->l0_table_bits);
+  const ModelName* leaf = model_of(r->l1_model_id, 0);
+  if (!top || !leaf || leaf->root_only)
+    return fail(RMI_ERR_INVALID, fn + ": unknown model id (top " + std::to_string(r->l0_model_id) + ", leaf " +
+                                     std::to_string(r->l1_model_id) + ")");
+  if (int rc = check_leaf(leaf)) return rc;
+  if (!r->l1_params) return fail(RMI_ERR_INVALID, fn + ": the result holds no leaf parameters (RMI_FLAG_STATS_ONLY)");
+  if (r->l1_params_per_model != (uint32_t)leaf_params_per_model(leaf->kind))
+    return fail(RMI_ERR_INVALID, fn + ": wrong number of leaf parameters");
+  if (r->l0_model_id == M_RADIX_TABLE && (!r->l0_table32 || r->l0_table32_len != ((uint64_t)1 << r->l0_table_bits)))
+    return fail(RMI_ERR_INVALID, fn + ": radix table missing or of the wrong size");
+  if (r->l0_model_id == M_HISTOGRAM && (!r->l0_array2 || !r->l0_array2_len || (r->l0_array1_len && !r->l0_array1)))
+    return fail(RMI_ERR_INVALID, fn + ": histogram pivots missing");
+  if (int rc = check_build(ds->n, r->branching_factor, ds->sorted)) return rc;
+  return with_key_type(ds->key_type, [&](auto k) { return evaluate_typed<decltype(k)>(ds, r, *top, *leaf, flags, out); });
 }
 
 int rmi_cache_fix_device(const rmi_dataset* ds, uint64_t line_size, rmi_spline_point** out_points, uint64_t* out_count,

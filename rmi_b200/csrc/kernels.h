@@ -147,6 +147,14 @@ void leaf_statistics(const Launch& L, u64 n, u64 num_leaves, const u64* d_errors
                      BuildAux* d_aux, void* scratch);
 size_t stats_scratch_bytes(u64 num_leaves);
 
+// ---- error pass over given leaf tables (kernels_eval.cu, rmi_evaluate) ---------------------------
+// fit_leaves's forward pass and widening without the fit and without the empty-leaf constants: from the boundaries
+// d_S (compute_leaf_bounds) and N x ppm given parameters, writes N error bounds and N key counts.  no_dups: the keys
+// hold no two equal ones (the run tracking is skipped).  d_scratch: 2 x N u64.  Three launches.
+template <class T>
+void evaluate_leaves(const Launch& L, const T* keys, u64 n, bool no_dups, int leaf_kind, u64 N, const u64* d_S,
+                     const double* d_params, u64* d_scratch, u64* d_errors, u64* d_counts);
+
 // ---- cross-rank pieces of a range-partitioned build (kernels_leaf.cu) --------------------------
 // d_off[r] = first leaf owned by rank r, d_off[world] = N (d_bases: global index of every rank's first key,
 // world + 1 entries; r_last: last rank that holds keys).  One tiny kernel, no host involvement.
