@@ -310,6 +310,61 @@ void rmi_shard_comm_destroy(rmi_shard_comm* c);
 int rmi_shard_set_partition(rmi_shard_build* b, const uint64_t* bases, int world, int rank);
 int rmi_shard_train(rmi_shard_build* b, rmi_shard_comm* c, uint32_t flags, rmi_result** out);
 
+/* ---- Lookups over a range-partitioned data set (DESIGN.md section 14) ------------------------------------------
+ * Every rank holds the whole model and its own slab of the keys; together the slabs are the key set the model was
+ * trained on (or evaluated on).  Query q is answered by the last non-empty rank whose first key is < q (the first
+ * non-empty rank if none is, a NaN query included): every key before its slab is < q and every key after it is not,
+ * so the global lower bound is the slab's base + the lower bound inside the slab, exactly, with no key of another rank
+ * read.  predict is local (the model alone); lower_bound moves the queries (4 or 8 bytes each) to their ranks and the
+ * 8-byte answers back.
+ *
+ * rmi_shard_index_create uploads r's tables as rmi_index_create does and binds them to `local`.  ends_all holds every
+ * rank's rmi_shard_ends (rmi_shard_ends_get, gathered over the ranks).  Refused with RMI_ERR_INVALID before any device
+ * work: a null argument; rank / world out of range (1 <= world <= 63); a result without leaf tables (RMI_FLAG_STATS_ONLY,
+ * or a rank other than 0 of an RMI_FLAG_SHARD_ROOT_ONLY build); ends_all[rank].n_local != rmi_dataset_len(local);
+ * r->num_rmi_rows != the sum of n_local; non-empty slabs out of key order (a slab's last key above the next one's
+ * first); and every model rmi_index_create refuses.  local must outlive the index. */
+typedef struct rmi_shard_index rmi_shard_index;
+int rmi_shard_index_create(const rmi_result* r, const rmi_dataset* local, const rmi_shard_ends* ends_all, int world,
+                           int rank, rmi_shard_index** out);
+void rmi_shard_index_destroy(rmi_shard_index* idx);
+/* rmi_index_predict over the whole key set (n = the sum of n_local): local, no communication. */
+int rmi_shard_index_predict(const rmi_shard_index* idx, const void* d_queries, uint64_t n, uint64_t* d_pos,
+                            uint64_t* d_err, void* cuda_stream);
+/* The lower bound in phases; the caller exchanges the buffers between them (rmi_b200/sharded.py does it with
+ * torch.distributed):
+ *   route    d_send (n keys) receives the n queries grouped by rank in rank order, d_send_counts (world u64) the size
+ *            of each group, d_slot (n u64) the position of query i in d_send.  Three kernel launches (n == 0: none,
+ *            d_send_counts is zeroed).
+ *            -> every rank sends group p to rank p; the groups received are concatenated in source-rank order
+ *   search   exact global lower bounds of the m received queries, in received order; *d_fallbacks (may be NULL) grows by
+ *            the number of those queries whose window missed.  Two launches (the predict kernel, then the window search
+ *            over the slab; none for m == 0).  A rank without keys receives no queries (m > 0 there is refused).
+ *            -> every rank returns the answers of each source's group to that source, received in rank order
+ *   gather   d_out[i] = d_returned[d_slot[i]].  One launch.
+ * All calls are enqueued on cuda_stream without a host synchronisation; scratch comes from the stream-ordered pool. */
+int rmi_shard_index_route(const rmi_shard_index* idx, const void* d_queries, uint64_t n, void* d_send, uint64_t* d_slot,
+                          uint64_t* d_send_counts, void* cuda_stream);
+int rmi_shard_index_search(const rmi_shard_index* idx, const void* d_received, uint64_t m, uint64_t* d_answers,
+                           uint64_t* d_fallbacks, void* cuda_stream);
+int rmi_shard_index_gather(const rmi_shard_index* idx, const uint64_t* d_slot, const uint64_t* d_returned, uint64_t n,
+                           uint64_t* d_out, void* cuda_stream);
+/* The whole lower bound in one call, collective over c (every rank calls it, n = 0 allowed): route; all-gather of the
+ * world x world counts on the stream; one host read of them; grouped ncclSend / ncclRecv of the queries (a rank's own
+ * group included); search; grouped send / receive of the answers; gather.  c must have the index's world and rank.
+ * Returns after the exchanges are enqueued; the answers are in d_out when cuda_stream reaches them. */
+int rmi_shard_index_lower_bound(rmi_shard_index* idx, rmi_shard_comm* c, const void* d_queries, uint64_t n,
+                                uint64_t* d_out, uint64_t* d_fallbacks, void* cuda_stream);
+/* What the last rmi_shard_index_lower_bound on this index did (waits for it to finish).  phase_ms: CUDA-event times of
+ * route, count exchange with the host read, query exchange, search, answer exchange, gather. */
+typedef struct {
+  float phase_ms[6];
+  uint64_t queries_routed;     /* n: this rank's queries */
+  uint64_t queries_searched;   /* m: the queries this rank received and searched, its own included */
+  uint64_t queries_kept;       /* of the n, those this rank answered itself */
+} rmi_shard_lookup_stats;
+int rmi_shard_index_last_stats(const rmi_shard_index* idx, rmi_shard_lookup_stats* out);
+
 /* ---- `--bounded` support: rmi_lib::cache_fix (reference rmi_lib/src/cache_fix.rs:106-150) ----------
  * The error-bounded spline over key -> first-occurrence offset whose interpolation always lands in
  * the key's line (offset / line_size).  train_bounded (train/mod.rs:156-184) is then

@@ -753,16 +753,21 @@ int index_launch(const rmi_index* idx, const void* d_queries, uint64_t n, uint64
   CUDA_TRY(cudaGetLastError());
   return RMI_OK;
 }
-// The checks and the upload both kinds of index share: r's tables against ds, or against the knots of a bounded index
-// (num_knots > 0: r must have been trained on them).  Messages name `fn`.
-int index_check_tables(const rmi_result* r, const rmi_dataset* ds, uint64_t num_knots, const std::string& fn) {
+// The checks and the upload every kind of index shares.  First (it needs no dataset): r holds its leaf tables.
+int index_check_leaf_tables(const rmi_result* r, const std::string& fn) {
   if (!r->l1_params || !r->l1_errors)
     return fail(RMI_ERR_INVALID, fn + ": the result holds no leaf tables (trained with RMI_FLAG_STATS_ONLY)");
-  const uint64_t rows = num_knots ? num_knots : ds->n;
+  return RMI_OK;
+}
+// Then: r must have been trained on `rows` rows (the dataset's keys, the knots of a bounded index, or the keys of all
+// slabs of a range-partitioned one), which `holder` names in the message; `keys` is the number of keys the index
+// searches (0: an empty index).  Messages name `fn`.
+int index_check_tables(const rmi_result* r, uint64_t rows, const char* holder, uint64_t keys, const std::string& fn) {
+  if (int rc = index_check_leaf_tables(r, fn)) return rc;
   if (r->num_rmi_rows != rows)
     return fail(RMI_ERR_INVALID, fn + ": the result was trained on " + std::to_string(r->num_rmi_rows) + " keys, " +
-                                     (num_knots ? "the spline has " : "the dataset holds ") + std::to_string(rows));
-  if (ds->n == 0 || r->branching_factor == 0) return fail(RMI_ERR_INVALID, fn + ": empty index");
+                                     holder + std::to_string(rows));
+  if (keys == 0 || r->branching_factor == 0) return fail(RMI_ERR_INVALID, fn + ": empty index");
   if (lookup_top_group((int)r->l0_model_id) < 0 || lookup_leaf_group((int)r->l1_model_id) < 0)
     return fail(RMI_ERR_UNSUPPORTED, fn + ": unsupported model id (top " + std::to_string(r->l0_model_id) +
                                          ", leaf " + std::to_string(r->l1_model_id) + ")");
@@ -836,7 +841,8 @@ extern "C" {
 
 int rmi_index_create(const rmi_result* r, const rmi_dataset* ds, rmi_index** out) {
   if (!r || !ds || !out) return fail(RMI_ERR_INVALID, "rmi_index_create: null argument");
-  if (int rc = index_check_tables(r, ds, 0, "rmi_index_create")) return rc;
+  if (int rc = index_check_leaf_tables(r, "rmi_index_create")) return rc;
+  if (int rc = index_check_tables(r, ds->n, "the dataset holds ", ds->n, "rmi_index_create")) return rc;
   return index_upload(r, ds, nullptr, 0, 0, "rmi_index_create", out);
 }
 
@@ -847,7 +853,7 @@ int rmi_index_create_bounded(const rmi_result* r, const rmi_spline_point* knots,
   if (ds->key_type != RMI_KEY_U64) return fail(RMI_ERR_INVALID, fn + ": Can only construct a bounded RMI on u64 data");
   if (line_size == 0) return fail(RMI_ERR_INVALID, fn + ": line size 0");
   if (num_knots == 0) return fail(RMI_ERR_INVALID, fn + ": no spline knots");
-  if (int rc = index_check_tables(r, ds, num_knots, fn)) return rc;
+  if (int rc = index_check_tables(r, num_knots, "the spline has ", ds->n, fn)) return rc;
   for (uint64_t i = 0; i < num_knots; ++i) {
     if (knots[i].offset >= ds->n)
       return fail(RMI_ERR_INVALID, fn + ": knot " + std::to_string(i) + " has offset " + std::to_string(knots[i].offset) +
@@ -2308,6 +2314,296 @@ void rmi_shard_build_destroy(rmi_shard_build* b) {
   if (b->h_flags_all) cudaFreeHost(b->h_flags_all);
   for (cudaEvent_t e : {b->ev_off, b->ev_t0, b->ev_t1, b->ev_leaf0, b->ev_leaf1}) if (e) cudaEventDestroy(e);
   delete b;
+}
+
+}  // extern "C"
+
+// ---- lookups over a range-partitioned data set (DESIGN.md section 14) ----------------------------------------------
+constexpr int SHARD_LOOKUP_EVENTS = 7;   // around route, count exchange, query exchange, search, answer exchange, gather
+
+struct rmi_shard_index {
+  rmi_index* idx = nullptr;       // the tables, bound to this rank's slab
+  int world = 0, rank = 0;
+  uint64_t base = 0, n_global = 0;
+  // the route (kernels.h ShardRoute), as raw key bits
+  uint64_t first_bits[SHARD_ROUTE_MAX] = {};
+  unsigned char route_rank[SHARD_ROUTE_MAX] = {};
+  int route_count = 0;
+  uint64_t* h_counts = nullptr;   // world x world, pinned: the one host read of rmi_shard_index_lower_bound
+  cudaEvent_t ev[SHARD_LOOKUP_EVENTS] = {};
+  rmi_shard_lookup_stats last = {};
+  bool ran = false;
+};
+
+namespace {
+
+template <class T> ShardRoute<T> shard_route_of(const rmi_shard_index* si) {
+  ShardRoute<T> r;
+  memset(&r, 0, sizeof(r));
+  for (int k = 0; k < si->route_count; ++k) {
+    r.first[k] = key_from_bits<T>(si->first_bits[k]);
+    r.rank[k] = si->route_rank[k];
+  }
+  r.count = si->route_count;
+  return r;
+}
+
+// Frees a stream-ordered allocation when the scope ends (also on an early error return).
+struct PoolScratch {
+  void* p = nullptr;
+  cudaStream_t st = nullptr;
+  ~PoolScratch() { if (p) cudaFreeAsync(p, st); }
+};
+
+size_t round8(size_t b) { return (b + 7) & ~(size_t)7; }
+
+template <class T>
+int shard_lookup_route(const rmi_shard_index* si, const T* d_q, uint64_t n, T* d_send, u64* d_slot, u64* d_counts,
+                       cudaStream_t st) {
+  const u64 nb = shard_route_blocks(n), W = (u64)si->world;
+  PoolScratch s{nullptr, st};
+  if (n) CUDA_TRY(cudaMallocAsync(&s.p, nb * W * (sizeof(u64) + sizeof(u32)), st));
+  Launch L{st, si->idx->num_sms};
+  shard_route<T>(L, shard_route_of<T>(si), si->world, d_q, n, (u32*)((u64*)s.p + nb * W), (u64*)s.p, d_send, d_slot,
+                 d_counts);
+  CUDA_TRY(cudaGetLastError());
+  return RMI_OK;
+}
+
+template <class T>
+int shard_lookup_search(const rmi_shard_index* si, const T* d_recv, uint64_t m, u64* d_answers, u64* d_fallbacks,
+                        cudaStream_t st) {
+  if (m == 0) return RMI_OK;
+  const rmi_index* idx = si->idx;
+  const rmi_dataset* ds = idx->ds;
+  if (ds->n == 0)
+    return fail(RMI_ERR_INVALID, "rmi_shard_index_search: this rank holds no keys, so no query is routed to it");
+  PoolScratch s{nullptr, st};
+  CUDA_TRY(cudaMallocAsync(&s.p, 2 * sizeof(u64) * m, st));
+  u64* pos = (u64*)s.p;
+  Launch L{st, idx->num_sms};
+  lookup_batch<T>(L, idx->top, idx->leaf_kind, idx->d_records, idx->N, (const T*)ds->d_keys, si->n_global, d_recv, m,
+                  pos, pos + m, nullptr, false);
+  shard_search<T>(L, (const T*)ds->d_keys, ds->n, si->base, si->n_global, d_recv, m, pos, pos + m, d_answers,
+                  d_fallbacks);
+  CUDA_TRY(cudaGetLastError());
+  return RMI_OK;
+}
+
+template <class T>
+int shard_lookup_one_call(rmi_shard_index* si, rmi_shard_comm* c, const T* d_q, uint64_t n, u64* d_out, u64* d_fallbacks,
+                          cudaStream_t st) {
+  const NcclApi& nc = nccl_api();
+  const int W = si->world, me = si->rank;
+  const size_t kb = sizeof(T);
+  // send | slot | count matrix
+  PoolScratch s1{nullptr, st};
+  const size_t send_b = round8(n * kb), slot_b = n * sizeof(u64), mat_b = (size_t)W * W * sizeof(u64);
+  CUDA_TRY(cudaMallocAsync(&s1.p, send_b + slot_b + mat_b, st));
+  T* d_send = (T*)s1.p;
+  u64* d_slot = (u64*)((char*)s1.p + send_b);
+  u64* d_mat = (u64*)((char*)s1.p + send_b + slot_b);
+  cudaEventRecord(si->ev[0], st);
+  if (int rc = shard_lookup_route<T>(si, d_q, n, d_send, d_slot, d_mat + (size_t)me * W, st)) return rc;
+  cudaEventRecord(si->ev[1], st);
+  NCCL_TRY(nc.AllGather(d_mat + (size_t)me * W, d_mat, W, ncclUint64, c->comm, st));
+  CUDA_TRY(cudaMemcpyAsync(si->h_counts, d_mat, mat_b, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  cudaEventRecord(si->ev[2], st);
+  // row r of the matrix: what rank r sends to every rank
+  std::vector<u64> scount(W), rcount(W), soff(W + 1, 0), roff(W + 1, 0);
+  for (int p = 0; p < W; ++p) {
+    scount[p] = si->h_counts[(size_t)me * W + p];
+    rcount[p] = si->h_counts[(size_t)p * W + me];
+    soff[p + 1] = soff[p] + scount[p];
+    roff[p + 1] = roff[p] + rcount[p];
+  }
+  if (soff[W] != n) return fail(RMI_ERR_CUDA, "rmi_shard_index_lower_bound: the route's counts do not add up to the queries");
+  const u64 m = roff[W];
+  // received queries | their answers | the answers returned to this rank
+  PoolScratch s2{nullptr, st};
+  const size_t recv_b = round8(m * kb);
+  CUDA_TRY(cudaMallocAsync(&s2.p, recv_b + (m + n) * sizeof(u64) + 8, st));
+  T* d_recv = (T*)s2.p;
+  u64* d_ans = (u64*)((char*)s2.p + recv_b);
+  u64* d_ret = d_ans + m;
+  NCCL_TRY(nc.GroupStart());
+  for (int p = 0; p < W; ++p) {
+    if (scount[p]) NCCL_TRY(nc.Send(d_send + soff[p], scount[p] * kb, ncclUint8, p, c->comm, st));
+    if (rcount[p]) NCCL_TRY(nc.Recv(d_recv + roff[p], rcount[p] * kb, ncclUint8, p, c->comm, st));
+  }
+  NCCL_TRY(nc.GroupEnd());
+  cudaEventRecord(si->ev[3], st);
+  if (int rc = shard_lookup_search<T>(si, d_recv, m, d_ans, d_fallbacks, st)) return rc;
+  cudaEventRecord(si->ev[4], st);
+  NCCL_TRY(nc.GroupStart());
+  for (int p = 0; p < W; ++p) {
+    if (rcount[p]) NCCL_TRY(nc.Send(d_ans + roff[p], rcount[p], ncclUint64, p, c->comm, st));
+    if (scount[p]) NCCL_TRY(nc.Recv(d_ret + soff[p], scount[p], ncclUint64, p, c->comm, st));
+  }
+  NCCL_TRY(nc.GroupEnd());
+  cudaEventRecord(si->ev[5], st);
+  Launch L{st, si->idx->num_sms};
+  shard_gather(L, d_slot, d_ret, n, d_out);
+  CUDA_TRY(cudaGetLastError());
+  cudaEventRecord(si->ev[6], st);
+  si->last.queries_routed = n;
+  si->last.queries_searched = m;
+  si->last.queries_kept = scount[me];
+  si->ran = true;
+  return RMI_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int rmi_shard_index_create(const rmi_result* r, const rmi_dataset* local, const rmi_shard_ends* ends_all, int world,
+                           int rank, rmi_shard_index** out) {
+  const std::string fn = "rmi_shard_index_create";
+  g_last_error.clear();
+  if (!r || !local || !ends_all || !out) return fail(RMI_ERR_INVALID, fn + ": null argument");
+  if (world < 1 || world > SHARD_ROUTE_MAX - 1 || rank < 0 || rank >= world)
+    return fail(RMI_ERR_INVALID, fn + ": bad world or rank (0 <= rank < world <= 63)");
+  if (!r->l1_params || !r->l1_errors)
+    return fail(RMI_ERR_INVALID, fn + ": the result holds no leaf tables (trained with RMI_FLAG_STATS_ONLY, or received "
+                                      "by a rank other than 0 of an RMI_FLAG_SHARD_ROOT_ONLY build)");
+  if (ends_all[rank].n_local != local->n)
+    return fail(RMI_ERR_INVALID, fn + ": ends_all[" + std::to_string(rank) + "] describes " +
+                                     std::to_string(ends_all[rank].n_local) + " keys, the local dataset holds " +
+                                     std::to_string(local->n));
+  uint64_t total = 0, base = 0;
+  for (int p = 0; p < world; ++p) {
+    if (p == rank) base = total;
+    total += ends_all[p].n_local;
+  }
+  // the non-empty slabs must follow each other in key order: no slab's last key above the next one's first
+  int prev = -1;
+  const int bad = with_key_type(local->key_type, [&](auto k) {
+    using T = decltype(k);
+    for (int p = 0; p < world; ++p) {
+      if (!ends_all[p].n_local) continue;
+      if (prev >= 0 && key_from_bits<T>(ends_all[p].first_key_bits) < key_from_bits<T>(ends_all[prev].last_key_bits))
+        return p;
+      prev = p;
+    }
+    return -1;
+  });
+  if (bad >= 0)
+    return fail(RMI_ERR_INVALID, fn + ": the slabs are out of order (rank " + std::to_string(bad) +
+                                     "'s first key is below the last key of rank " + std::to_string(prev) + ")");
+  if (int rc = index_check_tables(r, total, "the slabs hold ", total, fn)) return rc;
+  rmi_index* idx = nullptr;
+  if (int rc = index_upload(r, local, nullptr, 0, 0, fn, &idx)) return rc;
+  auto* si = new rmi_shard_index();
+  si->idx = idx;
+  si->world = world;
+  si->rank = rank;
+  si->base = base;
+  si->n_global = total;
+  for (int p = 0; p < world; ++p) {
+    if (!ends_all[p].n_local) continue;
+    si->first_bits[si->route_count] = ends_all[p].first_key_bits;
+    si->route_rank[si->route_count++] = (unsigned char)p;
+  }
+  bool ok = cudaMallocHost((void**)&si->h_counts, sizeof(u64) * world * world) == cudaSuccess;
+  for (int q = 0; q < SHARD_LOOKUP_EVENTS; ++q) ok = ok && cudaEventCreate(&si->ev[q]) == cudaSuccess;
+  if (!ok) {
+    rmi_shard_index_destroy(si);
+    return fail(RMI_ERR_CUDA, fn + ": allocation failed");
+  }
+  *out = si;
+  return RMI_OK;
+}
+
+void rmi_shard_index_destroy(rmi_shard_index* si) {
+  if (!si) return;
+  rmi_index_destroy(si->idx);
+  if (si->h_counts) cudaFreeHost(si->h_counts);
+  for (cudaEvent_t e : si->ev) if (e) cudaEventDestroy(e);
+  delete si;
+}
+
+int rmi_shard_index_predict(const rmi_shard_index* si, const void* d_queries, uint64_t n, uint64_t* d_pos,
+                            uint64_t* d_err, void* cuda_stream) {
+  if (!si) return fail(RMI_ERR_INVALID, "rmi_shard_index_predict: null index");
+  if (int rc = index_check_call(si->idx, d_queries, n, d_pos, "rmi_shard_index_predict")) return rc;
+  if (n == 0) return RMI_OK;
+  const rmi_index* idx = si->idx;
+  CUDA_TRY(cudaSetDevice(idx->ds->device));
+  Launch L{(cudaStream_t)cuda_stream, idx->num_sms};
+  with_key_type(idx->ds->key_type, [&](auto k) {
+    using T = decltype(k);
+    lookup_batch<T>(L, idx->top, idx->leaf_kind, idx->d_records, idx->N, (const T*)idx->ds->d_keys, si->n_global,
+                    (const T*)d_queries, n, (u64*)d_pos, (u64*)d_err, nullptr, false);
+  });
+  CUDA_TRY(cudaGetLastError());
+  return RMI_OK;
+}
+
+int rmi_shard_index_route(const rmi_shard_index* si, const void* d_queries, uint64_t n, void* d_send, uint64_t* d_slot,
+                          uint64_t* d_send_counts, void* cuda_stream) {
+  const char* fn = "rmi_shard_index_route";
+  if (!si || !d_send_counts) return fail(RMI_ERR_INVALID, std::string(fn) + ": null index or count pointer");
+  if (n && (!d_queries || !d_send || !d_slot)) return fail(RMI_ERR_INVALID, std::string(fn) + ": null query, send or slot pointer");
+  CUDA_TRY(cudaSetDevice(si->idx->ds->device));
+  return with_key_type(si->idx->ds->key_type, [&](auto k) {
+    using T = decltype(k);
+    return shard_lookup_route<T>(si, (const T*)d_queries, n, (T*)d_send, (u64*)d_slot, (u64*)d_send_counts,
+                                 (cudaStream_t)cuda_stream);
+  });
+}
+
+int rmi_shard_index_search(const rmi_shard_index* si, const void* d_received, uint64_t m, uint64_t* d_answers,
+                           uint64_t* d_fallbacks, void* cuda_stream) {
+  if (!si) return fail(RMI_ERR_INVALID, "rmi_shard_index_search: null index");
+  if (int rc = index_check_call(si->idx, d_received, m, d_answers, "rmi_shard_index_search")) return rc;
+  CUDA_TRY(cudaSetDevice(si->idx->ds->device));
+  return with_key_type(si->idx->ds->key_type, [&](auto k) {
+    using T = decltype(k);
+    return shard_lookup_search<T>(si, (const T*)d_received, m, (u64*)d_answers, (u64*)d_fallbacks,
+                                  (cudaStream_t)cuda_stream);
+  });
+}
+
+int rmi_shard_index_gather(const rmi_shard_index* si, const uint64_t* d_slot, const uint64_t* d_returned, uint64_t n,
+                           uint64_t* d_out, void* cuda_stream) {
+  if (!si) return fail(RMI_ERR_INVALID, "rmi_shard_index_gather: null index");
+  if (n && (!d_slot || !d_returned || !d_out)) return fail(RMI_ERR_INVALID, "rmi_shard_index_gather: null pointer");
+  CUDA_TRY(cudaSetDevice(si->idx->ds->device));
+  Launch L{(cudaStream_t)cuda_stream, si->idx->num_sms};
+  shard_gather(L, (const u64*)d_slot, (const u64*)d_returned, n, (u64*)d_out);
+  CUDA_TRY(cudaGetLastError());
+  return RMI_OK;
+}
+
+int rmi_shard_index_lower_bound(rmi_shard_index* si, rmi_shard_comm* c, const void* d_queries, uint64_t n,
+                                uint64_t* d_out, uint64_t* d_fallbacks, void* cuda_stream) {
+  const char* fn = "rmi_shard_index_lower_bound";
+  g_last_error.clear();
+  if (!si || !c) return fail(RMI_ERR_INVALID, std::string(fn) + ": null index or communicator");
+  if (n && (!d_queries || !d_out)) return fail(RMI_ERR_INVALID, std::string(fn) + ": null query or output pointer");
+  if (c->world != si->world || c->rank != si->rank)
+    return fail(RMI_ERR_INVALID, std::string(fn) + ": the communicator is rank " + std::to_string(c->rank) + " of " +
+                                     std::to_string(c->world) + ", the index rank " + std::to_string(si->rank) + " of " +
+                                     std::to_string(si->world));
+  const NcclApi& nc = nccl_api();
+  if (!nc.ok) return fail(RMI_ERR_UNSUPPORTED, nc.error);
+  CUDA_TRY(cudaSetDevice(si->idx->ds->device));
+  return with_key_type(si->idx->ds->key_type, [&](auto k) {
+    using T = decltype(k);
+    return shard_lookup_one_call<T>(si, c, (const T*)d_queries, n, (u64*)d_out, (u64*)d_fallbacks,
+                                    (cudaStream_t)cuda_stream);
+  });
+}
+
+int rmi_shard_index_last_stats(const rmi_shard_index* si, rmi_shard_lookup_stats* out) {
+  if (!si || !out) return fail(RMI_ERR_INVALID, "rmi_shard_index_last_stats: null argument");
+  if (!si->ran) return fail(RMI_ERR_INVALID, "rmi_shard_index_last_stats: no rmi_shard_index_lower_bound has run");
+  CUDA_TRY(cudaEventSynchronize(si->ev[SHARD_LOOKUP_EVENTS - 1]));
+  *out = si->last;
+  for (int q = 0; q + 1 < SHARD_LOOKUP_EVENTS; ++q) CUDA_TRY(cudaEventElapsedTime(&out->phase_ms[q], si->ev[q], si->ev[q + 1]));
+  return RMI_OK;
 }
 
 }  // extern "C"

@@ -189,6 +189,31 @@ void lookup_bounded_batch(const Launch& L, const TopModel& top, int leaf_kind, c
                           const void* d_knots, u64 K, u64 line_size, const u64* keys, u64 n, const u64* d_queries,
                           u64 nq, u64* d_out, u64* d_out_err, u64* d_fallbacks, bool lower_bound);
 
+// ---- lookups over a range-partitioned data set (kernels_shard_lookup.cu, DESIGN.md section 14) -------------------
+// A query goes to the last non-empty rank whose first key is < q (the first non-empty rank if none is).
+constexpr int SHARD_ROUTE_MAX = 64;
+template <class T> struct ShardRoute {
+  T first[SHARD_ROUTE_MAX];                // first key of every non-empty rank, in rank order (non-decreasing)
+  unsigned char rank[SHARD_ROUTE_MAX];     // that rank
+  int count;                               // non-empty ranks, >= 1
+};
+// Per-block counts per rank of the route: d_block_counts holds world x shard_route_blocks(n) u32, d_block_offsets as
+// many u64.
+u64 shard_route_blocks(u64 n);
+// Three launches (none for n == 0, where d_send_counts is zeroed): d_send receives the n queries in per-rank segments
+// in rank order, d_send_counts[r] the length of rank r's segment, d_slot[i] the position of query i in d_send.
+template <class T>
+void shard_route(const Launch& L, const ShardRoute<T>& route, int world, const T* d_q, u64 n, u32* d_block_counts,
+                 u64* d_block_offsets, T* d_send, u64* d_slot, u64* d_send_counts);
+// Exact global lower bounds of m queries routed to this rank (slab keys[0, n_local) at global index base), from the
+// predictions d_pos / d_err of lookup_batch (predict, n = n_global).  One launch; *d_fallbacks (may be null) grows by
+// the number of windows that missed.  n_local >= 1.
+template <class T>
+void shard_search(const Launch& L, const T* keys, u64 n_local, u64 base, u64 n_global, const T* d_q, u64 m,
+                  const u64* d_pos, const u64* d_err, u64* d_out, u64* d_fallbacks);
+// d_out[i] = d_returned[d_slot[i]].  One launch (none for n == 0).
+void shard_gather(const Launch& L, const u64* d_slot, const u64* d_returned, u64 n, u64* d_out);
+
 // ---- the `--bounded` cache-fix scan (kernels_cachefix.cu, DESIGN.md section 12) ----------------------------------
 // Key indices per speculation chunk, and how many of a chunk's speculative knots the stitch can join.
 // (DESIGN.md section 12.3 gives the sweep.)

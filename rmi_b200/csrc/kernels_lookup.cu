@@ -8,7 +8,8 @@
 //               that does not bracket the answer falls back to a galloping search outward from its edge
 //               and is counted.  For every key of the data set the window brackets the answer (the
 //               reference's property, tests/simple_model_wiki/main.cpp:26-42), so the fallback only runs
-//               for queries the index was not trained on.
+//               for queries the index was not trained on.  The window search lives in lookup_search.cuh, shared
+//               with the search over a rank's slab of a range-partitioned data set (kernels_shard_lookup.cu).
 //
 // Thread mapping: a block takes a tile of LOOKUP_THREADS * LOOKUP_Q consecutive queries (grid-stride over
 // tiles); thread x owns queries x, x + LOOKUP_THREADS, ... of the tile, so every query load and result store
@@ -17,6 +18,7 @@
 #include <cstring>
 
 #include "kernels.h"
+#include "lookup_search.cuh"
 #include "spline.cuh"
 
 namespace rmi {
@@ -52,41 +54,6 @@ template <int LEAF> struct Rec {
     }
   }
 };
-
-// First index in [lo, hi) whose key is not < q, or hi.
-template <class T> __device__ __forceinline__ u64 search_range(const T* __restrict__ keys, u64 lo, u64 hi, T q) {
-  while (lo < hi) {
-    u64 mid = lo + ((hi - lo) >> 1);
-    if (keys[mid] < q) lo = mid + 1; else hi = mid;
-  }
-  return lo;
-}
-
-// The window [lo, hi] missed: the answer is below lo (!left_ok: keys[lo-1] is not < q) or above hi
-// (keys[hi] < q).  Gallop outward from that edge until the answer is bracketed, then search the bracket.
-template <class T>
-__device__ __noinline__ u64 lookup_fallback(const T* __restrict__ keys, u64 n, T q, u64 lo, u64 hi, bool left_ok) {
-  if (!left_ok) {
-    u64 R = lo - 1, step = 1, L = 0;   // answer <= R
-    while (true) {
-      if (R < step) { L = 0; break; }
-      u64 c = R - step;
-      if (keys[c] < q) { L = c + 1; break; }
-      R = c;
-      step <<= 1;
-    }
-    return search_range(keys, L, R, q);
-  }
-  u64 L = hi + 1, step = 1, R = n;     // answer >= L
-  while (true) {
-    if (n - L < step) { R = n; break; }
-    u64 c = L + step - 1;
-    if (!(keys[c] < q)) { R = c; break; }
-    L = c + 1;
-    step <<= 1;
-  }
-  return search_range(keys, L, R, q);
-}
 
 template <class T, int TOP, int LEAF>
 __global__ void __launch_bounds__(LOOKUP_THREADS)
@@ -136,45 +103,14 @@ k_lookup(const __grid_constant__ TopModel top, const ulonglong2* __restrict__ re
       continue;
     }
     // window [lo, hi] of candidate answers; the search covers keys [lo, hi)
-    u64 lo[Q], hi[Q], b[Q], len[Q];
-    T edge_l[Q], edge_r[Q];
+    u64 lo[Q], hi[Q];
 #pragma unroll
     for (int j = 0; j < Q; ++j) {
       lo[j] = pos[j] >= err[j] ? pos[j] - err[j] : 0;
       hi[j] = err[j] >= n - pos[j] ? n : pos[j] + err[j];
-      b[j] = lo[j];
-      len[j] = live[j] ? hi[j] - lo[j] : 0;
-      // the confirmation probes do not depend on the search: issued with its first probe
-      edge_l[j] = keys[lo[j] > 0 ? lo[j] - 1 : 0];
-      edge_r[j] = keys[hi[j] < n ? hi[j] : n - 1];
     }
-    while (true) {
-      bool more = false;
-#pragma unroll
-      for (int j = 0; j < Q; ++j) {
-        if (len[j] > 1) {
-          u64 h = len[j] >> 1;
-          b[j] = keys[b[j] + h] < q[j] ? b[j] + h : b[j];
-          len[j] -= h;
-          more |= len[j] > 1;
-        }
-      }
-      if (!more) break;
-    }
-#pragma unroll
-    for (int j = 0; j < Q; ++j) {
-      u64 r = b[j];
-      if (len[j] == 1) r += keys[r] < q[j] ? 1 : 0;
-      bool left_ok = lo[j] == 0 || edge_l[j] < q[j];
-      bool right_ok = hi[j] == n || !(edge_r[j] < q[j]);
-      if (live[j]) {
-        if (!(left_ok && (r < hi[j] || right_ok))) {
-          ++misses;
-          r = lookup_fallback(keys, n, q[j], lo[j], hi[j], left_ok);
-        }
-        __stcs(out + base + threadIdx.x + (u64)j * LOOKUP_THREADS, r);
-      }
-    }
+    window_search<T, Q>(keys, n, q, live, lo, hi, misses,
+                        [&](int j, u64 r) { __stcs(out + base + threadIdx.x + (u64)j * LOOKUP_THREADS, r); });
   }
   if (fallbacks) {
     misses = __reduce_add_sync(0xffffffffu, misses);

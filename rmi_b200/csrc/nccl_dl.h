@@ -2,7 +2,7 @@
 // on it: single-GPU users never load NCCL, and inside a torch process the already-loaded
 // libnccl.so.2 (the one torch.distributed uses) is the one that gets picked up.
 //
-// Only the handful of entry points the range-partitioned build issues are bound; types and
+// Only the handful of entry points the range-partitioned build and lookups issue are bound; types and
 // enumerators come from the system header (ABI-stable across the 2.x series).
 #pragma once
 #include <dlfcn.h>
@@ -21,6 +21,8 @@ struct NcclApi {
   ncclResult_t (*AllReduce)(const void*, void*, size_t, ncclDataType_t, ncclRedOp_t, ncclComm_t, cudaStream_t) = nullptr;
   ncclResult_t (*AllGather)(const void*, void*, size_t, ncclDataType_t, ncclComm_t, cudaStream_t) = nullptr;
   ncclResult_t (*Broadcast)(const void*, void*, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t) = nullptr;
+  ncclResult_t (*Send)(const void*, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t) = nullptr;
+  ncclResult_t (*Recv)(void*, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t) = nullptr;
   ncclResult_t (*GroupStart)() = nullptr;
   ncclResult_t (*GroupEnd)() = nullptr;
   ncclResult_t (*GetVersion)(int*) = nullptr;
@@ -49,6 +51,8 @@ inline const NcclApi& nccl_api() {
     bind(api.AllReduce, "ncclAllReduce");
     bind(api.AllGather, "ncclAllGather");
     bind(api.Broadcast, "ncclBroadcast");
+    bind(api.Send, "ncclSend");
+    bind(api.Recv, "ncclRecv");
     bind(api.GroupStart, "ncclGroupStart");
     bind(api.GroupEnd, "ncclGroupEnd");
     bind(api.GetVersion, "ncclGetVersion");

@@ -17,6 +17,9 @@ Data path per build (SURVEY.md section 8(e)):
     all-reduce SUM   N x (ppm+2) x 8 B  leaf parameters, error bounds, key counts (zero where not owned)
 The orchestration below is engine-agnostic: `CudaShardEngine` drives librmi_b200.so; the
 CPU tests (gloo, world_size 2) plug in a numpy engine to exercise exactly this host logic.
+
+ShardedRMIIndex serves lookups over the same slabs (DESIGN.md section 14): a query goes to the rank whose slab holds
+its lower bound, is searched there, and its global answer comes back.
 """
 from __future__ import annotations
 
@@ -292,6 +295,9 @@ class CudaShardEngine:
         api._check(self.lib.rmi_shard_finish(self._build, int(flags), C.byref(res)))
         return api.result_from_pointer(res, self._spec)
 
+    def lookup_index(self, trained, ends_all: np.ndarray, world: int, rank: int) -> "CudaShardIndex":
+        return CudaShardIndex(self, trained, ends_all, world, rank)
+
     def end(self):
         if self._build is not None:
             self.lib.rmi_shard_build_destroy(self._build)
@@ -347,6 +353,23 @@ def native_comm(group, device: torch.device, single_rank_ok: bool = False):
     return comm
 
 
+def gather_ends(data, eng, group) -> np.ndarray:
+    """Every rank's rmi_shard_ends (first / last key bits, last run start, n_local, no_dups) as a (world, 5) uint64
+    array, identical on every rank.  Collective on the first call; cached on `data` (the keys are immutable)."""
+    ends_all = getattr(data, "_ends_all", None)
+    if ends_all is None:
+        rank, world = _world(group)
+        e = torch.tensor(np.array(eng.ends(), dtype=np.uint64).view(np.int64), dtype=torch.int64, device=eng.device)
+        gathered = [torch.empty_like(e) for _ in range(world)]
+        if world > 1:
+            dist.all_gather(gathered, e, group=group)
+        else:
+            gathered = [e]
+        ends_all = torch.stack(gathered).cpu().numpy().view(np.uint64)
+        data._ends_all = ends_all
+    return ends_all
+
+
 def train_sharded(data, model_spec: str, num_leaves: int, flags: int = 0, group=None, engine=None, counts: bool = True,
                   native: bool | None = None):
     """rmi_lib::train on a range-partitioned key array; returns the full TrainedRMI on every rank.
@@ -372,14 +395,7 @@ def train_sharded(data, model_spec: str, num_leaves: int, flags: int = 0, group=
     # 1. what every rank's slab looks like at its ends (cached on the data object: the data is immutable)
     layout = getattr(data, "_layout", None)
     if layout is None or layout[0] != N:
-        e = torch.tensor(np.array(eng.ends(), dtype=np.uint64).view(np.int64), dtype=torch.int64, device=dev)
-        gathered = [torch.empty_like(e) for _ in range(world)]
-        if world > 1:
-            dist.all_gather(gathered, e, group=group)
-        else:
-            gathered = [e]
-        ends_all = torch.stack(gathered).cpu().numpy().view(np.uint64)
-        layout = (N, plan_global_layout(ends_all, data.key_type, N))
+        layout = (N, plan_global_layout(gather_ends(data, eng, group), data.key_type, N))
         data._layout = layout
     info = layout[1][rank]
     bases, n_global = info["bases"], info["n_global"]
@@ -526,3 +542,185 @@ def _min_halo_capacity(data, group, world, dev):
         cap = int(t.item())
         data._min_cap = cap
     return cap
+
+
+# ---- lookups over the slabs (include/rmi_b200.h rmi_shard_index_*, DESIGN.md section 14) ------------------------------
+
+class _LookupStats(C.Structure):
+    _fields_ = [("phase_ms", C.c_float * 6), ("queries_routed", C.c_uint64), ("queries_searched", C.c_uint64),
+                ("queries_kept", C.c_uint64)]
+
+
+LOOKUP_PHASES = ("route", "count_exchange", "query_exchange", "search", "answer_exchange", "gather")
+
+
+class CudaShardIndex:
+    """One rank's side of the lookups over the slabs on librmi_b200.so (rmi_shard_index_*).  Every call enqueues on
+    the current torch stream of the data's device and returns device tensors."""
+
+    def __init__(self, eng: CudaShardEngine, trained, ends_all: np.ndarray, world: int, rank: int):
+        L = self.lib = api.load_library()
+        L.rmi_shard_index_create.argtypes = [C.POINTER(api._Result), C.c_void_p, C.POINTER(_Ends), C.c_int, C.c_int,
+                                             C.POINTER(C.c_void_p)]
+        L.rmi_shard_index_destroy.argtypes = [C.c_void_p]
+        L.rmi_shard_index_predict.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.rmi_shard_index_route.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p]
+        L.rmi_shard_index_search.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.rmi_shard_index_gather.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]
+        L.rmi_shard_index_lower_bound.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p,
+                                                  C.c_void_p, C.c_void_p]
+        L.rmi_shard_index_last_stats.argtypes = [C.c_void_p, C.POINTER(_LookupStats)]
+        self.device = eng.device
+        self.world = world
+        self._ds = eng.ds            # the slab the index searches: kept alive with it
+        self._trained = trained
+        ends = (_Ends * world)(*[_Ends(*(int(v) for v in row[:5])) for row in ends_all])
+        self._h = C.c_void_p()
+        api._check(L.rmi_shard_index_create(api._result_ptr(trained), eng.ds._h, ends, world, rank, C.byref(self._h)))
+
+    def _stream(self):
+        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream or None)
+
+    def _u64(self, n: int) -> torch.Tensor:
+        return torch.empty(n, dtype=torch.int64, device=self.device)
+
+    def predict(self, q: torch.Tensor):
+        pos, err = self._u64(q.numel()), self._u64(q.numel())
+        api._check(self.lib.rmi_shard_index_predict(self._h, q.data_ptr(), q.numel(), pos.data_ptr(), err.data_ptr(),
+                                                    self._stream()))
+        return pos, err
+
+    def route(self, q: torch.Tensor):
+        send, slot, counts = torch.empty_like(q), self._u64(q.numel()), self._u64(self.world)
+        api._check(self.lib.rmi_shard_index_route(self._h, q.data_ptr(), q.numel(), send.data_ptr(), slot.data_ptr(),
+                                                  counts.data_ptr(), self._stream()))
+        return send, slot, counts
+
+    def search(self, recv: torch.Tensor):
+        answers, fb = self._u64(recv.numel()), torch.zeros(1, dtype=torch.int64, device=self.device)
+        api._check(self.lib.rmi_shard_index_search(self._h, recv.data_ptr(), recv.numel(), answers.data_ptr(),
+                                                   fb.data_ptr(), self._stream()))
+        return answers, fb
+
+    def gather(self, slot: torch.Tensor, returned: torch.Tensor):
+        out = self._u64(slot.numel())
+        api._check(self.lib.rmi_shard_index_gather(self._h, slot.data_ptr(), returned.data_ptr(), slot.numel(),
+                                                   out.data_ptr(), self._stream()))
+        return out
+
+    def lower_bound_native(self, comm, q: torch.Tensor):
+        out, fb = self._u64(q.numel()), torch.zeros(1, dtype=torch.int64, device=self.device)
+        api._check(self.lib.rmi_shard_index_lower_bound(self._h, comm, q.data_ptr(), q.numel(), out.data_ptr(),
+                                                        fb.data_ptr(), self._stream()))
+        return out, fb
+
+    def last_stats(self) -> dict:
+        st = _LookupStats()
+        api._check(self.lib.rmi_shard_index_last_stats(self._h, C.byref(st)))
+        return dict(phase_ms=dict(zip(LOOKUP_PHASES, (float(x) for x in st.phase_ms))),
+                    queries_routed=int(st.queries_routed), queries_searched=int(st.queries_searched),
+                    queries_kept=int(st.queries_kept))
+
+    def close(self):
+        if getattr(self, "_h", None) and self._h.value:
+            self.lib.rmi_shard_index_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class ShardedRMIIndex:
+    """A trained RMI served over range-partitioned keys: rank r holds the r-th slab (`data`, a ShardedTrainingData)
+    and the whole model.  `trained` is any TrainedRMI of the whole key set: from train_sharded, from rmi_train of the
+    whole keys, or loaded from an artefact (ShardedRMIIndex.load).  Constructing it gathers the ends of every slab once
+    (cached on `data`, shared with train_sharded).
+
+    predict(q) -> (pos, err): the model's prediction over the whole key set; local, no communication.
+    lower_bound(q): exact global lower bounds (np.searchsorted(all_keys, q, "left"); 0 for NaN); collective: every
+    rank calls it, with its own queries (0 is fine).  Under an NCCL group it is one library call (route, exchanges,
+    search, gather on the stream); otherwise (gloo, native=False) the phases are driven here with all_to_all_single.
+    Queries are a 1-D tensor on the data's device in its storage dtype (int64 for uint64 keys, int32, float64);
+    results are int64 tensors (uint64 values) there.  The orchestration is engine-agnostic: the CPU tests plug in a
+    numpy engine (`engine=`)."""
+
+    def __init__(self, trained, data, group=None, engine=None):
+        eng = engine if engine is not None else data.engine
+        self.group = group if group is not None else getattr(data, "group", None)
+        self.rank, self.world = _world(self.group)
+        self.device = eng.device
+        self.key_type = data.key_type
+        self.index = eng.lookup_index(trained, gather_ends(data, eng, self.group), self.world, self.rank)
+
+    @classmethod
+    def load(cls, namespace: str, data, out_dir: str = ".", data_dir: str = "rmi_data", group=None) -> "ShardedRMIIndex":
+        """load_rmi of a generated artefact, served over the slabs: train once, serve over shards."""
+        trained, cf = api.load_rmi(namespace, out_dir, data_dir)
+        if cf is not None:
+            raise api.RMIError("a --bounded artefact cannot be served over range-partitioned keys: its cache-fix spline "
+                               "indexes the whole key array on one GPU")
+        if trained.last_layer_max_l1s is None:
+            raise api.RMIError("a --no-errors artefact cannot be served over range-partitioned keys: its error bounds "
+                               "would have to be measured over the slabs, and a sharded evaluate does not exist")
+        want = (api.KEY_F64,) if trained.key_type == api.KEY_F64 else (api.KEY_U64, api.KEY_U32)
+        if data.key_type not in want:
+            raise api.RMIError(f"the artefact's lookup takes {'double' if trained.key_type == api.KEY_F64 else 'uint64_t'} "
+                               f"keys, the data holds {np.dtype(_NP_OF_KEY[data.key_type])}")
+        return cls(trained, data, group)
+
+    def _queries(self, q: torch.Tensor) -> torch.Tensor:
+        want = _TORCH_OF_KEY[self.key_type]
+        if not isinstance(q, torch.Tensor) or q.dtype != want or q.dim() != 1 or q.device != self.device:
+            got = f"{q.dtype} on {q.device}" if isinstance(q, torch.Tensor) else type(q).__name__
+            raise TypeError(f"queries must be a 1-D {want} tensor on {self.device}, got {got}")
+        return q.contiguous()
+
+    def predict(self, q: torch.Tensor):
+        """(pos, err) per query over the whole key set."""
+        return self.index.predict(self._queries(q))
+
+    def lower_bound(self, q: torch.Tensor, return_fallbacks: bool = False, native: bool | None = None):
+        """Exact global lower bounds of this rank's queries.  return_fallbacks: also the number of windows that
+        missed among the queries THIS rank searched (the sum over ranks covers every query once)."""
+        q = self._queries(q)
+        comm = None
+        if native is not False and isinstance(self.index, CudaShardIndex):
+            comm = native_comm(self.group, self.device, single_rank_ok=native is True)
+            if native is True and comm is None:
+                raise api.RMIError("native=True needs an NCCL process group (or a single rank) and a loadable libnccl.so.2")
+        if comm is not None:
+            out, fb = self.index.lower_bound_native(comm, q)
+        else:
+            out, fb = self._lower_bound_phases(q)
+        return (out, int(fb)) if return_fallbacks else out
+
+    def _lower_bound_phases(self, q: torch.Tensor):
+        idx, group = self.index, self.group
+        send, slot, counts = idx.route(q)
+        if self.world <= 1:
+            answers, fb = idx.search(send)
+            return idx.gather(slot, answers), fb
+        # gloo cannot exchange device memory (one-GPU test boxes): stage through the host there
+        stage = self.device.type == "cuda" and dist.get_backend(group) == "gloo"
+        c_send = counts.cpu() if stage else counts
+        c_recv = torch.empty_like(c_send)
+        dist.all_to_all_single(c_recv, c_send, group=group)
+        scount, rcount = c_send.tolist(), c_recv.tolist()      # the one host read of the counts
+        recv = self._exchange(send, rcount, scount, stage)
+        answers, fb = idx.search(recv)
+        returned = self._exchange(answers, scount, rcount, stage)
+        return idx.gather(slot, returned), fb
+
+    def _exchange(self, x: torch.Tensor, out_splits: list[int], in_splits: list[int], stage: bool) -> torch.Tensor:
+        src = x.cpu() if stage else x
+        out = torch.empty(sum(out_splits), dtype=x.dtype, device=src.device)
+        dist.all_to_all_single(out, src, output_split_sizes=out_splits, input_split_sizes=in_splits, group=self.group)
+        return out.to(self.device) if stage else out
+
+    def close(self):
+        if hasattr(self.index, "close"):
+            self.index.close()
