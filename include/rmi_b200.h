@@ -151,6 +151,17 @@ int rmi_train(const rmi_dataset* ds, const char* model_spec, uint64_t branch_fac
 int rmi_train_with_top(const rmi_dataset* ds, const char* model_spec, uint64_t branch_factor, uint32_t flags,
                        const double* l0_fparams, uint32_t n_fparams, rmi_result** out);
 void rmi_result_free(rmi_result* r);
+/* The calls that take a given trained result (rmi_evaluate, rmi_index_create, rmi_index_create_bounded,
+ * rmi_shard_index_create) first check it the same way, before they read a dataset, and refuse it with the same code
+ * and the message "<function>: <reason>":
+ *   RMI_ERR_INVALID      no l1_params, or (the indexes, which serve the error bounds) no l1_errors: "the result holds
+ *                        no leaf tables ..." (RMI_FLAG_STATS_ONLY, or a rank other than 0 of an
+ *                        RMI_FLAG_SHARD_ROOT_ONLY build);
+ *   RMI_ERR_INVALID      a top or leaf model id that rmi_train does not offer there (radix tables: radix8, 18, 22, 26,
+ *                        28 only; radix, bradix and histogram only as the top): "unknown model id";
+ *   RMI_ERR_UNSUPPORTED  a radix-table leaf, with rmi_train's message;
+ *   RMI_ERR_INVALID      l1_params_per_model not the leaf model's; a radix table absent or not of 2^l0_table_bits
+ *                        entries; histogram pivots absent or empty; l0_array1_len > 0 with no l0_array1. */
 /* The reference's error pass, lower-bound widening and statistics (two_layer.rs:205-284) of r's top and leaf tables
  * over ds's keys.  Parameters are never refitted or replaced: the returned result holds r's tables bit for bit,
  * with l1_errors, (with RMI_FLAG_LEAF_COUNTS) l1_counts and the summary statistics measured on ds, and
@@ -178,16 +189,17 @@ int rmi_train_stats_batch(const rmi_dataset* ds, const char* top_model, const ch
 typedef struct rmi_index rmi_index;
 /* One knot of a `--bounded` RMI's cache-fix spline (rmi_cache_fix below): a key and its first-occurrence offset. */
 typedef struct { uint64_t key, offset; } rmi_spline_point;
-/* Upload r's top model (incl. radix table / histogram arrays) and its leaf tables, packed, to ds's device and
- * bind them to ds's keys.  r must hold the leaf tables (not RMI_FLAG_STATS_ONLY) and r->num_rmi_rows must equal
- * rmi_dataset_len(ds); ds must outlive the index.  Immutable: concurrent calls on different streams are fine. */
+/* Upload r's top model (incl. radix table / histogram pivots) and its leaf tables, packed, to ds's device and
+ * bind them to ds's keys.  r must pass the checks of a given result (above, before rmi_evaluate) and r->num_rmi_rows
+ * must equal rmi_dataset_len(ds); ds must outlive the index.  Immutable: concurrent calls on different streams are
+ * fine. */
 int rmi_index_create(const rmi_result* r, const rmi_dataset* ds, rmi_index** out);
 /* A `--bounded` RMI (train_bounded, below): r is the RMI over the K knots of the cache-fix spline
  * (r->num_rmi_rows == num_knots), knots are those K {key, offset} points (the _L2_PARAMETERS layout, keys strictly
  * increasing, offsets non-decreasing and < n), ds holds the n u64 keys the spline was fitted to.  The knots are
  * copied to the device (the caller's array need not outlive the call); ds must outlive the index.  Refused (before
- * any device work): a non-u64 dataset, line_size 0, no knots, knots out of order or past the keys, and every case
- * rmi_index_create refuses.  The other rmi_index_* calls take either kind of index; on a bounded one:
+ * any device work): every result rmi_index_create refuses, then a non-u64 dataset, line_size 0, no knots, knots out
+ * of order or past the keys.  The other rmi_index_* calls take either kind of index; on a bounded one:
  *   predict      the generated spline lookup(q, &err) (codegen.rs:410-437): (start, e) = the RMI's predict over the
  *                knots; res = the first knot in [start-e, min(start+e, K)) whose key is not < q (that upper end if
  *                none); res == K: pos = n-1; res == 0: pos = 0 (the generated code reads knots[-1] there);
@@ -319,11 +331,11 @@ int rmi_shard_train(rmi_shard_build* b, rmi_shard_comm* c, uint32_t flags, rmi_r
  * 8-byte answers back.
  *
  * rmi_shard_index_create uploads r's tables as rmi_index_create does and binds them to `local`.  ends_all holds every
- * rank's rmi_shard_ends (rmi_shard_ends_get, gathered over the ranks).  Refused with RMI_ERR_INVALID before any device
- * work: a null argument; rank / world out of range (1 <= world <= 63); a result without leaf tables (RMI_FLAG_STATS_ONLY,
- * or a rank other than 0 of an RMI_FLAG_SHARD_ROOT_ONLY build); ends_all[rank].n_local != rmi_dataset_len(local);
- * r->num_rmi_rows != the sum of n_local; non-empty slabs out of key order (a slab's last key above the next one's
- * first); and every model rmi_index_create refuses.  local must outlive the index. */
+ * rank's rmi_shard_ends (rmi_shard_ends_get, gathered over the ranks).  Refused before any device work, in this
+ * order: a null argument (RMI_ERR_INVALID); every result rmi_index_create refuses (the checks of a given result,
+ * before rmi_evaluate); then with RMI_ERR_INVALID: rank / world out of range (1 <= world <= 63);
+ * ends_all[rank].n_local != rmi_dataset_len(local); non-empty slabs out of key order (a slab's last key above the
+ * next one's first); r->num_rmi_rows != the sum of n_local.  local must outlive the index. */
 typedef struct rmi_shard_index rmi_shard_index;
 int rmi_shard_index_create(const rmi_result* r, const rmi_dataset* local, const rmi_shard_ends* ends_all, int world,
                            int rank, rmi_shard_index** out);

@@ -89,6 +89,14 @@ const ModelName* find_model(const std::string& s) {
   return nullptr;
 }
 
+// The model table entry of a result's model id: a radix table by its table bits, except for a leaf, whose width a
+// result does not record (any radix table matches, and check_leaf refuses it).
+const ModelName* model_of(uint32_t kind, uint32_t table_bits, bool leaf) {
+  for (const auto& m : kModels)
+    if (m.kind == (int)kind && (kind != M_RADIX_TABLE || leaf || m.table_bits == (int)table_bits)) return &m;
+  return nullptr;
+}
+
 // ---- the reference's checks of a model spec and of a build's arguments, in rmi_train's order ----------------
 int find_layer(const std::string& name, bool is_root, const ModelName** out) {
   const ModelName* m = find_model(name);
@@ -98,9 +106,10 @@ int find_layer(const std::string& name, bool is_root, const ModelName** out) {
   return RMI_OK;
 }
 
-int check_leaf(const ModelName* leaf) {
+// who: what the message starts with ("" for a build)
+int check_leaf(const ModelName* leaf, const std::string& who = "") {
   if (leaf->kind == M_RADIX_TABLE)
-    return fail(RMI_ERR_UNSUPPORTED, "radix tables are only offered as the top model in this build");
+    return fail(RMI_ERR_UNSUPPORTED, who + "radix tables are only offered as the top model in this build");
   return RMI_OK;
 }
 
@@ -127,6 +136,34 @@ int check_build(uint64_t n, uint64_t N, bool sorted) {
   if (N < 1) return fail(RMI_ERR_PANIC, "branching factor must be at least 1");
   if (n == 0) return fail(RMI_ERR_PANIC, "start index was 0 but end index was 0");
   if (!sorted) return fail(RMI_ERR_PANIC, "keys are not sorted in ascending order");
+  return RMI_OK;
+}
+
+// The check of a given trained result that rmi_evaluate and the indexes make first, before they read a dataset: the
+// leaf tables (with the error bounds if the caller serves them), models of the model table with a leaf model that is
+// not root-only, and the top model's tables.  Every (kind, table bits) it accepts has a lookup kernel
+// (lookup_top_group / lookup_leaf_group).  *top / *leaf (may be null) receive r's models.  Messages name fn.
+int check_result(const rmi_result* r, bool needs_errors, const std::string& fn, const ModelName** top = nullptr,
+                 const ModelName** leaf = nullptr) {
+  if (!r->l1_params || (needs_errors && !r->l1_errors))
+    return fail(RMI_ERR_INVALID, fn + ": the result holds no leaf tables (RMI_FLAG_STATS_ONLY, or a rank other than 0 "
+                                      "of an RMI_FLAG_SHARD_ROOT_ONLY build)");
+  const ModelName* t = model_of(r->l0_model_id, r->l0_table_bits, false);
+  const ModelName* l = model_of(r->l1_model_id, 0, true);
+  if (!t || !l || l->root_only)
+    return fail(RMI_ERR_INVALID, fn + ": unknown model id (top " + std::to_string(r->l0_model_id) + ", leaf " +
+                                     std::to_string(r->l1_model_id) + ")");
+  if (int rc = check_leaf(l, fn + ": ")) return rc;
+  if (r->l1_params_per_model != (uint32_t)leaf_params_per_model(l->kind))
+    return fail(RMI_ERR_INVALID, fn + ": wrong number of leaf parameters");
+  if (t->kind == M_RADIX_TABLE && (!r->l0_table32 || r->l0_table32_len != ((uint64_t)1 << t->table_bits)))
+    return fail(RMI_ERR_INVALID, fn + ": radix table missing or of the wrong size");
+  if (t->kind == M_HISTOGRAM && (!r->l0_array2 || !r->l0_array2_len))
+    return fail(RMI_ERR_INVALID, fn + ": histogram pivots missing");
+  if (t->kind == M_HISTOGRAM && r->l0_array1_len && !r->l0_array1)
+    return fail(RMI_ERR_INVALID, fn + ": histogram radix index missing");
+  if (top) *top = t;
+  if (leaf) *leaf = l;
   return RMI_OK;
 }
 
@@ -282,11 +319,17 @@ struct ResultBox {
 
 namespace {
 
-// The device tables of a table top: radix8..28's hint table, the histogram's pivots and radix index.
+// An Alloc for TopTables that outlive the call (rmi_index, rmi_shard_build): null if cudaMalloc failed.
+void* device_alloc(size_t bytes) {
+  void* p = nullptr;
+  return cudaMalloc(&p, bytes) == cudaSuccess ? p : nullptr;
+}
+
+// The device tables of a table top: radix8..28's hint table, the histogram's pivots and, in a build, its radix index.
 struct TopTables {
   u32* t32 = nullptr;
-  u64* pivots = nullptr;        // hist_bins + 1
-  u64* radix_index = nullptr;   // ri_len
+  u64* pivots = nullptr;        // hist_bins (+ 1 in a build)
+  u64* radix_index = nullptr;   // ri_len; a build's output only: no kernel reads it through TopModel
   u64 t32_len = 0, ri_len = 0;
   u64 hist_bins = 0, hist_ipb = 0;
 
@@ -307,24 +350,24 @@ struct TopTables {
     return true;
   }
 
-  // The tables of a given result's top model (rmi_evaluate): allocated with alloc and uploaded on st.
-  template <class Alloc> bool upload(const rmi_result& r, cudaStream_t st, Alloc&& alloc) {
+  // The tables of a given result's top model (check_result passed), allocated with alloc and copied on st: the first
+  // CUDA error, cudaErrorMemoryAllocation where alloc returned null.  Of the histogram's radix index only the length
+  // is kept: the lookups and the error pass read the pivots alone.
+  template <class Alloc> cudaError_t upload(const rmi_result& r, cudaStream_t st, Alloc&& alloc) {
     if (r.l0_model_id == M_RADIX_TABLE) {
       t32_len = r.l0_table32_len;
       t32 = (u32*)alloc(sizeof(u32) * t32_len);
-      if (!t32) return false;
-      cudaMemcpyAsync(t32, r.l0_table32, sizeof(u32) * t32_len, cudaMemcpyHostToDevice, st);
+      if (!t32) return cudaErrorMemoryAllocation;
+      return cudaMemcpyAsync(t32, r.l0_table32, sizeof(u32) * t32_len, cudaMemcpyHostToDevice, st);
     }
     if (r.l0_model_id == M_HISTOGRAM) {
       hist_bins = r.l0_array2_len;
       ri_len = r.l0_array1_len;
       pivots = (u64*)alloc(sizeof(u64) * hist_bins);
-      radix_index = (u64*)alloc(sizeof(u64) * ri_len);
-      if (!pivots || !radix_index) return false;
-      cudaMemcpyAsync(pivots, r.l0_array2, sizeof(u64) * hist_bins, cudaMemcpyHostToDevice, st);
-      cudaMemcpyAsync(radix_index, r.l0_array1, sizeof(u64) * ri_len, cudaMemcpyHostToDevice, st);
+      if (!pivots) return cudaErrorMemoryAllocation;
+      return cudaMemcpyAsync(pivots, r.l0_array2, sizeof(u64) * hist_bins, cudaMemcpyHostToDevice, st);
     }
-    return true;
+    return cudaSuccess;
   }
 
   // The TopModel of a given result, pointing at the tables upload() placed.
@@ -337,9 +380,15 @@ struct TopTables {
     for (int q = 0; q < 4; ++q) { h.f[q] = r.l0_fparams[q]; h.ip[q] = r.l0_iparams[q]; }
     h.t32 = t32;
     h.pivots = pivots;
-    h.radix_index = radix_index;
     h.npivots = hist_bins;
     return h;
+  }
+
+  // Frees tables placed with device_alloc.
+  void free_device() {
+    cudaFree(t32);
+    cudaFree(pivots);
+    cudaFree(radix_index);
   }
 
   // The TopModel a build starts from; f: nf injected top parameters, or null.
@@ -351,7 +400,6 @@ struct TopTables {
     h.table_bits = top.table_bits;
     h.t32 = t32;
     h.pivots = pivots;
-    h.radix_index = radix_index;
     h.npivots = hist_bins;
     if (top.kind == M_HISTOGRAM) h.ip[0] = hist_bins;
     for (uint32_t q = 0; f && q < nf && q < 4; ++q) h.f[q] = f[q];
@@ -367,7 +415,8 @@ bool reserve_result(ResultBox* box, const TopTables* tables, uint64_t N, int ppm
   if (leaves) ok = ok && box->l1_params.resize((size_t)N * ppm) && box->l1_errors.resize(N);
   if (leaves && counts) ok = ok && box->l1_counts.resize(N);
   if (tables && tables->t32_len) ok = ok && box->table32.resize(tables->t32_len);
-  if (tables && tables->ri_len) ok = ok && box->arr1.resize(tables->ri_len) && box->arr2.resize(tables->hist_bins);
+  if (tables && tables->ri_len) ok = ok && box->arr1.resize(tables->ri_len);
+  if (tables && tables->hist_bins) ok = ok && box->arr2.resize(tables->hist_bins);
   return ok;
 }
 const char* const kPinnedFailed = "pinned host allocation for the results failed";
@@ -703,13 +752,14 @@ void rmi_result_free(rmi_result* r) { delete reinterpret_cast<ResultBox*>(r); }
 // memory) and one packed record per leaf (kernels.h: lookup_record_bytes).  Immutable after creation.
 struct rmi_index {
   const rmi_dataset* ds = nullptr;
-  TopModel top;              // t32 / pivots / radix_index point at the device copies below
+  TopTables tables;          // the top model's tables, on the device
+  TopModel top;              // points at `tables`
   int leaf_kind = 0;
   uint64_t N = 0;
+  // the positions the model predicts over: ds->n, or the whole key set's size for the index inside an
+  // rmi_shard_index, which only predicts (shard_search turns the predictions into lower bounds in the slab)
+  uint64_t n = 0;
   void* d_records = nullptr;
-  u32* d_t32 = nullptr;
-  u64* d_pivots = nullptr;
-  u64* d_radix_index = nullptr;
   int num_sms = 0;
   // a bounded (cache-fix) index: the RMI above runs over K knots; null / 0 for a plain index
   void* d_knots = nullptr;   // K x rmi_spline_point
@@ -719,10 +769,8 @@ struct rmi_index {
 
 namespace {
 void index_free_device(rmi_index* idx) {
+  idx->tables.free_device();
   cudaFree(idx->d_records);
-  cudaFree(idx->d_t32);
-  cudaFree(idx->d_pivots);
-  cudaFree(idx->d_radix_index);
   cudaFree(idx->d_knots);
 }
 
@@ -740,49 +788,32 @@ int index_launch(const rmi_index* idx, const void* d_queries, uint64_t n, uint64
   Launch L{(cudaStream_t)cuda_stream, idx->num_sms};
   if (idx->d_knots) {
     lookup_bounded_batch(L, idx->top, idx->leaf_kind, idx->d_records, idx->N, idx->d_knots, idx->K, idx->line_size,
-                         (const u64*)ds->d_keys, ds->n, (const u64*)d_queries, n, (u64*)d_out, (u64*)d_err,
+                         (const u64*)ds->d_keys, idx->n, (const u64*)d_queries, n, (u64*)d_out, (u64*)d_err,
                          (u64*)d_fallbacks, lower_bound);
     CUDA_TRY(cudaGetLastError());
     return RMI_OK;
   }
   with_key_type(ds->key_type, [&](auto k) {
     using T = decltype(k);
-    lookup_batch<T>(L, idx->top, idx->leaf_kind, idx->d_records, idx->N, (const T*)ds->d_keys, ds->n,
+    lookup_batch<T>(L, idx->top, idx->leaf_kind, idx->d_records, idx->N, (const T*)ds->d_keys, idx->n,
                     (const T*)d_queries, n, (u64*)d_out, (u64*)d_err, (u64*)d_fallbacks, lower_bound);
   });
   CUDA_TRY(cudaGetLastError());
   return RMI_OK;
 }
-// The checks and the upload every kind of index shares.  First (it needs no dataset): r holds its leaf tables.
-int index_check_leaf_tables(const rmi_result* r, const std::string& fn) {
-  if (!r->l1_params || !r->l1_errors)
-    return fail(RMI_ERR_INVALID, fn + ": the result holds no leaf tables (trained with RMI_FLAG_STATS_ONLY)");
-  return RMI_OK;
-}
-// Then: r must have been trained on `rows` rows (the dataset's keys, the knots of a bounded index, or the keys of all
-// slabs of a range-partitioned one), which `holder` names in the message; `keys` is the number of keys the index
-// searches (0: an empty index).  Messages name `fn`.
+// After check_result, the checks every kind of index shares: r must have been trained on `rows` rows (the dataset's
+// keys, the knots of a bounded index, or the keys of all slabs of a range-partitioned one), which `holder` names in
+// the message; `keys` is the number of keys the index searches (0: an empty index).  Messages name `fn`.
 int index_check_tables(const rmi_result* r, uint64_t rows, const char* holder, uint64_t keys, const std::string& fn) {
-  if (int rc = index_check_leaf_tables(r, fn)) return rc;
   if (r->num_rmi_rows != rows)
     return fail(RMI_ERR_INVALID, fn + ": the result was trained on " + std::to_string(r->num_rmi_rows) + " keys, " +
                                      holder + std::to_string(rows));
   if (keys == 0 || r->branching_factor == 0) return fail(RMI_ERR_INVALID, fn + ": empty index");
-  if (lookup_top_group((int)r->l0_model_id) < 0 || lookup_leaf_group((int)r->l1_model_id) < 0)
-    return fail(RMI_ERR_UNSUPPORTED, fn + ": unsupported model id (top " + std::to_string(r->l0_model_id) +
-                                         ", leaf " + std::to_string(r->l1_model_id) + ")");
-  if (r->l1_params_per_model != (uint32_t)leaf_params_per_model((int)r->l1_model_id))
-    return fail(RMI_ERR_INVALID, fn + ": wrong number of leaf parameters");
-  if (r->l0_model_id == M_RADIX_TABLE &&
-      (!r->l0_table32 || r->l0_table_bits > 32 || r->l0_table32_len != ((uint64_t)1 << r->l0_table_bits)))
-    return fail(RMI_ERR_INVALID, fn + ": radix table missing or of the wrong size");
-  if (r->l0_model_id == M_HISTOGRAM && (!r->l0_array2 || !r->l0_array2_len))
-    return fail(RMI_ERR_INVALID, fn + ": histogram pivots missing");
   return RMI_OK;
 }
 
-// Builds the index on ds's device; knots (K of them, may be null) make it a bounded one.
-int index_upload(const rmi_result* r, const rmi_dataset* ds, const rmi_spline_point* knots, uint64_t K,
+// Builds the index on ds's device, predicting over n positions; knots (K of them, may be null) make it a bounded one.
+int index_upload(const rmi_result* r, const rmi_dataset* ds, uint64_t n, const rmi_spline_point* knots, uint64_t K,
                  uint64_t line_size, const std::string& fn, rmi_index** out) {
   CUDA_TRY(cudaSetDevice(ds->device));
   DeviceInfo di;
@@ -791,40 +822,22 @@ int index_upload(const rmi_result* r, const rmi_dataset* ds, const rmi_spline_po
   idx->ds = ds;
   idx->leaf_kind = (int)r->l1_model_id;
   idx->N = r->branching_factor;
+  idx->n = n;
   idx->num_sms = di.num_sms;
-  TopModel& t = idx->top;
-  memset(&t, 0, sizeof(t));
-  t.kind = (int)r->l0_model_id;
-  t.high = (int)r->l0_bradix_high;
-  t.table_bits = (int)r->l0_table_bits;
-  for (int q = 0; q < 4; ++q) { t.f[q] = r->l0_fparams[q]; t.ip[q] = r->l0_iparams[q]; }
   std::vector<char> packed((size_t)idx->N * lookup_record_bytes(idx->leaf_kind));
   pack_leaf_records(idx->leaf_kind, r->l1_params, (const u64*)r->l1_errors, idx->N, packed.data());
-  cudaError_t e = cudaMalloc(&idx->d_records, packed.size());
+  cudaError_t e = idx->tables.upload(*r, nullptr, device_alloc);
+  idx->top = idx->tables.given(*r);
+  if (e == cudaSuccess) e = cudaMalloc(&idx->d_records, packed.size());
   if (e == cudaSuccess) e = cudaMemcpy(idx->d_records, packed.data(), packed.size(), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess && t.kind == M_RADIX_TABLE) {
-    e = cudaMalloc(&idx->d_t32, sizeof(u32) * r->l0_table32_len);
-    if (e == cudaSuccess) e = cudaMemcpy(idx->d_t32, r->l0_table32, sizeof(u32) * r->l0_table32_len, cudaMemcpyHostToDevice);
-    t.t32 = idx->d_t32;
-  }
-  if (e == cudaSuccess && t.kind == M_HISTOGRAM) {
-    e = cudaMalloc(&idx->d_pivots, sizeof(u64) * r->l0_array2_len);
-    if (e == cudaSuccess) e = cudaMemcpy(idx->d_pivots, r->l0_array2, sizeof(u64) * r->l0_array2_len, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess && r->l0_array1 && r->l0_array1_len) {
-      e = cudaMalloc(&idx->d_radix_index, sizeof(u64) * r->l0_array1_len);
-      if (e == cudaSuccess)
-        e = cudaMemcpy(idx->d_radix_index, r->l0_array1, sizeof(u64) * r->l0_array1_len, cudaMemcpyHostToDevice);
-    }
-    t.pivots = idx->d_pivots;
-    t.radix_index = idx->d_radix_index;
-    t.npivots = r->l0_array2_len;
-  }
   if (e == cudaSuccess && knots) {
     e = cudaMalloc(&idx->d_knots, sizeof(rmi_spline_point) * K);
     if (e == cudaSuccess) e = cudaMemcpy(idx->d_knots, knots, sizeof(rmi_spline_point) * K, cudaMemcpyHostToDevice);
     idx->K = K;
     idx->line_size = line_size;
   }
+  // the table copies are asynchronous: r's host tables may be released once this returns
+  if (e == cudaSuccess) e = cudaStreamSynchronize(nullptr);
   if (e != cudaSuccess) {
     index_free_device(idx);
     delete idx;
@@ -840,16 +853,18 @@ int index_upload(const rmi_result* r, const rmi_dataset* ds, const rmi_spline_po
 extern "C" {
 
 int rmi_index_create(const rmi_result* r, const rmi_dataset* ds, rmi_index** out) {
-  if (!r || !ds || !out) return fail(RMI_ERR_INVALID, "rmi_index_create: null argument");
-  if (int rc = index_check_leaf_tables(r, "rmi_index_create")) return rc;
-  if (int rc = index_check_tables(r, ds->n, "the dataset holds ", ds->n, "rmi_index_create")) return rc;
-  return index_upload(r, ds, nullptr, 0, 0, "rmi_index_create", out);
+  const std::string fn = "rmi_index_create";
+  if (!r || !ds || !out) return fail(RMI_ERR_INVALID, fn + ": null argument");
+  if (int rc = check_result(r, true, fn)) return rc;
+  if (int rc = index_check_tables(r, ds->n, "the dataset holds ", ds->n, fn)) return rc;
+  return index_upload(r, ds, ds->n, nullptr, 0, 0, fn, out);
 }
 
 int rmi_index_create_bounded(const rmi_result* r, const rmi_spline_point* knots, uint64_t num_knots,
                              uint64_t line_size, const rmi_dataset* ds, rmi_index** out) {
   const std::string fn = "rmi_index_create_bounded";
   if (!r || !knots || !ds || !out) return fail(RMI_ERR_INVALID, fn + ": null argument");
+  if (int rc = check_result(r, true, fn)) return rc;
   if (ds->key_type != RMI_KEY_U64) return fail(RMI_ERR_INVALID, fn + ": Can only construct a bounded RMI on u64 data");
   if (line_size == 0) return fail(RMI_ERR_INVALID, fn + ": line size 0");
   if (num_knots == 0) return fail(RMI_ERR_INVALID, fn + ": no spline knots");
@@ -862,7 +877,7 @@ int rmi_index_create_bounded(const rmi_result* r, const rmi_spline_point* knots,
       return fail(RMI_ERR_INVALID, fn + ": knots " + std::to_string(i - 1) + " and " + std::to_string(i) +
                                        " are out of order (keys must increase strictly, offsets must not decrease)");
   }
-  return index_upload(r, ds, knots, num_knots, line_size, fn, out);
+  return index_upload(r, ds, ds->n, knots, num_knots, line_size, fn, out);
 }
 
 void rmi_index_destroy(rmi_index* idx) {
@@ -1357,13 +1372,6 @@ int train_entry(const rmi_dataset* ds, const char* model_spec, uint64_t N, uint3
   });
 }
 
-// The model table entry of a result's top / leaf model id (radix tables by their table bits).
-const ModelName* model_of(uint32_t kind, uint32_t table_bits) {
-  for (const auto& m : kModels)
-    if (m.kind == (int)kind && (kind != M_RADIX_TABLE || m.table_bits == (int)table_bits)) return &m;
-  return nullptr;
-}
-
 // The statuses of the boundary pass that concern a given top model: the error pass clamps the top's prediction to
 // N - 1 (two_layer.rs:210-211) and fits nothing, so only the order checks of two_layer.rs:50 remain.
 constexpr unsigned kEvaluateStatus = ST_NOT_SORTED | ST_NON_MONOTONE;
@@ -1398,14 +1406,13 @@ int evaluate_typed(const rmi_dataset* ds, const rmi_result* r, const ModelName& 
     u64* d_scratch = A.get<u64>(2 * N);
     void* d_stats = A.get<char>(stats_scratch_bytes(N));
     TopTables tables;
-    const bool host_ok = reserve_result(box, nullptr, N, ppm, !stats_only, want_counts) &&
-                         (r->l0_table32_len == 0 || box->table32.resize(r->l0_table32_len)) &&
-                         (r->l0_model_id != M_HISTOGRAM ||
-                          (box->arr1.resize(r->l0_array1_len) && box->arr2.resize(r->l0_array2_len)));
     cudaEventRecord(ev0, st);
-    const bool tables_ok = tables.upload(*r, st, [&](size_t bytes) -> void* { return A.get<char>(bytes); });
-    if (A.err != cudaSuccess || !tables_ok) {
+    const cudaError_t te = tables.upload(*r, st, [&](size_t bytes) -> void* { return A.get<char>(bytes); });
+    const bool host_ok = reserve_result(box, &tables, N, ppm, !stats_only, want_counts);
+    if (A.err != cudaSuccess) {
       rc = fail(RMI_ERR_CUDA, std::string("scratch allocation: ") + cudaGetErrorString(A.err));
+    } else if (te != cudaSuccess) {
+      rc = fail(RMI_ERR_CUDA, std::string("rmi_evaluate: ") + cudaGetErrorString(te));
     } else if (!host_ok) {
       rc = fail(RMI_ERR_CUDA, kPinnedFailed);
     } else {
@@ -1435,14 +1442,9 @@ int evaluate_typed(const rmi_dataset* ds, const rmi_result* r, const ModelName& 
       } else {
         // r's tables, as given (the device copies were only read)
         if (!stats_only) memcpy(box->l1_params.data(), r->l1_params, sizeof(double) * N * ppm);
-        if (r->l0_table32_len) memcpy(box->table32.data(), r->l0_table32, sizeof(u32) * r->l0_table32_len);
-        if (r->l0_model_id == M_HISTOGRAM) {
-          memcpy(box->arr1.data(), r->l0_array1, sizeof(u64) * r->l0_array1_len);
-          memcpy(box->arr2.data(), r->l0_array2, sizeof(u64) * r->l0_array2_len);
-        }
-        tables.t32_len = r->l0_table32_len;
-        tables.ri_len = r->l0_model_id == M_HISTOGRAM ? r->l0_array1_len : 0;
-        tables.hist_bins = r->l0_model_id == M_HISTOGRAM ? r->l0_array2_len : 0;
+        if (tables.t32_len) memcpy(box->table32.data(), r->l0_table32, sizeof(u32) * tables.t32_len);
+        if (tables.ri_len) memcpy(box->arr1.data(), r->l0_array1, sizeof(u64) * tables.ri_len);
+        if (tables.hist_bins) memcpy(box->arr2.data(), r->l0_array2, sizeof(u64) * tables.hist_bins);
         fill_result(box, top, leaf, tables, n, N);
         rmi_result& R = box->pub;
         R.l0_num_fparams = r->l0_num_fparams;
@@ -1502,19 +1504,8 @@ int rmi_evaluate(const rmi_dataset* ds, const rmi_result* r, uint32_t flags, rmi
   g_last_error.clear();
   const std::string fn = "rmi_evaluate";
   if (!ds || !r || !out) return fail(RMI_ERR_INVALID, fn + ": null argument");
-  const ModelName* top = model_of(r->l0_model_id, r->l0_table_bits);
-  const ModelName* leaf = model_of(r->l1_model_id, 0);
-  if (!top || !leaf || leaf->root_only)
-    return fail(RMI_ERR_INVALID, fn + ": unknown model id (top " + std::to_string(r->l0_model_id) + ", leaf " +
-                                     std::to_string(r->l1_model_id) + ")");
-  if (int rc = check_leaf(leaf)) return rc;
-  if (!r->l1_params) return fail(RMI_ERR_INVALID, fn + ": the result holds no leaf parameters (RMI_FLAG_STATS_ONLY)");
-  if (r->l1_params_per_model != (uint32_t)leaf_params_per_model(leaf->kind))
-    return fail(RMI_ERR_INVALID, fn + ": wrong number of leaf parameters");
-  if (r->l0_model_id == M_RADIX_TABLE && (!r->l0_table32 || r->l0_table32_len != ((uint64_t)1 << r->l0_table_bits)))
-    return fail(RMI_ERR_INVALID, fn + ": radix table missing or of the wrong size");
-  if (r->l0_model_id == M_HISTOGRAM && (!r->l0_array2 || !r->l0_array2_len || (r->l0_array1_len && !r->l0_array1)))
-    return fail(RMI_ERR_INVALID, fn + ": histogram pivots missing");
+  const ModelName *top = nullptr, *leaf = nullptr;
+  if (int rc = check_result(r, false, fn, &top, &leaf)) return rc;
   if (int rc = check_build(ds->n, r->branching_factor, ds->sorted)) return rc;
   return with_key_type(ds->key_type, [&](auto k) { return evaluate_typed<decltype(k)>(ds, r, *top, *leaf, flags, out); });
 }
@@ -1837,10 +1828,7 @@ int rmi_shard_build_create(const rmi_dataset* local, const rmi_shard_info* info,
          cudaEventCreateWithFlags(&b->ev_join, cudaEventDisableTiming) == cudaSuccess &&
          cudaMalloc((void**)&b->d_long, sizeof(u32) * (LONG_LEAF_CAP + 1)) == cudaSuccess;
   }
-  ok = ok && b->tables.allocate(*top, info->n_global, branch_factor, [](size_t bytes) -> void* {
-    void* p = nullptr;
-    return cudaMalloc(&p, bytes) == cudaSuccess ? p : nullptr;
-  });
+  ok = ok && b->tables.allocate(*top, info->n_global, branch_factor, device_alloc);
   if (!ok) { rmi_shard_build_destroy(b); return fail(RMI_ERR_CUDA, "rmi_shard_build_create: device allocation failed"); }
   *out = b;
   return RMI_OK;
@@ -2308,7 +2296,7 @@ void rmi_shard_build_destroy(rmi_shard_build* b) {
   if (b->ev_join) cudaEventDestroy(b->ev_join);
   if (b->side) cudaStreamDestroy(b->side);
   cudaFree(b->d_long);
-  cudaFree(b->tables.t32); cudaFree(b->tables.pivots); cudaFree(b->tables.radix_index);
+  b->tables.free_device();
   cudaFree(b->d_bases); cudaFree(b->d_off); cudaFree(b->d_parts); cudaFree(b->d_flags_mine); cudaFree(b->d_flags_all);
   if (b->h_off) cudaFreeHost(b->h_off);
   if (b->h_flags_all) cudaFreeHost(b->h_flags_all);
@@ -2380,12 +2368,11 @@ int shard_lookup_search(const rmi_shard_index* si, const T* d_recv, uint64_t m, 
     return fail(RMI_ERR_INVALID, "rmi_shard_index_search: this rank holds no keys, so no query is routed to it");
   PoolScratch s{nullptr, st};
   CUDA_TRY(cudaMallocAsync(&s.p, 2 * sizeof(u64) * m, st));
-  u64* pos = (u64*)s.p;
+  uint64_t* pos = (uint64_t*)s.p;   // m predictions, then their error bounds
+  if (int rc = index_launch(idx, d_recv, m, pos, pos + m, nullptr, st, false)) return rc;
   Launch L{st, idx->num_sms};
-  lookup_batch<T>(L, idx->top, idx->leaf_kind, idx->d_records, idx->N, (const T*)ds->d_keys, si->n_global, d_recv, m,
-                  pos, pos + m, nullptr, false);
-  shard_search<T>(L, (const T*)ds->d_keys, ds->n, si->base, si->n_global, d_recv, m, pos, pos + m, d_answers,
-                  d_fallbacks);
+  shard_search<T>(L, (const T*)ds->d_keys, ds->n, si->base, si->n_global, d_recv, m, (const u64*)pos,
+                  (const u64*)pos + m, d_answers, d_fallbacks);
   CUDA_TRY(cudaGetLastError());
   return RMI_OK;
 }
@@ -2463,11 +2450,9 @@ int rmi_shard_index_create(const rmi_result* r, const rmi_dataset* local, const 
   const std::string fn = "rmi_shard_index_create";
   g_last_error.clear();
   if (!r || !local || !ends_all || !out) return fail(RMI_ERR_INVALID, fn + ": null argument");
+  if (int rc = check_result(r, true, fn)) return rc;
   if (world < 1 || world > SHARD_ROUTE_MAX - 1 || rank < 0 || rank >= world)
     return fail(RMI_ERR_INVALID, fn + ": bad world or rank (0 <= rank < world <= 63)");
-  if (!r->l1_params || !r->l1_errors)
-    return fail(RMI_ERR_INVALID, fn + ": the result holds no leaf tables (trained with RMI_FLAG_STATS_ONLY, or received "
-                                      "by a rank other than 0 of an RMI_FLAG_SHARD_ROOT_ONLY build)");
   if (ends_all[rank].n_local != local->n)
     return fail(RMI_ERR_INVALID, fn + ": ends_all[" + std::to_string(rank) + "] describes " +
                                      std::to_string(ends_all[rank].n_local) + " keys, the local dataset holds " +
@@ -2494,7 +2479,7 @@ int rmi_shard_index_create(const rmi_result* r, const rmi_dataset* local, const 
                                      "'s first key is below the last key of rank " + std::to_string(prev) + ")");
   if (int rc = index_check_tables(r, total, "the slabs hold ", total, fn)) return rc;
   rmi_index* idx = nullptr;
-  if (int rc = index_upload(r, local, nullptr, 0, 0, fn, &idx)) return rc;
+  if (int rc = index_upload(r, local, total, nullptr, 0, 0, fn, &idx)) return rc;
   auto* si = new rmi_shard_index();
   si->idx = idx;
   si->world = world;
@@ -2528,17 +2513,7 @@ int rmi_shard_index_predict(const rmi_shard_index* si, const void* d_queries, ui
                             uint64_t* d_err, void* cuda_stream) {
   if (!si) return fail(RMI_ERR_INVALID, "rmi_shard_index_predict: null index");
   if (int rc = index_check_call(si->idx, d_queries, n, d_pos, "rmi_shard_index_predict")) return rc;
-  if (n == 0) return RMI_OK;
-  const rmi_index* idx = si->idx;
-  CUDA_TRY(cudaSetDevice(idx->ds->device));
-  Launch L{(cudaStream_t)cuda_stream, idx->num_sms};
-  with_key_type(idx->ds->key_type, [&](auto k) {
-    using T = decltype(k);
-    lookup_batch<T>(L, idx->top, idx->leaf_kind, idx->d_records, idx->N, (const T*)idx->ds->d_keys, si->n_global,
-                    (const T*)d_queries, n, (u64*)d_pos, (u64*)d_err, nullptr, false);
-  });
-  CUDA_TRY(cudaGetLastError());
-  return RMI_OK;
+  return index_launch(si->idx, d_queries, n, d_pos, d_err, nullptr, cuda_stream, false);
 }
 
 int rmi_shard_index_route(const rmi_shard_index* si, const void* d_queries, uint64_t n, void* d_send, uint64_t* d_slot,

@@ -178,7 +178,7 @@ void pack_leaf_records(int leaf_kind, const double* params, const u64* errors, u
 // One kernel launch on L.stream (none for nq == 0).  lower_bound = false: out = position estimates, out_err (may be
 // null) = the leaves' error bounds.  lower_bound = true: out = exact lower bounds over keys[0, n); *fallbacks (may be
 // null) grows by the number of queries whose error window missed.  `top` is passed by value; its table pointers
-// (t32, pivots, radix_index) are device memory.
+// (t32, pivots) are device memory.
 template <class T>
 void lookup_batch(const Launch& L, const TopModel& top, int leaf_kind, const void* d_records, u64 N, const T* keys, u64 n,
                   const T* d_queries, u64 nq, u64* d_out, u64* d_out_err, u64* d_fallbacks, bool lower_bound);

@@ -21,7 +21,7 @@ enum ModelKind : int {
 //   radix                                              : ip = {prefix, bits}
 //   bradix                                             : ip = {prefix, bits, clamp}, high
 //   radix table                                        : ip = {prefix}, table_bits, t32
-//   histogram                                          : ip = {num_pivots}, pivots, radix_index
+//   histogram                                          : ip = {num_pivots}, pivots
 struct TopModel {
   int kind;
   int high;
@@ -31,7 +31,6 @@ struct TopModel {
   u64 ip[4];
   const u32* t32;
   const u64* pivots;
-  const u64* radix_index;
   u64 npivots;
 };
 
