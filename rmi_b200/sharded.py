@@ -70,13 +70,24 @@ def key_bits_to_float(bits: int, key_type: int) -> float:
     return float(bits)
 
 
+def key_from_bits(bits: int, key_type: int):
+    """The key a raw key word holds, as a value that compares like the key type: float for f64 keys (so that
+    -0.0 == 0.0, as the kernels and the reference compare keys), int for the unsigned types."""
+    if key_type == api.KEY_F64:
+        return struct.unpack("<d", struct.pack("<Q", bits))[0]
+    if key_type == api.KEY_U32:
+        return bits & 0xFFFFFFFF
+    return bits
+
+
 def plan_global_layout(ends_all: np.ndarray, key_type: int, num_leaves: int) -> list[dict]:
     """From every rank's (first_key_bits, last_key_bits, last_run_start, n_local) derive, for every
     rank, its shard description.  Pure function of the gathered table: every rank computes the same.
 
     prev_key / prev_F: last key before the slab and the first global index of its run of equal keys
     (the offset FixDupsIter would report, reference models/mod.rs:154-185), which may lie several
-    ranks back when whole slabs consist of one repeated key."""
+    ranks back when whole slabs consist of one repeated key.  Keys at the cuts are compared by value,
+    not by bits: -0.0 and 0.0 are one run."""
     world = ends_all.shape[0]
     n_local = [int(x) for x in ends_all[:, 3]]
     bases = [0]
@@ -84,11 +95,13 @@ def plan_global_layout(ends_all: np.ndarray, key_type: int, num_leaves: int) -> 
         bases.append(bases[-1] + n_local[g])
     n_global = bases[-1]
     nonempty = [g for g in range(world) if n_local[g] > 0]
+    first_key = {g: key_from_bits(int(ends_all[g, 0]), key_type) for g in nonempty}
+    last_key = {g: key_from_bits(int(ends_all[g, 1]), key_type) for g in nonempty}
     last_F = {}
     prev = None
     for g in nonempty:
-        first_b, last_b, lrs = int(ends_all[g, 0]), int(ends_all[g, 1]), int(ends_all[g, 2])
-        if lrs == 0 and prev is not None and int(ends_all[prev, 1]) == first_b:
+        lrs = int(ends_all[g, 2])
+        if lrs == 0 and prev is not None and last_key[prev] == first_key[g]:
             last_F[g] = last_F[prev]           # the whole slab is one run that began on an earlier rank
         else:
             last_F[g] = bases[g] + lrs
@@ -96,7 +109,7 @@ def plan_global_layout(ends_all: np.ndarray, key_type: int, num_leaves: int) -> 
     # no two equal keys anywhere: every rank is duplicate-free and no cut separates two equal keys
     no_dups = ends_all.shape[1] > 4 and all(int(ends_all[g, 4]) == 1 for g in nonempty)
     for a, b in zip(nonempty, nonempty[1:]):
-        if int(ends_all[a, 1]) == int(ends_all[b, 0]):
+        if last_key[a] == first_key[b]:
             no_dups = False
     first_bits = int(ends_all[nonempty[0], 0]) if nonempty else 0
     last_bits = int(ends_all[nonempty[-1], 1]) if nonempty else 0

@@ -150,6 +150,63 @@ def test_layout_planner_handles_runs_spanning_ranks():
     assert lay[2]["base"] == 3 and lay[2]["n_global"] == 5
 
 
+def test_layout_planner_compares_f64_keys_at_the_cuts_by_value():
+    """-0.0 == 0.0: a cut between them separates two equal keys (the data set has duplicates, so the leaf kernel
+    must track runs) and a slab of zeros continues the run of a -0.0 before it, whatever the zeros' signs."""
+    from rmi_b200 import api, sharded
+
+    def b(x):
+        return int(np.array([x], dtype=np.float64).view(np.uint64)[0])
+
+    def ends(*rows):   # (first key, last key, last run start, n_local, no_dups) of every rank
+        return np.array([[b(f), b(l), s, n, d] for f, l, s, n, d in rows], dtype=np.uint64)
+
+    def planned(*rows):
+        return sharded.plan_global_layout(ends(*rows), api.KEY_F64, 16)
+
+    # [-1.0, -0.5, -0.0] | [0.0, 0.5, 1.0] and [-1.0, -0.5, 0.0] | [-0.0, 0.5, 1.0]: no equal keys inside a slab
+    for z0, z1 in ((-0.0, 0.0), (0.0, -0.0)):
+        lay = planned((-1.0, z0, 2, 3, 1), (z1, 1.0, 2, 3, 1))
+        assert lay[0]["no_dups"] == 0
+        assert lay[1]["has_prev"] == 1 and lay[1]["prev_key_bits"] == b(z0) and lay[1]["prev_F"] == 2
+        assert lay[0]["last_F"] == 5
+    # [-1.0, -0.5, -0.0] | [0.0, -0.0, 0.0] | [2.0, 3.0]: the middle slab is one run that began at global index 2
+    lay = planned((-1.0, -0.0, 2, 3, 1), (0.0, 0.0, 0, 3, 0), (2.0, 3.0, 1, 2, 1))
+    assert [d["base"] for d in lay] == [0, 3, 6] and lay[0]["no_dups"] == 0
+    assert lay[1]["prev_F"] == 2 and lay[1]["prev_key_bits"] == b(-0.0)
+    assert lay[2]["prev_F"] == 2 and lay[2]["prev_key_bits"] == b(0.0)
+    assert lay[0]["last_F"] == 7
+    # the last slab is the zeros: the data set's last run starts on rank 0
+    lay = planned((-1.0, -0.0, 1, 2, 1), (0.0, -0.0, 0, 4, 0))
+    assert lay[1]["prev_F"] == 1 and lay[0]["last_F"] == 1 and lay[0]["no_dups"] == 0
+    # [-1.0, -0.0] | (empty) | [0.0, 1.0]: the empty slab does not separate the two zeros
+    lay = planned((-1.0, -0.0, 1, 2, 1), (0.0, 0.0, 0, 0, 1), (0.0, 1.0, 1, 2, 1))
+    assert lay[0]["no_dups"] == 0 and [d["base"] for d in lay] == [0, 2, 2]
+    assert lay[1]["has_prev"] == 1 and lay[1]["prev_F"] == 1 and lay[1]["prev_key_bits"] == b(-0.0)
+    assert lay[2]["prev_F"] == 1 and lay[2]["prev_key_bits"] == b(-0.0) and lay[0]["last_F"] == 3
+    # [-1.0, -0.0] | (empty) | [0.0, -0.0] | [1.0]: a slab of zeros continues a run across the empty slab
+    lay = planned((-1.0, -0.0, 1, 2, 1), (0.0, 0.0, 0, 0, 1), (0.0, -0.0, 0, 2, 0), (1.0, 1.0, 0, 1, 1))
+    assert lay[3]["prev_F"] == 1 and lay[3]["prev_key_bits"] == b(-0.0) and lay[0]["last_F"] == 4
+    # distinct keys whose bits differ only in the sign stay distinct: [-1.0, -0.5] | [0.5, 1.0]
+    lay = planned((-1.0, -0.5, 1, 2, 1), (0.5, 1.0, 1, 2, 1))
+    assert lay[0]["no_dups"] == 1 and lay[1]["prev_F"] == 1 and lay[0]["last_F"] == 3
+
+
+def test_layout_planner_u32_keys_compare_as_32_bit_values():
+    from rmi_b200 import api, sharded
+    # rank 1 is one run of 0xFFFFFFF0 (negative in int32 storage) that began on rank 0
+    ends = np.array([[5, 0xFFFFFFF0, 3, 10, 1], [0xFFFFFFF0, 0xFFFFFFF0, 0, 4, 0], [0xFFFFFFF0, 0xFFFFFFFF, 2, 6, 0]],
+                    dtype=np.uint64)
+    lay = sharded.plan_global_layout(ends, api.KEY_U32, 64)
+    assert lay[1]["prev_F"] == 3 and lay[2]["prev_F"] == 3 and lay[2]["prev_key_bits"] == 0xFFFFFFF0
+    assert lay[0]["last_F"] == 16 and lay[0]["no_dups"] == 0
+    ends[:, 4] = 1
+    ends[1] = [0xFFFFFFF1, 0xFFFFFFF2, 1, 2, 1]
+    ends[2] = [0xFFFFFFF3, 0xFFFFFFFF, 5, 6, 1]
+    lay = sharded.plan_global_layout(ends, api.KEY_U32, 64)
+    assert lay[0]["no_dups"] == 1 and lay[2]["prev_F"] == 11 and lay[0]["last_F"] == 17
+
+
 def test_halo_planner():
     from rmi_b200 import sharded
     # rank 0's last leaf ends at 13 (inside rank 2): it needs [10, 14) = 2 keys of rank 1 + 2 of rank 2... rank 1 has 2 keys
