@@ -152,7 +152,7 @@ int rmi_train_with_top(const rmi_dataset* ds, const char* model_spec, uint64_t b
                        const double* l0_fparams, uint32_t n_fparams, rmi_result** out);
 void rmi_result_free(rmi_result* r);
 /* The calls that take a given trained result (rmi_evaluate, rmi_index_create, rmi_index_create_bounded,
- * rmi_shard_index_create) first check it the same way, before they read a dataset, and refuse it with the same code
+ * rmi_shard_index_create, rmi_shard_eval_create) first check it the same way, before they read a dataset, and refuse it with the same code
  * and the message "<function>: <reason>":
  *   RMI_ERR_INVALID      no l1_params, or (the indexes, which serve the error bounds) no l1_errors: "the result holds
  *                        no leaf tables ..." (RMI_FLAG_STATS_ONLY, or a rank other than 0 of an
@@ -376,6 +376,46 @@ typedef struct {
   uint64_t queries_kept;       /* of the n, those this rank answered itself */
 } rmi_shard_lookup_stats;
 int rmi_shard_index_last_stats(const rmi_shard_index* idx, rmi_shard_lookup_stats* out);
+
+/* ---- rmi_evaluate over a range-partitioned data set (DESIGN.md section 15) ----------------------------------------
+ * Every rank holds the whole model r and its own slab `local`; the result is rmi_evaluate(concatenation of the slabs, r),
+ * bit for bit in every field but the timings, on every rank.  Each rank reads only its own keys: the per-key errors,
+ * the runs of equal keys that end on its slab and the widening terms whose key it holds are MAXima of contributions,
+ * combined by one all-reduce MAX.  A top model that is not monotone on the keys (across a cut included) fails the
+ * evaluation on EVERY rank with rmi_evaluate's message (RMI_ERR_PANIC).
+ *
+ * rmi_shard_eval_create refuses, before any device work, in this order: a null argument (RMI_ERR_INVALID); every result
+ * rmi_evaluate refuses (the checks of a given result, above); the ends-table checks of rmi_shard_index_create (world /
+ * rank, ends_all[rank] not describing local, slabs out of key order); then rmi_evaluate's checks of the concatenated
+ * keys (branching factor 0, no keys, a local dataset that is not sorted: RMI_ERR_PANIC).  It derives every rank's
+ * base, the key before its slab and that key's run start, the next slab's first key and whether the whole key set is
+ * duplicate-free from ends_all, and allocates the device buffers of one evaluation.  r and local must outlive the
+ * evaluator; r's tables are read again at every evaluation.
+ *
+ * Phase form (the caller issues the collectives between the calls, rmi_b200/sharded.py does it with torch.distributed):
+ *   bounds   uploads r's tables, then the streaming boundary pass over the local keys into d_S ((N+1) u64, n_global
+ *            where no local key reaches a leaf)               -> all-reduce MIN of d_S
+ *   keys     this rank's contributions into d_partial (2N u64, part_err | part_run) and its status word into *d_status
+ *                                                              -> all-reduce MAX of the first rmi_shard_eval_partial_words
+ *                                                                 words of d_partial (N when the key set holds no two
+ *                                                                 equal keys, else 2N); OR of every rank's status word
+ *   finish   error bounds, counts and statistics from d_S and d_partial; waits for the stream of the last call and
+ *            returns the result (status: the OR of the ranks' words).
+ * bounds and keys are enqueued on cuda_stream without a host synchronisation.
+ * rmi_shard_evaluate: the same in one call, the collectives on the evaluator's own stream over c (which must have the
+ * evaluator's world and rank).  Flags: RMI_FLAG_STATS_ONLY, RMI_FLAG_LEAF_COUNTS.  num_rmi_rows = num_data_rows = the
+ * keys of all slabs.  phase_device_ns: [0] upload, [1] boundaries with their all-reduce, [2] error pass with its
+ * all-reduce, [3] statistics; device_time_ns is their sum. */
+typedef struct rmi_shard_eval rmi_shard_eval;
+int rmi_shard_eval_create(const rmi_result* r, const rmi_dataset* local, const rmi_shard_ends* ends_all, int world,
+                          int rank, rmi_shard_eval** out);
+void rmi_shard_eval_destroy(rmi_shard_eval* e);
+uint64_t rmi_shard_eval_partial_words(const rmi_shard_eval* e);
+int rmi_shard_eval_bounds(rmi_shard_eval* e, uint64_t* d_S, void* cuda_stream);
+int rmi_shard_eval_keys(rmi_shard_eval* e, const uint64_t* d_S, uint64_t* d_partial, uint32_t* d_status, void* cuda_stream);
+int rmi_shard_eval_finish(rmi_shard_eval* e, const uint64_t* d_S, const uint64_t* d_partial, uint32_t status,
+                          uint32_t flags, rmi_result** out);
+int rmi_shard_evaluate(rmi_shard_eval* e, rmi_shard_comm* c, uint32_t flags, rmi_result** out);
 
 /* ---- `--bounded` support: rmi_lib::cache_fix (reference rmi_lib/src/cache_fix.rs:106-150) ----------
  * The error-bounded spline over key -> first-occurrence offset whose interpolation always lands in

@@ -13,8 +13,8 @@ The product is the C-ABI shared library ``rmi_b200/lib/librmi_b200.so`` (CUDA, s
 
 plus RMIIndex and BoundedRMIIndex (a train_bounded build), batched lookups (position estimates and exact lower
 bounds) on the GPU.  cache_fix / train_bounded on an RMITrainingData fit the cache-fix spline on the GPU.
-rmi_b200.sharded (torch.distributed) trains over range-partitioned keys (train_sharded) and serves lookups over them
-(ShardedRMIIndex).
+rmi_b200.sharded (torch.distributed) trains over range-partitioned keys (train_sharded), evaluates a given RMI over
+them (evaluate_sharded) and serves lookups over them (ShardedRMIIndex).
 
 and does no arithmetic of its own.  There is no CPU fallback: if the CUDA library is missing
 or no device is present, calls raise.

@@ -1376,6 +1376,23 @@ int train_entry(const rmi_dataset* ds, const char* model_spec, uint64_t N, uint3
 // N - 1 (two_layer.rs:210-211) and fits nothing, so only the order checks of two_layer.rs:50 remain.
 constexpr unsigned kEvaluateStatus = ST_NOT_SORTED | ST_NON_MONOTONE;
 
+// The public struct of an evaluation of r over n keys, from what reserve_result / copy_result_to_host brought back (the
+// error bounds and counts included, the stream synchronised): r's tables as given (the device copies were only read),
+// the statistics measured.
+void fill_given_result(ResultBox* box, const rmi_result* r, const ModelName& top, const ModelName& leaf,
+                       const TopTables& tables, uint64_t n, bool stats_only) {
+  const uint64_t N = r->branching_factor;
+  if (!stats_only) memcpy(box->l1_params.data(), r->l1_params, sizeof(double) * N * leaf_params_per_model(leaf.kind));
+  if (tables.t32_len) memcpy(box->table32.data(), r->l0_table32, sizeof(u32) * tables.t32_len);
+  if (tables.ri_len) memcpy(box->arr1.data(), r->l0_array1, sizeof(u64) * tables.ri_len);
+  if (tables.hist_bins) memcpy(box->arr2.data(), r->l0_array2, sizeof(u64) * tables.hist_bins);
+  fill_result(box, top, leaf, tables, n, N);
+  rmi_result& R = box->pub;
+  R.l0_num_fparams = r->l0_num_fparams;
+  R.l0_num_iparams = r->l0_num_iparams;
+  R.top_fit_exact = r->top_fit_exact;
+}
+
 template <class T>
 int evaluate_typed(const rmi_dataset* ds, const rmi_result* r, const ModelName& top, const ModelName& leaf, uint32_t flags,
                    rmi_result** out) {
@@ -1440,19 +1457,11 @@ int evaluate_typed(const rmi_dataset* ds, const rmi_result* r, const ModelName& 
       } else if (status) {
         rc = fail(RMI_ERR_PANIC, status_text(status));
       } else {
-        // r's tables, as given (the device copies were only read)
-        if (!stats_only) memcpy(box->l1_params.data(), r->l1_params, sizeof(double) * N * ppm);
-        if (tables.t32_len) memcpy(box->table32.data(), r->l0_table32, sizeof(u32) * tables.t32_len);
-        if (tables.ri_len) memcpy(box->arr1.data(), r->l0_array1, sizeof(u64) * tables.ri_len);
-        if (tables.hist_bins) memcpy(box->arr2.data(), r->l0_array2, sizeof(u64) * tables.hist_bins);
-        fill_result(box, top, leaf, tables, n, N);
+        fill_given_result(box, r, top, leaf, tables, n, stats_only);
         rmi_result& R = box->pub;
-        R.l0_num_fparams = r->l0_num_fparams;
-        R.l0_num_iparams = r->l0_num_iparams;
         R.device_time_ns = elapsed_ns(ev0, ev1);
         cudaEvent_t seq[5] = {ev0, evp[0], evp[1], evp[2], ev1};
         for (int q = 0; q < 4; ++q) R.phase_device_ns[q] = elapsed_ns(seq[q], seq[q + 1]);
-        R.top_fit_exact = r->top_fit_exact;
       }
     }
   }   // arena frees (stream-ordered)
@@ -2443,24 +2452,24 @@ int shard_lookup_one_call(rmi_shard_index* si, rmi_shard_comm* c, const T* d_q, 
 
 }  // namespace
 
-extern "C" {
+namespace {
 
-int rmi_shard_index_create(const rmi_result* r, const rmi_dataset* local, const rmi_shard_ends* ends_all, int world,
-                           int rank, rmi_shard_index** out) {
-  const std::string fn = "rmi_shard_index_create";
-  g_last_error.clear();
-  if (!r || !local || !ends_all || !out) return fail(RMI_ERR_INVALID, fn + ": null argument");
-  if (int rc = check_result(r, true, fn)) return rc;
+// The checks of a gathered ends table that the consumers of range-partitioned keys (rmi_shard_index_create,
+// rmi_shard_eval_create) make before any device work, with RMI_ERR_INVALID and messages naming fn: world and rank in
+// range, ends_all[rank] describing `local`, the non-empty slabs in key order.  *base / *total: this rank's global
+// index of its first key and the keys of all slabs.
+int check_slabs(const std::string& fn, const rmi_dataset* local, const rmi_shard_ends* ends_all, int world, int rank,
+                uint64_t* base, uint64_t* total) {
   if (world < 1 || world > SHARD_ROUTE_MAX - 1 || rank < 0 || rank >= world)
     return fail(RMI_ERR_INVALID, fn + ": bad world or rank (0 <= rank < world <= 63)");
   if (ends_all[rank].n_local != local->n)
     return fail(RMI_ERR_INVALID, fn + ": ends_all[" + std::to_string(rank) + "] describes " +
                                      std::to_string(ends_all[rank].n_local) + " keys, the local dataset holds " +
                                      std::to_string(local->n));
-  uint64_t total = 0, base = 0;
+  *total = 0;
   for (int p = 0; p < world; ++p) {
-    if (p == rank) base = total;
-    total += ends_all[p].n_local;
+    if (p == rank) *base = *total;
+    *total += ends_all[p].n_local;
   }
   // the non-empty slabs must follow each other in key order: no slab's last key above the next one's first
   int prev = -1;
@@ -2477,6 +2486,21 @@ int rmi_shard_index_create(const rmi_result* r, const rmi_dataset* local, const 
   if (bad >= 0)
     return fail(RMI_ERR_INVALID, fn + ": the slabs are out of order (rank " + std::to_string(bad) +
                                      "'s first key is below the last key of rank " + std::to_string(prev) + ")");
+  return RMI_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int rmi_shard_index_create(const rmi_result* r, const rmi_dataset* local, const rmi_shard_ends* ends_all, int world,
+                           int rank, rmi_shard_index** out) {
+  const std::string fn = "rmi_shard_index_create";
+  g_last_error.clear();
+  if (!r || !local || !ends_all || !out) return fail(RMI_ERR_INVALID, fn + ": null argument");
+  if (int rc = check_result(r, true, fn)) return rc;
+  uint64_t total = 0, base = 0;
+  if (int rc = check_slabs(fn, local, ends_all, world, rank, &base, &total)) return rc;
   if (int rc = index_check_tables(r, total, "the slabs hold ", total, fn)) return rc;
   rmi_index* idx = nullptr;
   if (int rc = index_upload(r, local, total, nullptr, 0, 0, fn, &idx)) return rc;
@@ -2579,6 +2603,272 @@ int rmi_shard_index_last_stats(const rmi_shard_index* si, rmi_shard_lookup_stats
   *out = si->last;
   for (int q = 0; q + 1 < SHARD_LOOKUP_EVENTS; ++q) CUDA_TRY(cudaEventElapsedTime(&out->phase_ms[q], si->ev[q], si->ev[q + 1]));
   return RMI_OK;
+}
+
+}  // extern "C"
+
+// ---- rmi_evaluate over a range-partitioned data set (DESIGN.md section 15) -----------------------------------------
+constexpr int SHARD_EVAL_EVENTS = 5;   // upload | boundaries (+ all-reduce) | error pass (+ all-reduce) | statistics
+
+// Where a rank's slab sits among the others, from the gathered ends alone (the rule of sharded.py plan_global_layout):
+// the same on every rank for every field but the rank's own.
+struct SlabLayout {
+  uint64_t base = 0, n_global = 0;
+  int has_prev = 0, is_last = 0, is_first = 0, has_next = 0;
+  uint64_t prev_key_bits = 0, prev_F = 0;   // last key before the slab, first global index of its run
+  uint64_t next_key_bits = 0;               // first key of the next non-empty rank
+  bool no_dups = false;                     // no two keys of the whole data set are equal
+};
+
+struct rmi_shard_eval {
+  const rmi_result* r = nullptr;   // the caller's: read at every evaluation
+  const rmi_dataset* ds = nullptr;
+  const ModelName* top = nullptr;
+  const ModelName* leaf = nullptr;
+  int world = 0, rank = 0, num_sms = 0;
+  uint64_t N = 0;
+  SlabLayout lay;
+  TopTables tables;                // device copies of r's top tables (device_alloc)
+  TopModel* d_top = nullptr;
+  BuildAux* d_aux = nullptr;
+  double* d_params = nullptr;
+  u64* d_errors = nullptr;
+  u64* d_counts = nullptr;
+  void* d_stats = nullptr;
+  // rmi_shard_evaluate: its own stream and the exchanged buffers
+  cudaStream_t own = nullptr;
+  u64* d_S = nullptr;              // N + 1
+  u64* d_part = nullptr;           // 2 x N
+  unsigned* d_status = nullptr;    // world: every rank's status word
+  cudaStream_t st = nullptr;       // the stream of the evaluation under way
+  cudaEvent_t ev[SHARD_EVAL_EVENTS] = {};
+  std::chrono::steady_clock::time_point t_start;
+};
+
+namespace {
+
+template <class T> SlabLayout slab_layout(const rmi_shard_ends* e, int world, int rank) {
+  SlabLayout s;
+  std::vector<uint64_t> base(world + 1, 0), last_F(world, 0);
+  for (int g = 0; g < world; ++g) base[g + 1] = base[g] + e[g].n_local;
+  s.base = base[rank];
+  s.n_global = base[world];
+  s.no_dups = true;
+  int prev = -1, first = -1, last = -1;
+  for (int g = 0; g < world; ++g) {
+    if (!e[g].n_local) continue;
+    const bool joins = prev >= 0 && key_from_bits<T>(e[prev].last_key_bits) == key_from_bits<T>(e[g].first_key_bits);
+    // a slab that is one run begun ranks earlier carries that run's first index on
+    last_F[g] = e[g].last_run_start == 0 && joins ? last_F[prev] : base[g] + e[g].last_run_start;
+    if (joins || e[g].no_dups != 1) s.no_dups = false;
+    if (g < rank) { s.has_prev = 1; s.prev_key_bits = e[g].last_key_bits; s.prev_F = last_F[g]; }
+    if (g > rank && !s.has_next) { s.has_next = 1; s.next_key_bits = e[g].first_key_bits; }
+    if (first < 0) first = g;
+    last = g;
+    prev = g;
+  }
+  s.is_first = rank == first;
+  s.is_last = rank == last;
+  return s;
+}
+
+template <class T> Shard<T> eval_shard(const rmi_shard_eval* e) {
+  Shard<T> s;
+  s.base = e->lay.base;
+  s.n_global = e->lay.n_global;
+  s.n_local = e->ds->n;
+  s.n_avail = e->ds->n;
+  s.has_prev = e->lay.has_prev;
+  s.is_last = e->lay.is_last;
+  s.prev_key = key_from_bits<T>(e->lay.prev_key_bits);
+  s.prev_F = e->lay.prev_F;
+  s.no_dups = e->lay.no_dups ? 1 : 0;
+  return s;
+}
+
+uint64_t eval_partial_words(const rmi_shard_eval* e) { return e->lay.no_dups ? e->N : 2 * e->N; }
+
+int eval_bounds(rmi_shard_eval* e, u64* d_S, cudaStream_t st) {
+  CUDA_TRY(cudaSetDevice(e->ds->device));
+  e->st = st;
+  e->t_start = std::chrono::steady_clock::now();
+  const rmi_result& r = *e->r;
+  cudaEventRecord(e->ev[0], st);
+  const TopModel h_top = e->tables.given(r);
+  cudaMemcpyAsync(e->d_top, &h_top, sizeof(h_top), cudaMemcpyHostToDevice, st);
+  cudaMemcpyAsync(e->d_params, r.l1_params, sizeof(double) * e->N * leaf_params_per_model(e->leaf->kind),
+                  cudaMemcpyHostToDevice, st);
+  if (e->tables.t32_len) cudaMemcpyAsync(e->tables.t32, r.l0_table32, sizeof(u32) * e->tables.t32_len, cudaMemcpyHostToDevice, st);
+  if (e->tables.hist_bins) cudaMemcpyAsync(e->tables.pivots, r.l0_array2, sizeof(u64) * e->tables.hist_bins, cudaMemcpyHostToDevice, st);
+  cudaMemsetAsync(e->d_aux, 0, sizeof(BuildAux), st);
+  cudaEventRecord(e->ev[1], st);
+  Launch L{st, e->num_sms};
+  with_key_type(e->ds->key_type, [&](auto k) {
+    using T = decltype(k);
+    shard_bounds_given<T>(L, (const T*)e->ds->d_keys, eval_shard<T>(e), e->top->kind, e->d_top, e->N, d_S, e->d_aux);
+  });
+  CUDA_TRY(cudaGetLastError());
+  return RMI_OK;
+}
+
+int eval_keys(rmi_shard_eval* e, const u64* d_S, u64* d_part, unsigned* d_status, cudaStream_t st) {
+  CUDA_TRY(cudaSetDevice(e->ds->device));
+  e->st = st;
+  cudaEventRecord(e->ev[2], st);
+  Launch L{st, e->num_sms};
+  with_key_type(e->ds->key_type, [&](auto k) {
+    using T = decltype(k);
+    shard_evaluate_partials<T>(L, (const T*)e->ds->d_keys, eval_shard<T>(e), e->lay.is_first, e->lay.has_next,
+                               key_from_bits<T>(e->lay.next_key_bits), e->leaf->kind, e->N, d_S, e->d_params, d_part);
+  });
+  shard_copy_status(L, e->d_aux, d_status);
+  CUDA_TRY(cudaGetLastError());
+  return RMI_OK;
+}
+
+int eval_finish(rmi_shard_eval* e, const u64* d_S, const u64* d_part, unsigned status, uint32_t flags, const char* fn,
+                rmi_result** out) {
+  CUDA_TRY(cudaSetDevice(e->ds->device));
+  cudaStream_t st = e->st;
+  const uint64_t n = e->lay.n_global, N = e->N;
+  const bool stats_only = (flags & RMI_FLAG_STATS_ONLY) != 0;
+  const bool want_counts = !stats_only && (flags & RMI_FLAG_LEAF_COUNTS) != 0;
+  Launch L{st, e->num_sms};
+  cudaEventRecord(e->ev[3], st);
+  shard_evaluate_finish(L, n, N, e->lay.no_dups, d_S, d_part, e->d_errors, e->d_counts);
+  leaf_statistics(L, n, N, e->d_errors, e->d_counts, e->d_aux, e->d_stats);
+  cudaEventRecord(e->ev[4], st);
+  // the host buffers are taken while the kernels run
+  auto box = new ResultBox();
+  if (!reserve_result(box, &e->tables, N, leaf_params_per_model(e->leaf->kind), !stats_only, want_counts)) {
+    cudaStreamSynchronize(st);
+    delete box;
+    return fail(RMI_ERR_CUDA, kPinnedFailed);
+  }
+  copy_result_to_host(box, nullptr, e->d_aux, e->d_top, nullptr, nullptr, nullptr, st);
+  if (!stats_only) {
+    cudaMemcpyAsync(box->l1_errors.data(), e->d_errors, sizeof(u64) * N, cudaMemcpyDeviceToHost, st);
+    if (want_counts) cudaMemcpyAsync(box->l1_counts.data(), e->d_counts, sizeof(u64) * N, cudaMemcpyDeviceToHost, st);
+  }
+  const cudaError_t ce = cudaStreamSynchronize(st);
+  if (ce != cudaSuccess) { delete box; return fail(RMI_ERR_CUDA, std::string(fn) + ": " + cudaGetErrorString(ce)); }
+  // status: the OR over every rank, so that all of them fail alike; this rank's own word is in it
+  const unsigned bad = (status | result_aux(box).status) & kEvaluateStatus;
+  if (bad) { delete box; return fail(RMI_ERR_PANIC, status_text(bad)); }
+  fill_given_result(box, e->r, *e->top, *e->leaf, e->tables, n, stats_only);
+  rmi_result& R = box->pub;
+  for (int q = 0; q < 4; ++q) {
+    R.phase_device_ns[q] = elapsed_ns(e->ev[q], e->ev[q + 1]);
+    R.device_time_ns += R.phase_device_ns[q];
+  }
+  R.build_time_ns =
+      (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - e->t_start).count();
+  *out = &box->pub;
+  return RMI_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int rmi_shard_eval_create(const rmi_result* r, const rmi_dataset* local, const rmi_shard_ends* ends_all, int world,
+                          int rank, rmi_shard_eval** out) {
+  const std::string fn = "rmi_shard_eval_create";
+  g_last_error.clear();
+  if (!r || !local || !ends_all || !out) return fail(RMI_ERR_INVALID, fn + ": null argument");
+  const ModelName *top = nullptr, *leaf = nullptr;
+  if (int rc = check_result(r, false, fn, &top, &leaf)) return rc;
+  uint64_t total = 0, base = 0;
+  if (int rc = check_slabs(fn, local, ends_all, world, rank, &base, &total)) return rc;
+  // rmi_evaluate's checks of the concatenated keys: leaves, no keys, this slab's order
+  if (int rc = check_build(total, r->branching_factor, local->sorted)) return rc;
+  CUDA_TRY(cudaSetDevice(local->device));
+  DeviceInfo di;
+  if (int rc = device_info(local->device, &di)) return rc;
+  auto* e = new rmi_shard_eval();
+  e->r = r; e->ds = local; e->top = top; e->leaf = leaf;
+  e->world = world; e->rank = rank; e->num_sms = di.num_sms;
+  e->N = r->branching_factor;
+  e->lay = with_key_type(local->key_type, [&](auto k) { return slab_layout<decltype(k)>(ends_all, world, rank); });
+  const uint64_t N = e->N;
+  bool ok = cudaStreamCreateWithFlags(&e->own, cudaStreamNonBlocking) == cudaSuccess;
+  for (int q = 0; q < SHARD_EVAL_EVENTS; ++q) ok = ok && cudaEventCreate(&e->ev[q]) == cudaSuccess;
+  ok = ok && (e->d_top = (TopModel*)device_alloc(sizeof(TopModel))) && (e->d_aux = (BuildAux*)device_alloc(sizeof(BuildAux))) &&
+       (e->d_params = (double*)device_alloc(sizeof(double) * N * leaf_params_per_model(leaf->kind))) &&
+       (e->d_errors = (u64*)device_alloc(sizeof(u64) * N)) && (e->d_counts = (u64*)device_alloc(sizeof(u64) * N)) &&
+       (e->d_stats = device_alloc(stats_scratch_bytes(N))) && (e->d_S = (u64*)device_alloc(sizeof(u64) * (N + 1))) &&
+       (e->d_part = (u64*)device_alloc(sizeof(u64) * 2 * N)) &&
+       (e->d_status = (unsigned*)device_alloc(sizeof(unsigned) * world));
+  // the top tables' device homes (their contents are copied again at every evaluation)
+  ok = ok && e->tables.upload(*r, e->own, device_alloc) == cudaSuccess && cudaStreamSynchronize(e->own) == cudaSuccess;
+  if (!ok) {
+    cudaGetLastError();
+    rmi_shard_eval_destroy(e);
+    return fail(RMI_ERR_CUDA, fn + ": device allocation failed");
+  }
+  *out = e;
+  return RMI_OK;
+}
+
+void rmi_shard_eval_destroy(rmi_shard_eval* e) {
+  if (!e) return;
+  e->tables.free_device();
+  for (void* p : {(void*)e->d_top, (void*)e->d_aux, (void*)e->d_params, (void*)e->d_errors, (void*)e->d_counts, e->d_stats,
+                  (void*)e->d_S, (void*)e->d_part, (void*)e->d_status})
+    cudaFree(p);
+  for (cudaEvent_t v : e->ev) if (v) cudaEventDestroy(v);
+  if (e->own) cudaStreamDestroy(e->own);
+  delete e;
+}
+
+uint64_t rmi_shard_eval_partial_words(const rmi_shard_eval* e) { return e ? eval_partial_words(e) : 0; }
+
+int rmi_shard_eval_bounds(rmi_shard_eval* e, uint64_t* d_S, void* cuda_stream) {
+  g_last_error.clear();
+  if (!e || !d_S) return fail(RMI_ERR_INVALID, "rmi_shard_eval_bounds: null argument");
+  return eval_bounds(e, (u64*)d_S, (cudaStream_t)cuda_stream);
+}
+
+int rmi_shard_eval_keys(rmi_shard_eval* e, const uint64_t* d_S, uint64_t* d_partial, uint32_t* d_status, void* cuda_stream) {
+  g_last_error.clear();
+  if (!e || !d_S || !d_partial || !d_status) return fail(RMI_ERR_INVALID, "rmi_shard_eval_keys: null argument");
+  return eval_keys(e, (const u64*)d_S, (u64*)d_partial, (unsigned*)d_status, (cudaStream_t)cuda_stream);
+}
+
+int rmi_shard_eval_finish(rmi_shard_eval* e, const uint64_t* d_S, const uint64_t* d_partial, uint32_t status,
+                          uint32_t flags, rmi_result** out) {
+  g_last_error.clear();
+  if (!e || !d_S || !d_partial || !out) return fail(RMI_ERR_INVALID, "rmi_shard_eval_finish: null argument");
+  return eval_finish(e, (const u64*)d_S, (const u64*)d_partial, status, flags, "rmi_shard_eval_finish", out);
+}
+
+int rmi_shard_evaluate(rmi_shard_eval* e, rmi_shard_comm* c, uint32_t flags, rmi_result** out) {
+  const char* fn = "rmi_shard_evaluate";
+  g_last_error.clear();
+  if (!e || !c || !out) return fail(RMI_ERR_INVALID, std::string(fn) + ": null argument");
+  if (c->world != e->world || c->rank != e->rank)
+    return fail(RMI_ERR_INVALID, std::string(fn) + ": the communicator is rank " + std::to_string(c->rank) + " of " +
+                                     std::to_string(c->world) + ", the evaluator rank " + std::to_string(e->rank) + " of " +
+                                     std::to_string(e->world));
+  const NcclApi& nc = nccl_api();
+  if (!nc.ok) return fail(RMI_ERR_UNSUPPORTED, nc.error);
+  const int W = e->world;
+  cudaStream_t st = e->own;
+  if (int rc = eval_bounds(e, e->d_S, st)) return rc;
+  if (W > 1) NCCL_TRY(nc.AllReduce(e->d_S, e->d_S, e->N + 1, ncclUint64, ncclMin, c->comm, st));
+  if (int rc = eval_keys(e, e->d_S, e->d_part, e->d_status + e->rank, st)) return rc;
+  if (W > 1) {
+    NCCL_TRY(nc.GroupStart());
+    NCCL_TRY(nc.AllReduce(e->d_part, e->d_part, eval_partial_words(e), ncclUint64, ncclMax, c->comm, st));
+    NCCL_TRY(nc.AllGather(e->d_status + e->rank, e->d_status, 1, ncclUint32, c->comm, st));
+    NCCL_TRY(nc.GroupEnd());
+  }
+  std::vector<unsigned> all(W, 0);
+  CUDA_TRY(cudaMemcpyAsync(all.data(), e->d_status, sizeof(unsigned) * W, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  unsigned status = 0;
+  for (unsigned s : all) status |= s;
+  return eval_finish(e, e->d_S, e->d_part, status, flags, fn, out);
 }
 
 }  // extern "C"

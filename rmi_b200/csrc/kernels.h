@@ -155,6 +155,18 @@ template <class T>
 void evaluate_leaves(const Launch& L, const T* keys, u64 n, bool no_dups, int leaf_kind, u64 N, const u64* d_S,
                      const double* d_params, u64* d_scratch, u64* d_errors, u64* d_counts);
 
+// ---- error pass over given leaf tables on a range-partitioned key array (kernels_shard_eval.cu, DESIGN.md section 15)
+// This rank's contributions, from the global boundaries d_S, into d_part = part_err | part_run (2 x N u64, zeroed
+// here): the per-key errors and the runs that end on this slab, and the widening terms whose key this slab holds.
+// is_first: the first non-empty rank; has_next / next_key: the first key of the next non-empty rank.  sh.no_dups
+// (identical on every rank) skips the run tracking.  After an all-reduce MAX of d_part (its first N words suffice when
+// sh.no_dups), shard_evaluate_finish writes the N error bounds and key counts rmi_evaluate gives on the whole keys.
+template <class T>
+void shard_evaluate_partials(const Launch& L, const T* keys, const Shard<T>& sh, int is_first, int has_next, T next_key,
+                             int leaf_kind, u64 N, const u64* d_S, const double* d_params, u64* d_part);
+void shard_evaluate_finish(const Launch& L, u64 n, u64 N, bool no_dups, const u64* d_S, const u64* d_part, u64* d_errors,
+                           u64* d_counts);
+
 // ---- cross-rank pieces of a range-partitioned build (kernels_leaf.cu) --------------------------
 // d_off[r] = first leaf owned by rank r, d_off[world] = N (d_bases: global index of every rank's first key,
 // world + 1 entries; r_last: last rank that holds keys).  One tiny kernel, no host involvement.
@@ -254,6 +266,11 @@ void shard_top_finish(const Launch& L, const Shard<T>& sh, int kind, u64 N, doub
 template <class T>
 void shard_bounds(const Launch& L, const T* keys, const Shard<T>& sh, int kind, const TopModel* d_top, u64 N, u64* d_S,
                   BuildAux* d_aux);
+// The streaming boundary pass for every top group (a given top model, not known to be monotone): S_local, n_global
+// where no local key reaches a leaf, ST_NOT_SORTED / ST_NON_MONOTONE also across the cut before the slab.
+template <class T>
+void shard_bounds_given(const Launch& L, const T* keys, const Shard<T>& sh, int kind, const TopModel* d_top, u64 N,
+                        u64* d_S, BuildAux* d_aux);
 template <class T>
 void shard_split(const Launch& L, const T* keys, const Shard<T>& sh, int kind, const TopModel* d_top, u64 N,
                  const u64* d_S, BuildAux* d_aux);

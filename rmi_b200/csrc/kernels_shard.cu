@@ -652,6 +652,24 @@ void shard_bounds(const Launch& L, const T* keys, const Shard<T>& sh, int kind, 
   }
 }
 
+// A GIVEN top model (rmi_shard_eval) is not known to be monotone on the keys, so every top group takes the streaming
+// pass, which also checks the order of the targets across the cuts.
+template <class T>
+void shard_bounds_given(const Launch& L, const T* keys, const Shard<T>& sh, int kind, const TopModel* d_top, u64 N,
+                        u64* d_S, BuildAux* d_aux) {
+  switch (kind) {
+    case M_LINEAR: case M_ROBUST_LINEAR: case M_LINEAR_SPLINE: shard_bounds_stream<T, M_LINEAR>(L, keys, sh, d_top, N, d_S, d_aux); break;
+    case M_CUBIC: shard_bounds_stream<T, M_CUBIC>(L, keys, sh, d_top, N, d_S, d_aux); break;
+    case M_LOGLINEAR: shard_bounds_stream<T, M_LOGLINEAR>(L, keys, sh, d_top, N, d_S, d_aux); break;
+    case M_NORMAL: shard_bounds_stream<T, M_NORMAL>(L, keys, sh, d_top, N, d_S, d_aux); break;
+    case M_LOGNORMAL: shard_bounds_stream<T, M_LOGNORMAL>(L, keys, sh, d_top, N, d_S, d_aux); break;
+    case M_RADIX: shard_bounds_stream<T, M_RADIX>(L, keys, sh, d_top, N, d_S, d_aux); break;
+    case M_RADIX_TABLE: shard_bounds_stream<T, M_RADIX_TABLE>(L, keys, sh, d_top, N, d_S, d_aux); break;
+    case M_BRADIX: shard_bounds_stream<T, M_BRADIX>(L, keys, sh, d_top, N, d_S, d_aux); break;
+    default: shard_bounds_stream<T, M_HISTOGRAM>(L, keys, sh, d_top, N, d_S, d_aux); break;
+  }
+}
+
 template <class T>
 void shard_split(const Launch& L, const T* keys, const Shard<T>& sh, int kind, const TopModel* d_top, u64 N,
                  const u64* d_S, BuildAux* d_aux) {
@@ -708,6 +726,7 @@ void shard_copy_flags(const Launch& L, const BuildAux* d_aux, unsigned* d_out2) 
   template void shard_top_finish<T>(const Launch&, const Shard<T>&, int, u64, double, double, const double*, T, T, u64,   \
                                     const void*, TopModel*, BuildAux*);                                             \
   template void shard_bounds<T>(const Launch&, const T*, const Shard<T>&, int, const TopModel*, u64, u64*, BuildAux*); \
+  template void shard_bounds_given<T>(const Launch&, const T*, const Shard<T>&, int, const TopModel*, u64, u64*, BuildAux*); \
   template void shard_split<T>(const Launch&, const T*, const Shard<T>&, int, const TopModel*, u64, const u64*, BuildAux*); \
   template void shard_table_local<T>(const Launch&, const T*, const Shard<T>&, int, int, u64, T, T, BuildAux*, u32*, u64*, u64, u64);
 INST(u64)

@@ -20,6 +20,9 @@ CPU tests (gloo, world_size 2) plug in a numpy engine to exercise exactly this h
 
 ShardedRMIIndex serves lookups over the same slabs (DESIGN.md section 14): a query goes to the rank whose slab holds
 its lower bound, is searched there, and its global answer comes back.
+
+evaluate_sharded measures a given RMI's error bounds over the same slabs (DESIGN.md section 15): every rank streams
+only its own keys, and one all-reduce MAX of per-leaf maxima combines them.
 """
 from __future__ import annotations
 
@@ -311,6 +314,9 @@ class CudaShardEngine:
     def lookup_index(self, trained, ends_all: np.ndarray, world: int, rank: int) -> "CudaShardIndex":
         return CudaShardIndex(self, trained, ends_all, world, rank)
 
+    def evaluator(self, trained, ends_all: np.ndarray, world: int, rank: int) -> "CudaShardEval":
+        return CudaShardEval(self, trained, ends_all, world, rank)
+
     def end(self):
         if self._build is not None:
             self.lib.rmi_shard_build_destroy(self._build)
@@ -505,6 +511,60 @@ def train_sharded(data, model_spec: str, num_leaves: int, flags: int = 0, group=
     return _retry_with_larger_halo(data, bufs, bases, n_global, N, model_spec, num_leaves, flags, group, world, dev, counts, native)
 
 
+def evaluate_sharded(trained, data, flags: int = 0, group=None, engine=None, counts: bool = True,
+                     native: bool | None = None):
+    """api.evaluate of ``trained``'s tables over a range-partitioned key array (DESIGN.md section 15): the error bounds,
+    key counts (counts=True) and statistics of the concatenated slabs, bit for bit, on every rank; the tables are
+    returned unchanged.  Each rank reads only its own keys.  Raises RMIPanic on every rank where the top model is not
+    monotone on the keys (a cut included).
+
+    native=None (default): with the CUDA engine over an NCCL group it is ONE library call (rmi_shard_evaluate);
+    otherwise (gloo, a numpy engine, native=False) the phases are driven here: bounds -> all-reduce MIN of S -> keys ->
+    all-reduce MAX of the partial maxima and an all-gather of the status words -> finish."""
+    eng = engine if engine is not None else data.engine
+    group = group if group is not None else getattr(data, "group", None)
+    rank, world = _world(group)
+    dev = eng.device
+    flags = int(flags) | (api.FLAG_LEAF_COUNTS if counts else 0)
+    ev = eng.evaluator(trained, gather_ends(data, eng, group), world, rank)
+    try:
+        comm = None
+        if native is not False and isinstance(ev, CudaShardEval):
+            comm = native_comm(group, dev, single_rank_ok=native is True)
+            if native is True and comm is None:
+                raise api.RMIError("native=True needs an NCCL process group (or a single rank) and a loadable libnccl.so.2")
+        if comm is not None:
+            return ev.evaluate(comm, flags)
+        # gloo cannot reduce device memory (one-GPU test boxes): stage through the host there
+        stage = world > 1 and dev.type == "cuda" and dist.get_backend(group) == "gloo"
+
+        def all_reduce(t, op):
+            if world <= 1:
+                return
+            h = t.cpu() if stage else t
+            dist.all_reduce(h, op=op, group=group)
+            if stage:
+                t.copy_(h)
+
+        S = ev.bounds()
+        all_reduce(S, dist.ReduceOp.MIN)
+        part, status = ev.keys(S)
+        all_reduce(part[: ev.partial_words], dist.ReduceOp.MAX)
+        # the status word is a BIT MASK: every rank ORs every rank's word, so that all of them fail alike
+        st = status.cpu() if stage else status
+        st_all = [torch.empty_like(st) for _ in range(world)]
+        if world > 1:
+            dist.all_gather(st_all, st, group=group)
+        else:
+            st_all = [st]
+        acc = 0
+        for t in st_all:
+            acc |= int(t[0]) & 0xFFFFFFFF
+        return ev.finish(S, part, acc, flags)
+    finally:
+        ev.close()
+
+
 def _retry_with_larger_halo(data, bufs, bases, n_global, N, model_spec, num_leaves, flags, group, world, dev, counts, native):
     # A leaf reaches past the prefetched halo (heavy skew).  The status word is the OR over ranks, so
     # every rank arrives here together: size the halo from the global boundaries S and build again.
@@ -647,6 +707,69 @@ class CudaShardIndex:
             pass
 
 
+class CudaShardEval:
+    """One rank's side of evaluate_sharded on librmi_b200.so (rmi_shard_eval_*).  bounds / keys enqueue on the current
+    torch stream of the data's device and return device tensors (int64 storage of the u64 words)."""
+
+    def __init__(self, eng: CudaShardEngine, trained, ends_all: np.ndarray, world: int, rank: int):
+        L = self.lib = api.load_library()
+        L.rmi_shard_eval_create.argtypes = [C.POINTER(api._Result), C.c_void_p, C.POINTER(_Ends), C.c_int, C.c_int,
+                                            C.POINTER(C.c_void_p)]
+        L.rmi_shard_eval_destroy.argtypes = [C.c_void_p]
+        L.rmi_shard_eval_partial_words.argtypes = [C.c_void_p]
+        L.rmi_shard_eval_partial_words.restype = C.c_uint64
+        L.rmi_shard_eval_bounds.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        L.rmi_shard_eval_keys.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.rmi_shard_eval_finish.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32,
+                                            C.POINTER(C.POINTER(api._Result))]
+        L.rmi_shard_evaluate.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(C.POINTER(api._Result))]
+        self.device = eng.device
+        self._ds = eng.ds             # the slab and the result are read at every evaluation: kept alive with it
+        self._trained = trained
+        self._spec = trained.models
+        self.N = int(trained.branching_factor)
+        ends = (_Ends * world)(*[_Ends(*(int(v) for v in row[:5])) for row in ends_all])
+        self._h = C.c_void_p()
+        api._check(L.rmi_shard_eval_create(api._result_ptr(trained), eng.ds._h, ends, world, rank, C.byref(self._h)))
+        self.partial_words = int(L.rmi_shard_eval_partial_words(self._h))
+
+    def _stream(self):
+        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream or None)
+
+    def bounds(self) -> torch.Tensor:
+        S = torch.empty(self.N + 1, dtype=torch.int64, device=self.device)
+        api._check(self.lib.rmi_shard_eval_bounds(self._h, S.data_ptr(), self._stream()))
+        return S
+
+    def keys(self, S: torch.Tensor):
+        part = torch.empty(2 * self.N, dtype=torch.int64, device=self.device)
+        status = torch.zeros(1, dtype=torch.int32, device=self.device)
+        api._check(self.lib.rmi_shard_eval_keys(self._h, S.data_ptr(), part.data_ptr(), status.data_ptr(), self._stream()))
+        return part, status
+
+    def finish(self, S: torch.Tensor, part: torch.Tensor, status: int, flags: int):
+        res = C.POINTER(api._Result)()
+        api._check(self.lib.rmi_shard_eval_finish(self._h, S.data_ptr(), part.data_ptr(), int(status), int(flags),
+                                                  C.byref(res)))
+        return api.result_from_pointer(res, self._spec)
+
+    def evaluate(self, comm, flags: int):
+        res = C.POINTER(api._Result)()
+        api._check(self.lib.rmi_shard_evaluate(self._h, comm, int(flags), C.byref(res)))
+        return api.result_from_pointer(res, self._spec)
+
+    def close(self):
+        if getattr(self, "_h", None) and self._h.value:
+            self.lib.rmi_shard_eval_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 class ShardedRMIIndex:
     """A trained RMI served over range-partitioned keys: rank r holds the r-th slab (`data`, a ShardedTrainingData)
     and the whole model.  `trained` is any TrainedRMI of the whole key set: from train_sharded, from rmi_train of the
@@ -670,19 +793,24 @@ class ShardedRMIIndex:
         self.index = eng.lookup_index(trained, gather_ends(data, eng, self.group), self.world, self.rank)
 
     @classmethod
-    def load(cls, namespace: str, data, out_dir: str = ".", data_dir: str = "rmi_data", group=None) -> "ShardedRMIIndex":
-        """load_rmi of a generated artefact, served over the slabs: train once, serve over shards."""
+    def load(cls, namespace: str, data, out_dir: str = ".", data_dir: str = "rmi_data", group=None,
+             evaluate: bool = False) -> "ShardedRMIIndex":
+        """load_rmi of a generated artefact, served over the slabs: train once, serve over shards.  evaluate=True
+        measures the artefact's error bounds over the slabs first (evaluate_sharded, collective): a --no-errors
+        artefact, or one whose keys have changed since it was generated, is then served with bounds that hold."""
         trained, cf = api.load_rmi(namespace, out_dir, data_dir)
         if cf is not None:
             raise api.RMIError("a --bounded artefact cannot be served over range-partitioned keys: its cache-fix spline "
                                "indexes the whole key array on one GPU")
-        if trained.last_layer_max_l1s is None:
-            raise api.RMIError("a --no-errors artefact cannot be served over range-partitioned keys: its error bounds "
-                               "would have to be measured over the slabs, and a sharded evaluate does not exist")
+        if trained.last_layer_max_l1s is None and not evaluate:
+            raise api.RMIError("a --no-errors artefact holds no error bounds: load it with evaluate=True to measure them "
+                               "over the slabs")
         want = (api.KEY_F64,) if trained.key_type == api.KEY_F64 else (api.KEY_U64, api.KEY_U32)
         if data.key_type not in want:
             raise api.RMIError(f"the artefact's lookup takes {'double' if trained.key_type == api.KEY_F64 else 'uint64_t'} "
                                f"keys, the data holds {np.dtype(_NP_OF_KEY[data.key_type])}")
+        if evaluate:
+            trained = evaluate_sharded(trained, data, group=group)
         return cls(trained, data, group)
 
     def _queries(self, q: torch.Tensor) -> torch.Tensor:
