@@ -251,16 +251,6 @@ typedef struct {          /* what a rank publishes about its slab (host struct) 
 } rmi_shard_ends;
 int rmi_shard_ends_get(const rmi_dataset* ds, rmi_shard_ends* out);
 
-typedef struct {
-  uint64_t base, n_global;                 /* global index of local key 0, total keys */
-  int32_t has_prev, is_last;
-  uint64_t prev_key_bits, prev_F;          /* last key before this slab and its duplicate-fixed offset */
-  uint64_t first_key_bits, last_key_bits, last_F;   /* global first / last key, offset of the last */
-  uint64_t halo_capacity;                  /* keys of room behind the local keys in the device array */
-  uint64_t no_dups;                        /* 1 if no two keys of the WHOLE data set are equal */
-  double pivot_x, pivot_y;                 /* common pivot of the top-level sums (any value, same on all ranks) */
-} rmi_shard_info;
-
 typedef struct {          /* device buffers owned by the caller (the collectives run on them) */
   void* sums;             /* 16 x 8 bytes: [0,8) f64 sums (SUM rounds), [8,16) i64 slots (MIN round) */
   void* S;                /* (N+1) x u64 */
@@ -282,19 +272,27 @@ enum { RMI_PHASE_TOP_LOCAL = 0, RMI_PHASE_TOP_FINISH = 1, RMI_PHASE_BOUNDS = 2, 
  *                                                                       (normal, lognormal)
  *    3  TOP_LOCAL -> all-reduce MIN of sums[8,12) as SIGNED 64-bit integers -> TOP_MID
  *                 -> SUM f64 sums[0,8) -> TOP_FINISH                    (cubic)
- *    4  TOP_LOCAL -> all-reduce MAX of the top model's table (rmi_shard_top_table: 2^bits u32 hints of a radix
- *                 table, or the u64 pivots of a histogram; every entry has one writer, the others hold 0)
- *                 -> TOP_FINISH                                          (radix8..28, histogram) */
+ *    4  TOP_LOCAL -> all-reduce MAX of the top model's table (2^bits u32 hints of a radix table, or the u64 pivots
+ *                 of a histogram; every entry has one writer, the others hold 0) -> TOP_FINISH
+ *                                                                       (radix8..28, histogram)
+ *       rmi_shard_train merges the table itself; the host has no handle on it, so the host-driven phases cannot run
+ *       these tops over more than one rank. */
 int rmi_shard_top_rounds(const char* top_model_name);
 
+/* rmi_shard_build_create: one rank's build object.  ends_all holds every rank's rmi_shard_ends (rmi_shard_ends_get,
+ * gathered over the ranks), as for rmi_shard_index_create; the library derives from it this rank's base, the key before
+ * its slab and that key's run start, the global first and last keys and whether the whole key set is duplicate-free.
+ * halo_capacity: keys of room behind the local keys in local's device array (rmi_shard_set_halo may fill up to that).
+ * Refused before any device work, in this order: a null argument (RMI_ERR_INVALID); the model spec as rmi_train
+ * refuses it; a top model not offered here (RMI_ERR_UNSUPPORTED); the ends-table checks of rmi_shard_index_create
+ * (world / rank, ends_all[rank] not describing local, slabs out of key order); then rmi_train's checks of the
+ * concatenated keys (branching factor 0, no keys, a local dataset that is not sorted: RMI_ERR_PANIC).  The object may
+ * run any number of builds with these arguments; local and the buffers must outlive it. */
 typedef struct rmi_shard_build rmi_shard_build;
-int rmi_shard_build_create(const rmi_dataset* local, const rmi_shard_info* info, const char* model_spec,
-                           uint64_t branch_factor, const rmi_shard_buffers* buffers, void* cuda_stream,
-                           rmi_shard_build** out);
+int rmi_shard_build_create(const rmi_dataset* local, const rmi_shard_ends* ends_all, int world, int rank,
+                           const char* model_spec, uint64_t branch_factor, uint64_t halo_capacity,
+                           const rmi_shard_buffers* buffers, void* cuda_stream, rmi_shard_build** out);
 int rmi_shard_phase(rmi_shard_build* b, int phase);
-/* The device buffer a rounds-4 top model needs all-reduced with MAX between TOP_LOCAL and TOP_FINISH (elem_bytes 4 or 8;
- * count 0 for the other top models).  rmi_shard_train does this itself. */
-int rmi_shard_top_table(rmi_shard_build* b, void** device_ptr, uint64_t* count, int* elem_bytes);
 int rmi_shard_set_halo(rmi_shard_build* b, uint64_t halo_keys);
 int rmi_shard_finish(rmi_shard_build* b, uint32_t flags, rmi_result** out);
 void rmi_shard_build_destroy(rmi_shard_build* b);
@@ -313,13 +311,12 @@ uint32_t rmi_params_per_model(const char* leaf_model_name);
  *                    panic on any rank, fails the call on EVERY rank with the same message)
  * Setup per communicator: rank 0 calls rmi_shard_comm_unique_id and ships the 128 bytes to the other ranks by any
  * means (rmi_b200/sharded.py: torch.distributed broadcast); every rank then calls rmi_shard_comm_create (collective).
- * Setup per build object: rmi_shard_set_partition (global index of every rank's first key, world+1 entries) and, as
- * before, rmi_shard_set_halo.  The host-driven rmi_shard_phase flow above remains (CPU tests drive it over gloo). */
+ * Setup per build object: rmi_shard_set_halo, as for the phases; c must have the build's world and rank.  The
+ * host-driven rmi_shard_phase flow above remains (CPU tests drive it over gloo). */
 typedef struct rmi_shard_comm rmi_shard_comm;
 int rmi_shard_comm_unique_id(void* out_id128);
 int rmi_shard_comm_create(const void* id128, int world, int rank, int device, rmi_shard_comm** out);
 void rmi_shard_comm_destroy(rmi_shard_comm* c);
-int rmi_shard_set_partition(rmi_shard_build* b, const uint64_t* bases, int world, int rank);
 int rmi_shard_train(rmi_shard_build* b, rmi_shard_comm* c, uint32_t flags, rmi_result** out);
 
 /* ---- Lookups over a range-partitioned data set (DESIGN.md section 14) ------------------------------------------

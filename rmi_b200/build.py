@@ -16,7 +16,8 @@ SOURCES = ["kernels_top.cu", "kernels_leaf.cu", "kernels_shard.cu", "kernels_loo
            "kernels_shard_lookup.cu", "kernels_shard_eval.cu", "api.cu"]
 HEADERS = ["rust_math.cuh", "models.cuh", "device_util.cuh", "spline.cuh", "lookup_search.cuh", "kernels.h", "nccl_dl.h",
            os.path.join("..", "..", "include", "rmi_b200.h"), os.path.join("..", "..", "host", "cache_fix.hpp"), os.path.join("..", "..", "host", "codegen.hpp"),
-           os.path.join("..", "..", "host", "optimizer.hpp"), os.path.join("..", "..", "host", "artefact_load.hpp")]
+           os.path.join("..", "..", "host", "optimizer.hpp"), os.path.join("..", "..", "host", "artefact_load.hpp"),
+           os.path.join("..", "..", "host", "slab_layout.hpp")]
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 # -fmad=false: the reference fuses a multiply-add only where it writes mul_add; everything

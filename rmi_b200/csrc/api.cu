@@ -27,6 +27,7 @@
 #include "../../host/artefact_load.hpp"
 #include "../../host/codegen.hpp"
 #include "../../host/optimizer.hpp"
+#include "../../host/slab_layout.hpp"
 
 using namespace rmi;
 
@@ -1611,9 +1612,14 @@ int rmi_cache_fix_device(const rmi_dataset* ds, uint64_t line_size, rmi_spline_p
 // ===========================================================================================
 // Range-partitioned build (include/rmi_b200.h, "Range-partitioned (multi-GPU) build")
 // ===========================================================================================
+using rmihost::bits_from_key;
+using rmihost::key_from_bits;
+using rmihost::SlabLayout;
+
 struct rmi_shard_build {
   const rmi_dataset* ds = nullptr;
-  rmi_shard_info info{};
+  SlabLayout lay;
+  uint64_t halo_capacity = 0;           // keys of room behind the local keys in the device array
   rmi_shard_buffers buf{};
   const ModelName* top = nullptr;
   const ModelName* leaf = nullptr;
@@ -1634,9 +1640,8 @@ struct rmi_shard_build {
   cudaEvent_t ev_end[RMI_NUM_PHASES] = {};
   bool ran[RMI_NUM_PHASES] = {};
   // rmi_shard_train: the partition of the key array over the ranks and the exchange scratch
-  int world = 0, rank = -1, r_last = 0;
-  std::vector<uint64_t> bases;          // world + 1
-  u64* d_bases = nullptr;               // world + 1
+  int world = 0, rank = 0, r_last = 0;  // r_last: the last rank that holds keys
+  u64* d_bases = nullptr;               // world + 1: global index of every rank's first key
   u64* d_off = nullptr;                 // world + 1: first leaf owned by every rank
   u64* h_off = nullptr;                 // pinned mirror
   void* d_parts = nullptr;              // world x statistics partials
@@ -1648,7 +1653,7 @@ struct rmi_shard_build {
   u64 leaf_lo = 0, leaf_hi = 0;             //   each slice's records copied to the host while the next slice computes
   // table tops (radix8..28, histogram): the table every rank fills its part of, merged by an all-reduce MAX
   TopTables tables;
-  cudaEvent_t ev_off = nullptr, ev_t0 = nullptr, ev_t1 = nullptr, ev_leaf0 = nullptr, ev_leaf1 = nullptr;
+  cudaEvent_t ev_off = nullptr, ev_t0 = nullptr, ev_t1 = nullptr;
 };
 
 struct rmi_shard_comm {
@@ -1670,30 +1675,18 @@ struct rmi_shard_comm {
 
 namespace {
 
-template <class T> T key_from_bits(uint64_t bits) {
-  T k;
-  if (sizeof(T) == 4) { uint32_t v = (uint32_t)bits; memcpy(&k, &v, 4); }
-  else memcpy(&k, &bits, 8);
-  return k;
-}
-template <class T> uint64_t bits_from_key(T k) {
-  uint64_t bits = 0;
-  if (sizeof(T) == 4) { uint32_t v; memcpy(&v, &k, 4); bits = v; }
-  else memcpy(&bits, &k, 8);
-  return bits;
-}
-
-template <class T> Shard<T> make_shard(const rmi_shard_build* b) {
+// The kernels' view of a rank's slab: its place among the others, its own keys and the halo keys readable behind them.
+template <class T> Shard<T> shard_of(const SlabLayout& lay, uint64_t n_local, uint64_t n_avail) {
   Shard<T> s;
-  s.base = b->info.base;
-  s.n_global = b->info.n_global;
-  s.n_local = b->ds->n;
-  s.n_avail = b->ds->n + b->halo;
-  s.has_prev = b->info.has_prev;
-  s.is_last = b->info.is_last;
-  s.prev_key = key_from_bits<T>(b->info.prev_key_bits);
-  s.prev_F = b->info.prev_F;
-  s.no_dups = b->info.no_dups ? 1 : 0;   // global: no rank has equal keys and none straddle a cut
+  s.base = lay.base;
+  s.n_global = lay.n_global;
+  s.n_local = n_local;
+  s.n_avail = n_avail;
+  s.has_prev = lay.has_prev;
+  s.is_last = lay.is_last;
+  s.prev_key = key_from_bits<T>(lay.prev_key_bits);
+  s.prev_F = lay.prev_F;
+  s.no_dups = lay.no_dups ? 1 : 0;   // global: no rank has equal keys and none straddle a cut
   return s;
 }
 
@@ -1722,7 +1715,7 @@ template <class T> int shard_ends_typed(const rmi_dataset* ds, rmi_shard_ends* o
 
 template <class T> int shard_phase_typed(rmi_shard_build* b, int phase) {
   const T* keys = (const T*)b->ds->d_keys;
-  Shard<T> sh = make_shard<T>(b);
+  Shard<T> sh = shard_of<T>(b->lay, b->ds->n, b->ds->n + b->halo);
   Launch L{b->st, b->num_sms};
   L.side = b->side; L.ev_fork = b->ev_fork; L.ev_join = b->ev_join; L.d_long = b->d_long;
   const int ppm = leaf_params_per_model(b->leaf->kind);
@@ -1732,7 +1725,7 @@ template <class T> int shard_phase_typed(rmi_shard_build* b, int phase) {
     b->host_status = 0;
     for (int q = 1; q < RMI_NUM_PHASES; ++q) b->ran[q] = false;
   }
-  const T first_key = key_from_bits<T>(b->info.first_key_bits), last_key = key_from_bits<T>(b->info.last_key_bits);
+  const T first_key = key_from_bits<T>(b->lay.first_key_bits), last_key = key_from_bits<T>(b->lay.last_key_bits);
   const TopTables& tt = b->tables;
   switch (phase) {
     case RMI_PHASE_TOP_LOCAL:
@@ -1742,7 +1735,7 @@ template <class T> int shard_phase_typed(rmi_shard_build* b, int phase) {
         cudaMemcpyAsync(b->d_top, &h, sizeof(h), cudaMemcpyHostToDevice, b->st);
       }
       if (b->top->kind == M_HISTOGRAM && (tt.hist_bins == 0 || tt.hist_ipb < 1)) b->host_status |= ST_HIST_BINS;   // histogram.rs:25-27
-      b->host_status |= shard_top_local<T>(L, keys, sh, b->top->kind, b->N, b->info.pivot_x, b->info.pivot_y, first_key,
+      b->host_status |= shard_top_local<T>(L, keys, sh, b->top->kind, b->N, b->lay.pivot_x, b->lay.pivot_y, first_key,
                                            last_key, b->d_scratch, (double*)b->buf.sums);
       if ((b->top->kind == M_RADIX_TABLE || b->top->kind == M_HISTOGRAM) && b->host_status == 0)
         shard_table_local<T>(L, keys, sh, b->top->kind, b->top->table_bits, b->N, first_key, last_key, b->d_aux, tt.t32,
@@ -1752,8 +1745,8 @@ template <class T> int shard_phase_typed(rmi_shard_build* b, int phase) {
       shard_top_mid<T>(L, keys, sh, b->top->kind, b->N, first_key, last_key, b->d_scratch, (double*)b->buf.sums, b->d_aux);
       break;
     case RMI_PHASE_TOP_FINISH:
-      shard_top_finish<T>(L, sh, b->top->kind, b->N, b->info.pivot_x, b->info.pivot_y, (const double*)b->buf.sums,
-                          first_key, last_key, b->info.last_F, b->d_scratch, b->d_top, b->d_aux);
+      shard_top_finish<T>(L, sh, b->top->kind, b->N, b->lay.pivot_x, b->lay.pivot_y, (const double*)b->buf.sums,
+                          first_key, last_key, b->lay.last_F, b->d_scratch, b->d_top, b->d_aux);
       if (b->top->kind == M_RADIX_TABLE && b->host_status == 0) shard_table_decode(L, b->top->table_bits, tt.t32);
       if (b->top->kind == M_HISTOGRAM && b->host_status == 0) hist_radix_index(L, tt.pivots, tt.hist_bins, tt.radix_index);
       break;
@@ -1776,7 +1769,7 @@ template <class T> int shard_phase_typed(rmi_shard_build* b, int phase) {
       shard_copy_status(L, b->d_aux, (unsigned*)b->buf.status);
       break;
     case RMI_PHASE_STATS:
-      leaf_statistics(L, b->info.n_global, b->N, (const u64*)b->buf.errors, (const u64*)b->buf.counts, b->d_aux, b->d_stats);
+      leaf_statistics(L, b->lay.n_global, b->N, (const u64*)b->buf.errors, (const u64*)b->buf.counts, b->d_aux, b->d_stats);
       break;
     default:
       return fail(RMI_ERR_INVALID, "rmi_shard_phase: unknown phase");
@@ -1784,6 +1777,41 @@ template <class T> int shard_phase_typed(rmi_shard_build* b, int phase) {
   if (phase >= 0 && phase < RMI_NUM_PHASES) cudaEventRecord(b->ev_end[phase], b->st);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(RMI_ERR_CUDA, std::string("rmi_shard_phase: ") + cudaGetErrorString(e));
+  return RMI_OK;
+}
+
+// The checks of a gathered ends table that the consumers of range-partitioned keys (rmi_shard_build_create,
+// rmi_shard_index_create, rmi_shard_eval_create) make before any device work, with RMI_ERR_INVALID and messages naming
+// fn: world and rank in range, ends_all[rank] describing `local`, the non-empty slabs in key order.  *base / *total:
+// this rank's global index of its first key and the keys of all slabs.
+int check_slabs(const std::string& fn, const rmi_dataset* local, const rmi_shard_ends* ends_all, int world, int rank,
+                uint64_t* base, uint64_t* total) {
+  if (world < 1 || world > SHARD_ROUTE_MAX - 1 || rank < 0 || rank >= world)
+    return fail(RMI_ERR_INVALID, fn + ": bad world or rank (0 <= rank < world <= 63)");
+  if (ends_all[rank].n_local != local->n)
+    return fail(RMI_ERR_INVALID, fn + ": ends_all[" + std::to_string(rank) + "] describes " +
+                                     std::to_string(ends_all[rank].n_local) + " keys, the local dataset holds " +
+                                     std::to_string(local->n));
+  *total = 0;
+  for (int p = 0; p < world; ++p) {
+    if (p == rank) *base = *total;
+    *total += ends_all[p].n_local;
+  }
+  // the non-empty slabs must follow each other in key order: no slab's last key above the next one's first
+  int prev = -1;
+  const int bad = with_key_type(local->key_type, [&](auto k) {
+    using T = decltype(k);
+    for (int p = 0; p < world; ++p) {
+      if (!ends_all[p].n_local) continue;
+      if (prev >= 0 && key_from_bits<T>(ends_all[p].first_key_bits) < key_from_bits<T>(ends_all[prev].last_key_bits))
+        return p;
+      prev = p;
+    }
+    return -1;
+  });
+  if (bad >= 0)
+    return fail(RMI_ERR_INVALID, fn + ": the slabs are out of order (rank " + std::to_string(bad) +
+                                     "'s first key is below the last key of rank " + std::to_string(prev) + ")");
   return RMI_OK;
 }
 
@@ -1807,24 +1835,36 @@ int rmi_shard_ends_get(const rmi_dataset* ds, rmi_shard_ends* out) {
   return with_key_type(ds->key_type, [&](auto k) { return shard_ends_typed<decltype(k)>(ds, out); });
 }
 
-int rmi_shard_build_create(const rmi_dataset* local, const rmi_shard_info* info, const char* model_spec,
-                           uint64_t branch_factor, const rmi_shard_buffers* buffers, void* cuda_stream,
-                           rmi_shard_build** out) {
+int rmi_shard_build_create(const rmi_dataset* local, const rmi_shard_ends* ends_all, int world, int rank,
+                           const char* model_spec, uint64_t branch_factor, uint64_t halo_capacity,
+                           const rmi_shard_buffers* buffers, void* cuda_stream, rmi_shard_build** out) {
+  const std::string fn = "rmi_shard_build_create";
   g_last_error.clear();
-  if (!local || !info || !model_spec || !buffers || !out) return fail(RMI_ERR_INVALID, "rmi_shard_build_create: null argument");
+  if (!local || !ends_all || !model_spec || !buffers || !out) return fail(RMI_ERR_INVALID, fn + ": null argument");
   const ModelName *top = nullptr, *leaf = nullptr;
   if (int rc = parse_two_layer(model_spec, &top, &leaf)) return rc;
   if (top->shard_rounds < 0)
     return fail(RMI_ERR_UNSUPPORTED, "range-partitioned builds offer the top models linear, robust_linear, linear_spline, "
                                      "cubic, normal, lognormal, radix, radix8..28, histogram");
-  if (int rc = check_build(info->n_global, branch_factor, local->sorted)) return rc;
+  uint64_t total = 0, base = 0;
+  if (int rc = check_slabs(fn, local, ends_all, world, rank, &base, &total)) return rc;
+  if (int rc = check_build(total, branch_factor, local->sorted)) return rc;
   CUDA_TRY(cudaSetDevice(local->device));
   DeviceInfo di;
   if (int rc = device_info(local->device, &di)) return rc;
   auto* b = new rmi_shard_build();
-  b->ds = local; b->info = *info; b->buf = *buffers; b->top = top; b->leaf = leaf; b->N = branch_factor;
-  b->st = (cudaStream_t)cuda_stream; b->num_sms = di.num_sms; b->halo = 0;
+  b->ds = local; b->buf = *buffers; b->top = top; b->leaf = leaf; b->N = branch_factor;
+  b->st = (cudaStream_t)cuda_stream; b->num_sms = di.num_sms; b->halo = 0; b->halo_capacity = halo_capacity;
   b->t_start = std::chrono::steady_clock::now();
+  b->lay = with_key_type(local->key_type, [&](auto k) {
+    return rmihost::slab_layout<decltype(k)>(ends_all, world, rank, branch_factor);
+  });
+  b->world = world; b->rank = rank;
+  std::vector<uint64_t> bases(world + 1, 0);
+  for (int r = 0; r < world; ++r) {
+    bases[r + 1] = bases[r] + ends_all[r].n_local;
+    if (ends_all[r].n_local) b->r_last = r;
+  }
   bool ok = cudaMalloc(&b->d_top, sizeof(TopModel)) == cudaSuccess && cudaMalloc(&b->d_aux, sizeof(BuildAux)) == cudaSuccess &&
             cudaMalloc(&b->d_scratch, shard_scratch_bytes()) == cudaSuccess &&
             cudaMalloc(&b->d_stats, stats_scratch_bytes(branch_factor)) == cudaSuccess;
@@ -1837,18 +1877,20 @@ int rmi_shard_build_create(const rmi_dataset* local, const rmi_shard_info* info,
          cudaEventCreateWithFlags(&b->ev_join, cudaEventDisableTiming) == cudaSuccess &&
          cudaMalloc((void**)&b->d_long, sizeof(u32) * (LONG_LEAF_CAP + 1)) == cudaSuccess;
   }
-  ok = ok && b->tables.allocate(*top, info->n_global, branch_factor, device_alloc);
-  if (!ok) { rmi_shard_build_destroy(b); return fail(RMI_ERR_CUDA, "rmi_shard_build_create: device allocation failed"); }
+  ok = ok && b->tables.allocate(*top, total, branch_factor, device_alloc);
+  // rmi_shard_train's exchange: leaf ownership, statistics partials and status words of every rank
+  ok = ok && cudaMalloc((void**)&b->d_bases, sizeof(u64) * (world + 1)) == cudaSuccess &&
+       cudaMalloc((void**)&b->d_off, sizeof(u64) * (world + 1)) == cudaSuccess &&
+       cudaMalloc(&b->d_parts, stats_partial_bytes() * world) == cudaSuccess &&
+       cudaMalloc((void**)&b->d_flags_mine, 2 * sizeof(unsigned)) == cudaSuccess &&
+       cudaMalloc((void**)&b->d_flags_all, 2 * sizeof(unsigned) * world) == cudaSuccess &&
+       cudaMallocHost((void**)&b->h_off, sizeof(u64) * (world + 1)) == cudaSuccess &&
+       cudaMallocHost((void**)&b->h_flags_all, 2 * sizeof(unsigned) * world) == cudaSuccess &&
+       cudaEventCreateWithFlags(&b->ev_off, cudaEventDisableTiming) == cudaSuccess &&
+       cudaEventCreate(&b->ev_t0) == cudaSuccess && cudaEventCreate(&b->ev_t1) == cudaSuccess &&
+       cudaMemcpy(b->d_bases, bases.data(), sizeof(u64) * (world + 1), cudaMemcpyHostToDevice) == cudaSuccess;
+  if (!ok) { rmi_shard_build_destroy(b); return fail(RMI_ERR_CUDA, fn + ": device allocation failed"); }
   *out = b;
-  return RMI_OK;
-}
-
-int rmi_shard_top_table(rmi_shard_build* b, void** device_ptr, uint64_t* count, int* elem_bytes) {
-  if (!b || !device_ptr || !count || !elem_bytes) return fail(RMI_ERR_INVALID, "rmi_shard_top_table: null argument");
-  const TopTables& tt = b->tables;
-  if (tt.t32) { *device_ptr = tt.t32; *count = tt.t32_len; *elem_bytes = 4; return RMI_OK; }
-  if (tt.pivots) { *device_ptr = tt.pivots; *count = tt.hist_bins; *elem_bytes = 8; return RMI_OK; }
-  *device_ptr = nullptr; *count = 0; *elem_bytes = 0;
   return RMI_OK;
 }
 
@@ -1861,7 +1903,7 @@ int rmi_shard_phase(rmi_shard_build* b, int phase) {
 
 int rmi_shard_set_halo(rmi_shard_build* b, uint64_t halo_keys) {
   if (!b) return fail(RMI_ERR_INVALID, "rmi_shard_set_halo: null build");
-  if (halo_keys > b->info.halo_capacity) return fail(RMI_ERR_INVALID, "rmi_shard_set_halo: halo exceeds the capacity behind the local keys");
+  if (halo_keys > b->halo_capacity) return fail(RMI_ERR_INVALID, "rmi_shard_set_halo: halo exceeds the capacity behind the local keys");
   b->halo = halo_keys;
   return RMI_OK;
 }
@@ -1879,7 +1921,7 @@ static int shard_result(rmi_shard_build* b, ResultBox* box, unsigned st_all, boo
     delete box;
     return fail(RMI_ERR_PANIC, msg);
   }
-  fill_result(box, *b->top, *b->leaf, b->tables, b->info.n_global, b->N);
+  fill_result(box, *b->top, *b->leaf, b->tables, b->lay.n_global, b->N);
   rmi_result& R = box->pub;
   {   // device time of this rank's phases (collectives between them are not included)
     const int map[RMI_NUM_PHASES] = {0, 0, 1, 1, 2, 3, 0};
@@ -2048,40 +2090,6 @@ void rmi_shard_comm_destroy(rmi_shard_comm* c) {
   delete c;
 }
 
-int rmi_shard_set_partition(rmi_shard_build* b, const uint64_t* bases, int world, int rank) {
-  g_last_error.clear();
-  if (!b || !bases || world < 1 || world > 63 || rank < 0 || rank >= world)
-    return fail(RMI_ERR_INVALID, "rmi_shard_set_partition: bad argument (1 <= world <= 63)");
-  if (bases[rank] != b->info.base || bases[world] != b->info.n_global)
-    return fail(RMI_ERR_INVALID, "rmi_shard_set_partition: bases do not agree with this rank's rmi_shard_info");
-  if (b->world == world && b->rank == rank && b->d_off && b->bases.size() == (size_t)world + 1 &&
-      std::equal(bases, bases + world + 1, b->bases.begin()))
-    return RMI_OK;   // unchanged: nothing to (re)allocate — this is called before every build
-  CUDA_TRY(cudaSetDevice(b->ds->device));
-  b->bases.assign(bases, bases + world + 1);
-  b->world = world; b->rank = rank;
-  b->r_last = 0;
-  for (int r = 0; r < world; ++r) if (bases[r + 1] > bases[r]) b->r_last = r;
-  const size_t pb = stats_partial_bytes();
-  for (void* p : {(void*)b->d_bases, (void*)b->d_off, b->d_parts, (void*)b->d_flags_mine, (void*)b->d_flags_all}) cudaFree(p);
-  if (b->h_off) cudaFreeHost(b->h_off);
-  if (b->h_flags_all) cudaFreeHost(b->h_flags_all);
-  b->d_bases = b->d_off = nullptr; b->d_parts = nullptr; b->d_flags_mine = b->d_flags_all = nullptr; b->h_off = nullptr; b->h_flags_all = nullptr;
-  bool ok = cudaMalloc((void**)&b->d_bases, sizeof(u64) * (world + 1)) == cudaSuccess &&
-            cudaMalloc((void**)&b->d_off, sizeof(u64) * (world + 1)) == cudaSuccess &&
-            cudaMalloc(&b->d_parts, pb * world) == cudaSuccess &&
-            cudaMalloc((void**)&b->d_flags_mine, 2 * sizeof(unsigned)) == cudaSuccess &&
-            cudaMalloc((void**)&b->d_flags_all, 2 * sizeof(unsigned) * world) == cudaSuccess &&
-            cudaMallocHost((void**)&b->h_off, sizeof(u64) * (world + 1)) == cudaSuccess &&
-            cudaMallocHost((void**)&b->h_flags_all, 2 * sizeof(unsigned) * world) == cudaSuccess;
-  for (cudaEvent_t* e : {&b->ev_off, &b->ev_leaf0, &b->ev_leaf1})
-    if (!*e) ok = ok && cudaEventCreateWithFlags(e, cudaEventDisableTiming) == cudaSuccess;
-  for (cudaEvent_t* e : {&b->ev_t0, &b->ev_t1}) if (!*e) ok = ok && cudaEventCreate(e) == cudaSuccess;
-  if (ok) ok = cudaMemcpy(b->d_bases, bases, sizeof(u64) * (world + 1), cudaMemcpyHostToDevice) == cudaSuccess;
-  if (!ok) return fail(RMI_ERR_CUDA, "rmi_shard_set_partition: allocation failed");
-  return RMI_OK;
-}
-
 }  // extern "C"
 
 template <class T>
@@ -2189,7 +2197,7 @@ static int shard_train_typed(rmi_shard_build* b, rmi_shard_comm* c, uint32_t fla
   if (rc == RMI_OK) {
     shard_copy_flags(L, b->d_aux, b->d_flags_mine);
     // statistics of the owned leaves (needs only local results), gathered below
-    leaf_statistics_owned(L, b->info.n_global, N, (const u64*)b->buf.errors, (const u64*)b->buf.counts, b->d_off, rank, W,
+    leaf_statistics_owned(L, b->lay.n_global, N, (const u64*)b->buf.errors, (const u64*)b->buf.counts, b->d_off, rank, W,
                           (char*)b->d_parts + stats_partial_bytes() * rank, b->d_stats);
     if (shared && !co) cudaEventRecord(c->ev_leaf_done, st);
     if (!shared) {
@@ -2290,8 +2298,10 @@ extern "C" {
 int rmi_shard_train(rmi_shard_build* b, rmi_shard_comm* c, uint32_t flags, rmi_result** out) {
   g_last_error.clear();
   if (!b || !c || !out) return fail(RMI_ERR_INVALID, "rmi_shard_train: null argument");
-  if (b->world != c->world || b->rank != c->rank || b->world < 1)
-    return fail(RMI_ERR_INVALID, "rmi_shard_train: call rmi_shard_set_partition with the communicator's world size and rank first");
+  if (c->world != b->world || c->rank != b->rank)
+    return fail(RMI_ERR_INVALID, "rmi_shard_train: the communicator is rank " + std::to_string(c->rank) + " of " +
+                                     std::to_string(c->world) + ", the build rank " + std::to_string(b->rank) + " of " +
+                                     std::to_string(b->world));
   if (!nccl_api().ok) return fail(RMI_ERR_UNSUPPORTED, nccl_api().error);
   CUDA_TRY(cudaSetDevice(b->ds->device));
   return with_key_type(b->ds->key_type, [&](auto k) { return shard_train_typed<decltype(k)>(b, c, flags, out); });
@@ -2309,7 +2319,7 @@ void rmi_shard_build_destroy(rmi_shard_build* b) {
   cudaFree(b->d_bases); cudaFree(b->d_off); cudaFree(b->d_parts); cudaFree(b->d_flags_mine); cudaFree(b->d_flags_all);
   if (b->h_off) cudaFreeHost(b->h_off);
   if (b->h_flags_all) cudaFreeHost(b->h_flags_all);
-  for (cudaEvent_t e : {b->ev_off, b->ev_t0, b->ev_t1, b->ev_leaf0, b->ev_leaf1}) if (e) cudaEventDestroy(e);
+  for (cudaEvent_t e : {b->ev_off, b->ev_t0, b->ev_t1}) if (e) cudaEventDestroy(e);
   delete b;
 }
 
@@ -2452,45 +2462,6 @@ int shard_lookup_one_call(rmi_shard_index* si, rmi_shard_comm* c, const T* d_q, 
 
 }  // namespace
 
-namespace {
-
-// The checks of a gathered ends table that the consumers of range-partitioned keys (rmi_shard_index_create,
-// rmi_shard_eval_create) make before any device work, with RMI_ERR_INVALID and messages naming fn: world and rank in
-// range, ends_all[rank] describing `local`, the non-empty slabs in key order.  *base / *total: this rank's global
-// index of its first key and the keys of all slabs.
-int check_slabs(const std::string& fn, const rmi_dataset* local, const rmi_shard_ends* ends_all, int world, int rank,
-                uint64_t* base, uint64_t* total) {
-  if (world < 1 || world > SHARD_ROUTE_MAX - 1 || rank < 0 || rank >= world)
-    return fail(RMI_ERR_INVALID, fn + ": bad world or rank (0 <= rank < world <= 63)");
-  if (ends_all[rank].n_local != local->n)
-    return fail(RMI_ERR_INVALID, fn + ": ends_all[" + std::to_string(rank) + "] describes " +
-                                     std::to_string(ends_all[rank].n_local) + " keys, the local dataset holds " +
-                                     std::to_string(local->n));
-  *total = 0;
-  for (int p = 0; p < world; ++p) {
-    if (p == rank) *base = *total;
-    *total += ends_all[p].n_local;
-  }
-  // the non-empty slabs must follow each other in key order: no slab's last key above the next one's first
-  int prev = -1;
-  const int bad = with_key_type(local->key_type, [&](auto k) {
-    using T = decltype(k);
-    for (int p = 0; p < world; ++p) {
-      if (!ends_all[p].n_local) continue;
-      if (prev >= 0 && key_from_bits<T>(ends_all[p].first_key_bits) < key_from_bits<T>(ends_all[prev].last_key_bits))
-        return p;
-      prev = p;
-    }
-    return -1;
-  });
-  if (bad >= 0)
-    return fail(RMI_ERR_INVALID, fn + ": the slabs are out of order (rank " + std::to_string(bad) +
-                                     "'s first key is below the last key of rank " + std::to_string(prev) + ")");
-  return RMI_OK;
-}
-
-}  // namespace
-
 extern "C" {
 
 int rmi_shard_index_create(const rmi_result* r, const rmi_dataset* local, const rmi_shard_ends* ends_all, int world,
@@ -2610,16 +2581,6 @@ int rmi_shard_index_last_stats(const rmi_shard_index* si, rmi_shard_lookup_stats
 // ---- rmi_evaluate over a range-partitioned data set (DESIGN.md section 15) -----------------------------------------
 constexpr int SHARD_EVAL_EVENTS = 5;   // upload | boundaries (+ all-reduce) | error pass (+ all-reduce) | statistics
 
-// Where a rank's slab sits among the others, from the gathered ends alone (the rule of sharded.py plan_global_layout):
-// the same on every rank for every field but the rank's own.
-struct SlabLayout {
-  uint64_t base = 0, n_global = 0;
-  int has_prev = 0, is_last = 0, is_first = 0, has_next = 0;
-  uint64_t prev_key_bits = 0, prev_F = 0;   // last key before the slab, first global index of its run
-  uint64_t next_key_bits = 0;               // first key of the next non-empty rank
-  bool no_dups = false;                     // no two keys of the whole data set are equal
-};
-
 struct rmi_shard_eval {
   const rmi_result* r = nullptr;   // the caller's: read at every evaluation
   const rmi_dataset* ds = nullptr;
@@ -2647,45 +2608,6 @@ struct rmi_shard_eval {
 
 namespace {
 
-template <class T> SlabLayout slab_layout(const rmi_shard_ends* e, int world, int rank) {
-  SlabLayout s;
-  std::vector<uint64_t> base(world + 1, 0), last_F(world, 0);
-  for (int g = 0; g < world; ++g) base[g + 1] = base[g] + e[g].n_local;
-  s.base = base[rank];
-  s.n_global = base[world];
-  s.no_dups = true;
-  int prev = -1, first = -1, last = -1;
-  for (int g = 0; g < world; ++g) {
-    if (!e[g].n_local) continue;
-    const bool joins = prev >= 0 && key_from_bits<T>(e[prev].last_key_bits) == key_from_bits<T>(e[g].first_key_bits);
-    // a slab that is one run begun ranks earlier carries that run's first index on
-    last_F[g] = e[g].last_run_start == 0 && joins ? last_F[prev] : base[g] + e[g].last_run_start;
-    if (joins || e[g].no_dups != 1) s.no_dups = false;
-    if (g < rank) { s.has_prev = 1; s.prev_key_bits = e[g].last_key_bits; s.prev_F = last_F[g]; }
-    if (g > rank && !s.has_next) { s.has_next = 1; s.next_key_bits = e[g].first_key_bits; }
-    if (first < 0) first = g;
-    last = g;
-    prev = g;
-  }
-  s.is_first = rank == first;
-  s.is_last = rank == last;
-  return s;
-}
-
-template <class T> Shard<T> eval_shard(const rmi_shard_eval* e) {
-  Shard<T> s;
-  s.base = e->lay.base;
-  s.n_global = e->lay.n_global;
-  s.n_local = e->ds->n;
-  s.n_avail = e->ds->n;
-  s.has_prev = e->lay.has_prev;
-  s.is_last = e->lay.is_last;
-  s.prev_key = key_from_bits<T>(e->lay.prev_key_bits);
-  s.prev_F = e->lay.prev_F;
-  s.no_dups = e->lay.no_dups ? 1 : 0;
-  return s;
-}
-
 uint64_t eval_partial_words(const rmi_shard_eval* e) { return e->lay.no_dups ? e->N : 2 * e->N; }
 
 int eval_bounds(rmi_shard_eval* e, u64* d_S, cudaStream_t st) {
@@ -2705,7 +2627,8 @@ int eval_bounds(rmi_shard_eval* e, u64* d_S, cudaStream_t st) {
   Launch L{st, e->num_sms};
   with_key_type(e->ds->key_type, [&](auto k) {
     using T = decltype(k);
-    shard_bounds_given<T>(L, (const T*)e->ds->d_keys, eval_shard<T>(e), e->top->kind, e->d_top, e->N, d_S, e->d_aux);
+    shard_bounds_given<T>(L, (const T*)e->ds->d_keys, shard_of<T>(e->lay, e->ds->n, e->ds->n), e->top->kind, e->d_top,
+                          e->N, d_S, e->d_aux);
   });
   CUDA_TRY(cudaGetLastError());
   return RMI_OK;
@@ -2718,8 +2641,9 @@ int eval_keys(rmi_shard_eval* e, const u64* d_S, u64* d_part, unsigned* d_status
   Launch L{st, e->num_sms};
   with_key_type(e->ds->key_type, [&](auto k) {
     using T = decltype(k);
-    shard_evaluate_partials<T>(L, (const T*)e->ds->d_keys, eval_shard<T>(e), e->lay.is_first, e->lay.has_next,
-                               key_from_bits<T>(e->lay.next_key_bits), e->leaf->kind, e->N, d_S, e->d_params, d_part);
+    shard_evaluate_partials<T>(L, (const T*)e->ds->d_keys, shard_of<T>(e->lay, e->ds->n, e->ds->n), e->lay.is_first,
+                               e->lay.has_next, key_from_bits<T>(e->lay.next_key_bits), e->leaf->kind, e->N, d_S,
+                               e->d_params, d_part);
   });
   shard_copy_status(L, e->d_aux, d_status);
   CUDA_TRY(cudaGetLastError());
@@ -2789,7 +2713,9 @@ int rmi_shard_eval_create(const rmi_result* r, const rmi_dataset* local, const r
   e->r = r; e->ds = local; e->top = top; e->leaf = leaf;
   e->world = world; e->rank = rank; e->num_sms = di.num_sms;
   e->N = r->branching_factor;
-  e->lay = with_key_type(local->key_type, [&](auto k) { return slab_layout<decltype(k)>(ends_all, world, rank); });
+  e->lay = with_key_type(local->key_type, [&](auto k) {
+    return rmihost::slab_layout<decltype(k)>(ends_all, world, rank, e->N);
+  });
   const uint64_t N = e->N;
   bool ok = cudaStreamCreateWithFlags(&e->own, cudaStreamNonBlocking) == cudaSuccess;
   for (int q = 0; q < SHARD_EVAL_EVENTS; ++q) ok = ok && cudaEventCreate(&e->ev[q]) == cudaSuccess;

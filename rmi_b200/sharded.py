@@ -27,7 +27,6 @@ only its own keys, and one all-reduce MAX of per-leaf maxima combines them.
 from __future__ import annotations
 
 import ctypes as C
-import struct
 
 import numpy as np
 import torch
@@ -54,82 +53,14 @@ class _Ends(C.Structure):
                 ("n_local", C.c_uint64), ("no_dups", C.c_uint64)]
 
 
-class _Info(C.Structure):
-    _fields_ = [("base", C.c_uint64), ("n_global", C.c_uint64), ("has_prev", C.c_int32), ("is_last", C.c_int32),
-                ("prev_key_bits", C.c_uint64), ("prev_F", C.c_uint64), ("first_key_bits", C.c_uint64),
-                ("last_key_bits", C.c_uint64), ("last_F", C.c_uint64), ("halo_capacity", C.c_uint64),
-                ("no_dups", C.c_uint64), ("pivot_x", C.c_double), ("pivot_y", C.c_double)]
-
-
 class _Buffers(C.Structure):
     _fields_ = [("sums", C.c_void_p), ("S", C.c_void_p), ("params", C.c_void_p), ("errors", C.c_void_p),
                 ("counts", C.c_void_p), ("status", C.c_void_p)]
 
 
-def key_bits_to_float(bits: int, key_type: int) -> float:
-    """key.as_float() of a raw key (only used to place the common pivot of the sums)."""
-    if key_type == api.KEY_F64:
-        return struct.unpack("<d", struct.pack("<Q", bits))[0]
-    return float(bits)
-
-
-def key_from_bits(bits: int, key_type: int):
-    """The key a raw key word holds, as a value that compares like the key type: float for f64 keys (so that
-    -0.0 == 0.0, as the kernels and the reference compare keys), int for the unsigned types."""
-    if key_type == api.KEY_F64:
-        return struct.unpack("<d", struct.pack("<Q", bits))[0]
-    if key_type == api.KEY_U32:
-        return bits & 0xFFFFFFFF
-    return bits
-
-
-def plan_global_layout(ends_all: np.ndarray, key_type: int, num_leaves: int) -> list[dict]:
-    """From every rank's (first_key_bits, last_key_bits, last_run_start, n_local) derive, for every
-    rank, its shard description.  Pure function of the gathered table: every rank computes the same.
-
-    prev_key / prev_F: last key before the slab and the first global index of its run of equal keys
-    (the offset FixDupsIter would report, reference models/mod.rs:154-185), which may lie several
-    ranks back when whole slabs consist of one repeated key.  Keys at the cuts are compared by value,
-    not by bits: -0.0 and 0.0 are one run."""
-    world = ends_all.shape[0]
-    n_local = [int(x) for x in ends_all[:, 3]]
-    bases = [0]
-    for g in range(world):
-        bases.append(bases[-1] + n_local[g])
-    n_global = bases[-1]
-    nonempty = [g for g in range(world) if n_local[g] > 0]
-    first_key = {g: key_from_bits(int(ends_all[g, 0]), key_type) for g in nonempty}
-    last_key = {g: key_from_bits(int(ends_all[g, 1]), key_type) for g in nonempty}
-    last_F = {}
-    prev = None
-    for g in nonempty:
-        lrs = int(ends_all[g, 2])
-        if lrs == 0 and prev is not None and last_key[prev] == first_key[g]:
-            last_F[g] = last_F[prev]           # the whole slab is one run that began on an earlier rank
-        else:
-            last_F[g] = bases[g] + lrs
-        prev = g
-    # no two equal keys anywhere: every rank is duplicate-free and no cut separates two equal keys
-    no_dups = ends_all.shape[1] > 4 and all(int(ends_all[g, 4]) == 1 for g in nonempty)
-    for a, b in zip(nonempty, nonempty[1:]):
-        if last_key[a] == first_key[b]:
-            no_dups = False
-    first_bits = int(ends_all[nonempty[0], 0]) if nonempty else 0
-    last_bits = int(ends_all[nonempty[-1], 1]) if nonempty else 0
-    gl_last_F = last_F[nonempty[-1]] if nonempty else 0
-    px = 0.5 * key_bits_to_float(first_bits, key_type) + 0.5 * key_bits_to_float(last_bits, key_type)
-    py = 0.5 * float(num_leaves)
-    out = []
-    for g in range(world):
-        before = [r for r in nonempty if r < g]
-        p = before[-1] if before else None
-        out.append(dict(base=bases[g], n_global=n_global, has_prev=int(p is not None),
-                        is_last=int(bool(nonempty) and g == nonempty[-1]),
-                        prev_key_bits=int(ends_all[p, 1]) if p is not None else 0,
-                        prev_F=last_F[p] if p is not None else 0,
-                        first_key_bits=first_bits, last_key_bits=last_bits, last_F=gl_last_F,
-                        no_dups=int(bool(no_dups)), pivot_x=px, pivot_y=py, bases=bases))
-    return out
+def _ends_array(ends_all: np.ndarray):
+    """gather_ends' table as the C array of rmi_shard_ends that the rmi_shard_*_create calls take."""
+    return (_Ends * len(ends_all))(*[_Ends(*(int(v) for v in row[:5])) for row in ends_all])
 
 
 def plan_halo(bases: list[int], v: list[int], n_global: int) -> list[tuple[int, int, int, int]]:
@@ -244,8 +175,8 @@ class CudaShardEngine:
         self.lib = api.load_library()
         L = self.lib
         L.rmi_shard_ends_get.argtypes = [C.c_void_p, C.POINTER(_Ends)]
-        L.rmi_shard_build_create.argtypes = [C.c_void_p, C.POINTER(_Info), C.c_char_p, C.c_uint64, C.POINTER(_Buffers),
-                                             C.c_void_p, C.POINTER(C.c_void_p)]
+        L.rmi_shard_build_create.argtypes = [C.c_void_p, C.POINTER(_Ends), C.c_int, C.c_int, C.c_char_p, C.c_uint64,
+                                             C.c_uint64, C.POINTER(_Buffers), C.c_void_p, C.POINTER(C.c_void_p)]
         L.rmi_shard_phase.argtypes = [C.c_void_p, C.c_int]
         L.rmi_shard_set_halo.argtypes = [C.c_void_p, C.c_uint64]
         L.rmi_shard_finish.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.POINTER(api._Result))]
@@ -253,7 +184,6 @@ class CudaShardEngine:
         L.rmi_shard_comm_unique_id.argtypes = [C.c_void_p]
         L.rmi_shard_comm_create.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p)]
         L.rmi_shard_comm_destroy.argtypes = [C.c_void_p]
-        L.rmi_shard_set_partition.argtypes = [C.c_void_p, C.POINTER(C.c_uint64), C.c_int, C.c_int]
         L.rmi_shard_train.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(C.POINTER(api._Result))]
         self.device = data.buf.device
         self.ds = api.RMITrainingData.from_device(data.buf.data_ptr(), data.n_local, data.key_type,
@@ -265,21 +195,18 @@ class CudaShardEngine:
         api._check(self.lib.rmi_shard_ends_get(self.ds._h, C.byref(e)))
         return int(e.first_key_bits), int(e.last_key_bits), int(e.last_run_start), int(e.n_local), int(e.no_dups)
 
-    def begin(self, info: dict, spec: str, num_leaves: int, bufs: dict):
+    def begin(self, ends_all: np.ndarray, world: int, rank: int, spec: str, num_leaves: int, bufs: dict):
         key = (spec, num_leaves, tuple(bufs[k].data_ptr() for k in sorted(bufs)))
         if self._build is not None and getattr(self, "_build_key", None) == key:
             return      # same spec / buffers: the build object (scratch, events) is reused
         self.end()
         self._build_key = key
-        ci = _Info(base=info["base"], n_global=info["n_global"], has_prev=info["has_prev"], is_last=info["is_last"],
-                   prev_key_bits=info["prev_key_bits"], prev_F=info["prev_F"], first_key_bits=info["first_key_bits"],
-                   last_key_bits=info["last_key_bits"], last_F=info["last_F"], halo_capacity=self.data.halo_capacity,
-                   no_dups=info.get("no_dups", 0), pivot_x=info["pivot_x"], pivot_y=info["pivot_y"])
         cb = _Buffers(*(bufs[k].data_ptr() for k in ("sums", "S", "params", "errors", "counts", "status")))
         h = C.c_void_p()
         stream = torch.cuda.current_stream(self.device).cuda_stream
-        api._check(self.lib.rmi_shard_build_create(self.ds._h, C.byref(ci), spec.encode(), num_leaves, C.byref(cb),
-                                                   C.c_void_p(stream), C.byref(h)))
+        api._check(self.lib.rmi_shard_build_create(self.ds._h, _ends_array(ends_all), world, rank, spec.encode(),
+                                                   num_leaves, self.data.halo_capacity, C.byref(cb), C.c_void_p(stream),
+                                                   C.byref(h)))
         self._build = h
         self._spec = spec
 
@@ -295,10 +222,6 @@ class CudaShardEngine:
 
     def local_view(self, offset: int, count: int) -> torch.Tensor:
         return self.data.buf[offset: offset + count]
-
-    def set_partition(self, bases: list[int], world: int, rank: int):
-        arr = (C.c_uint64 * (world + 1))(*bases)
-        api._check(self.lib.rmi_shard_set_partition(self._build, arr, world, rank))
 
     def train(self, comm, flags: int = 0):
         """The whole build in one library call: phases and NCCL collectives on the build's stream (rmi_shard_train)."""
@@ -412,12 +335,11 @@ def train_sharded(data, model_spec: str, num_leaves: int, flags: int = 0, group=
     N = int(num_leaves)
 
     # 1. what every rank's slab looks like at its ends (cached on the data object: the data is immutable)
-    layout = getattr(data, "_layout", None)
-    if layout is None or layout[0] != N:
-        layout = (N, plan_global_layout(gather_ends(data, eng, group), data.key_type, N))
-        data._layout = layout
-    info = layout[1][rank]
-    bases, n_global = info["bases"], info["n_global"]
+    ends_all = gather_ends(data, eng, group)
+    bases = [0]
+    for n_local in ends_all[:, 3]:
+        bases.append(bases[-1] + int(n_local))
+    n_global = bases[-1]
 
     bufs = getattr(data, "_bufs", None)
     if bufs is None or bufs["S"].numel() != N + 1 or bufs["params"].numel() != N * ppm:
@@ -430,7 +352,7 @@ def train_sharded(data, model_spec: str, num_leaves: int, flags: int = 0, group=
                     counts=rec[N * (ppm + 1):],
                     status=torch.zeros(1, dtype=torch.int32, device=dev), records=rec)
         data._bufs = bufs
-    eng.begin(info, model_spec, N, bufs)
+    eng.begin(ends_all, world, rank, model_spec, N, bufs)
 
     comm = None
     if native is not False and isinstance(eng, CudaShardEngine):
@@ -447,7 +369,6 @@ def train_sharded(data, model_spec: str, num_leaves: int, flags: int = 0, group=
             else:
                 data._halo_have = 0
         eng.set_halo(data._halo_have or 0)
-        eng.set_partition(bases, world, rank)
         try:
             return eng.train(comm, int(flags) | (api.FLAG_LEAF_COUNTS if counts else 0))
         except api.RMIPanic as e:
@@ -648,9 +569,9 @@ class CudaShardIndex:
         self.world = world
         self._ds = eng.ds            # the slab the index searches: kept alive with it
         self._trained = trained
-        ends = (_Ends * world)(*[_Ends(*(int(v) for v in row[:5])) for row in ends_all])
         self._h = C.c_void_p()
-        api._check(L.rmi_shard_index_create(api._result_ptr(trained), eng.ds._h, ends, world, rank, C.byref(self._h)))
+        api._check(L.rmi_shard_index_create(api._result_ptr(trained), eng.ds._h, _ends_array(ends_all), world, rank,
+                                            C.byref(self._h)))
 
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream or None)
@@ -728,9 +649,9 @@ class CudaShardEval:
         self._trained = trained
         self._spec = trained.models
         self.N = int(trained.branching_factor)
-        ends = (_Ends * world)(*[_Ends(*(int(v) for v in row[:5])) for row in ends_all])
         self._h = C.c_void_p()
-        api._check(L.rmi_shard_eval_create(api._result_ptr(trained), eng.ds._h, ends, world, rank, C.byref(self._h)))
+        api._check(L.rmi_shard_eval_create(api._result_ptr(trained), eng.ds._h, _ends_array(ends_all), world, rank,
+                                           C.byref(self._h)))
         self.partial_words = int(L.rmi_shard_eval_partial_words(self._h))
 
     def _stream(self):

@@ -5,13 +5,16 @@ the oracle's per-model constructors, following the *global-index formulation* th
 use (DESIGN.md section 4): leaf j owns [S[j], S[j+1]), its training vector is a contiguous
 index range, offsets are duplicate-fixed global indices.  Running the real orchestrator
 (train_sharded) over this engine with world_size >= 2 therefore checks (a) the host logic —
-layout planning, the collectives, halo planning and exchange, ownership — and (b) that the
-formulation reproduces the oracle's streaming restatement of the reference bit for bit.
+the collectives, halo planning and exchange, ownership — and (b) that the formulation
+reproduces the oracle's streaming restatement of the reference bit for bit.  The stand-in
+derives each rank's slab layout with plan_global_layout below, a second statement of the
+library's rule (host/slab_layout.hpp) that tests/test_sharded_gloo.py holds the two to.
 TEST INFRASTRUCTURE: never imported by the product.
 """
 from __future__ import annotations
 
 import math
+import struct
 from fractions import Fraction
 
 import numpy as np
@@ -75,6 +78,72 @@ def _fma_floor_u64(beta: float, x: float, alpha: float) -> int:
     return min(int(math.floor(v)), U64)
 
 
+def key_bits_to_float(bits: int, key_type: int) -> float:
+    """key.as_float() of a raw key (only used to place the common pivot of the sums)."""
+    if key_type == api.KEY_F64:
+        return struct.unpack("<d", struct.pack("<Q", bits))[0]
+    return float(bits)
+
+
+def key_from_bits(bits: int, key_type: int):
+    """The key a raw key word holds, as a value that compares like the key type: float for f64 keys (so that
+    -0.0 == 0.0, as the kernels and the reference compare keys), int for the unsigned types."""
+    if key_type == api.KEY_F64:
+        return struct.unpack("<d", struct.pack("<Q", bits))[0]
+    if key_type == api.KEY_U32:
+        return bits & 0xFFFFFFFF
+    return bits
+
+
+def plan_global_layout(ends_all: np.ndarray, key_type: int, num_leaves: int) -> list[dict]:
+    """From every rank's (first_key_bits, last_key_bits, last_run_start, n_local, no_dups) derive, for every
+    rank, its shard description.  Pure function of the gathered table: every rank computes the same.
+
+    prev_key / prev_F: last key before the slab and the first global index of its run of equal keys
+    (the offset FixDupsIter would report, reference models/mod.rs:154-185), which may lie several
+    ranks back when whole slabs consist of one repeated key.  Keys at the cuts are compared by value,
+    not by bits: -0.0 and 0.0 are one run."""
+    world = ends_all.shape[0]
+    n_local = [int(x) for x in ends_all[:, 3]]
+    bases = [0]
+    for g in range(world):
+        bases.append(bases[-1] + n_local[g])
+    n_global = bases[-1]
+    nonempty = [g for g in range(world) if n_local[g] > 0]
+    first_key = {g: key_from_bits(int(ends_all[g, 0]), key_type) for g in nonempty}
+    last_key = {g: key_from_bits(int(ends_all[g, 1]), key_type) for g in nonempty}
+    last_F = {}
+    prev = None
+    for g in nonempty:
+        lrs = int(ends_all[g, 2])
+        if lrs == 0 and prev is not None and last_key[prev] == first_key[g]:
+            last_F[g] = last_F[prev]           # the whole slab is one run that began on an earlier rank
+        else:
+            last_F[g] = bases[g] + lrs
+        prev = g
+    # no two equal keys anywhere: every rank is duplicate-free and no cut separates two equal keys
+    no_dups = all(int(ends_all[g, 4]) == 1 for g in nonempty)
+    for a, b in zip(nonempty, nonempty[1:]):
+        if last_key[a] == first_key[b]:
+            no_dups = False
+    first_bits = int(ends_all[nonempty[0], 0]) if nonempty else 0
+    last_bits = int(ends_all[nonempty[-1], 1]) if nonempty else 0
+    gl_last_F = last_F[nonempty[-1]] if nonempty else 0
+    px = 0.5 * key_bits_to_float(first_bits, key_type) + 0.5 * key_bits_to_float(last_bits, key_type)
+    py = 0.5 * float(num_leaves)
+    out = []
+    for g in range(world):
+        before = [r for r in nonempty if r < g]
+        p = before[-1] if before else None
+        out.append(dict(base=bases[g], n_global=n_global, has_prev=int(p is not None),
+                        is_last=int(bool(nonempty) and g == nonempty[-1]),
+                        prev_key_bits=int(ends_all[p, 1]) if p is not None else 0,
+                        prev_F=last_F[p] if p is not None else 0,
+                        first_key_bits=first_bits, last_key_bits=last_bits, last_F=gl_last_F,
+                        no_dups=int(bool(no_dups)), pivot_x=px, pivot_y=py))
+    return out
+
+
 class NumpyShardEngine:
     device = torch.device("cpu")
 
@@ -100,7 +169,8 @@ class NumpyShardEngine:
         count = self.n_local + self.halo if count is None else count
         return self.buf[:count].numpy().view(np.uint64)
 
-    def begin(self, info, spec, N, bufs):
+    def begin(self, ends_all, world, rank, spec, N, bufs):
+        info = plan_global_layout(ends_all, self.key_type, N)[rank]
         self.info, self.N, self.bufs = info, int(N), bufs
         self.top_name, self.leaf_name = spec.split(",")
         self.n = info["n_global"]

@@ -65,13 +65,16 @@ def shard_create(rmi, data, spec, bf):
     """rmi_shard_build_create through ctypes: one rank holding the whole data set."""
     from rmi_b200 import sharded
     lib = rmi.load_library()
-    lib.rmi_shard_build_create.argtypes = [C.c_void_p, C.POINTER(sharded._Info), C.c_char_p, C.c_uint64,
-                                           C.POINTER(sharded._Buffers), C.c_void_p, C.POINTER(C.c_void_p)]
+    lib.rmi_shard_build_create.argtypes = [C.c_void_p, C.POINTER(sharded._Ends), C.c_int, C.c_int, C.c_char_p,
+                                           C.c_uint64, C.c_uint64, C.POINTER(sharded._Buffers), C.c_void_p,
+                                           C.POINTER(C.c_void_p)]
     lib.rmi_shard_build_destroy.argtypes = [C.c_void_p]
-    info = sharded._Info(base=0, n_global=len(data), has_prev=0, is_last=1)
+    lib.rmi_shard_ends_get.argtypes = [C.c_void_p, C.POINTER(sharded._Ends)]
+    ends = sharded._Ends()
+    rmi.api._check(lib.rmi_shard_ends_get(data._h, C.byref(ends)))
     h = C.c_void_p()
-    rc = lib.rmi_shard_build_create(data._h, C.byref(info), spec.encode(), bf, C.byref(sharded._Buffers()), None,
-                                    C.byref(h))
+    rc = lib.rmi_shard_build_create(data._h, C.byref(ends), 1, 0, spec.encode(), bf, 0, C.byref(sharded._Buffers()),
+                                    None, C.byref(h))
     if rc == 0:
         lib.rmi_shard_build_destroy(h)
     rmi.api._check(rc)

@@ -16,7 +16,7 @@ import torch.multiprocessing as mp
 
 from rmi_b200 import api
 from tests import datasets, evaluate_oracle
-from tests.shard_engine_numpy import U64, NumpyShardEngine, _fma_floor_u64
+from tests.shard_engine_numpy import U64, NumpyShardEngine, _fma_floor_u64, plan_global_layout
 
 N_LEAVES = 64
 ST_NON_MONOTONE = 2
@@ -43,11 +43,10 @@ class _NumpyEval:
     """The phases of rmi_shard_eval_* on one rank's slab, in plain Python."""
 
     def __init__(self, keys, tables, ends_all, world, rank):
-        from rmi_b200 import sharded
         self.slab = [int(k) for k in keys]
         (self.alpha, self.beta), self.params = tables
         self.N = len(self.params)
-        info = sharded.plan_global_layout(ends_all, api.KEY_U64, self.N)[rank]
+        info = plan_global_layout(ends_all, api.KEY_U64, self.N)[rank]
         self.info, self.base, self.n = info, info["base"], info["n_global"]
         nonempty = [r for r in range(world) if int(ends_all[r, 3]) > 0]
         later = [r for r in nonempty if r > rank]

@@ -1,9 +1,12 @@
-"""The range-partitioned build's host logic (rmi_b200/sharded.py: layout planning, the three
-collectives, halo planning + exchange, ownership) under torch.distributed/gloo with
-world_size 2 and 3 on CPU.  The arithmetic engine is tests/shard_engine_numpy.py; the result
-on every rank must equal the oracle's single-process build of the concatenated keys."""
+"""The range-partitioned build's host logic (rmi_b200/sharded.py: the three collectives, halo
+planning + exchange, ownership) under torch.distributed/gloo with world_size 2 and 3 on CPU.
+The arithmetic engine is tests/shard_engine_numpy.py; the result on every rank must equal the
+oracle's single-process build of the concatenated keys.  The slab layout rule is checked here
+in both its statements: the library's (host/slab_layout.hpp, through tests/cxx/slab_layout_tool.cpp)
+and the stand-in engine's."""
 import os
 import socket
+import subprocess
 
 import numpy as np
 import pytest
@@ -11,7 +14,10 @@ import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
+from rmi_b200 import api
 from tests import datasets, parity
+from tests.shard_engine_numpy import plan_global_layout
+from tests.test_codegen import ROOT
 
 
 def _free_port():
@@ -135,25 +141,54 @@ def test_halo_grows_when_a_leaf_reaches_past_the_prefetched_keys(oracle):
     assert not [r for r in results if r[1] != "ok"], results
 
 
-def test_layout_planner_handles_runs_spanning_ranks():
-    from rmi_b200 import sharded
+@pytest.fixture(scope="module")
+def layout_tool(tmp_path_factory):
+    exe = str(tmp_path_factory.mktemp("slab_layout") / "slab_layout_tool")
+    subprocess.run(["g++", "-std=c++17", "-O1", "-Wall", os.path.join(ROOT, "tests", "cxx", "slab_layout_tool.cpp"), "-o",
+                    exe], check=True)
+    return exe
+
+
+_KEY_NAME = {api.KEY_U64: "u64", api.KEY_U32: "u32", api.KEY_F64: "f64"}
+
+
+def tool_layouts(tool, tables):
+    """The library's rule (host/slab_layout.hpp) on every (ends, key_type, N) of `tables`: per table, every rank's
+    layout as a dict."""
+    text = "".join(f"{_KEY_NAME[kt]} {N} {len(e)}\n" + "".join(" ".join(str(int(v)) for v in row) + "\n" for row in e)
+                   for e, kt, N in tables)
+    r = subprocess.run([tool], input=text, capture_output=True, text=True, check=True)
+    rows = [dict(kv.split("=") for kv in ln.split()) for ln in r.stdout.splitlines()]
+    assert len(rows) == sum(len(e) for e, _, _ in tables)
+    out = []
+    for e, _, _ in tables:
+        out.append([{k: float.fromhex(v) if k.startswith("pivot") else int(v) for k, v in d.items()} for d in rows[:len(e)]])
+        rows = rows[len(e):]
+    return out
+
+
+def both_rules(tool, ends, key_type, N):
+    """Every rank's layout of one ends table by the library's rule and by the numpy stand-in's."""
+    return [tool_layouts(tool, [(ends, key_type, N)])[0], plan_global_layout(ends, key_type, N)]
+
+
+def test_layout_planner_handles_runs_spanning_ranks(layout_tool):
     # rank 1 consists of one repeated key that began on rank 0 and continues into rank 2
-    ends = np.array([[5, 9, 3, 10], [9, 9, 0, 4], [9, 12, 2, 6]], dtype=np.uint64)
-    lay = sharded.plan_global_layout(ends, 0, 64)
-    assert [d["base"] for d in lay] == [0, 10, 14]
-    assert lay[1]["prev_F"] == 3 and lay[2]["prev_F"] == 3 and lay[2]["prev_key_bits"] == 9
-    assert lay[0]["last_F"] == 16 and lay[2]["is_last"] == 1 and lay[0]["has_prev"] == 0
+    ends = np.array([[5, 9, 3, 10, 0], [9, 9, 0, 4, 0], [9, 12, 2, 6, 0]], dtype=np.uint64)
+    for lay in both_rules(layout_tool, ends, api.KEY_U64, 64):
+        assert [d["base"] for d in lay] == [0, 10, 14]
+        assert lay[1]["prev_F"] == 3 and lay[2]["prev_F"] == 3 and lay[2]["prev_key_bits"] == 9
+        assert lay[0]["last_F"] == 16 and lay[2]["is_last"] == 1 and lay[0]["has_prev"] == 0
     # empty rank in the middle
-    ends = np.array([[1, 4, 2, 3], [0, 0, 0, 0], [7, 8, 1, 2]], dtype=np.uint64)
-    lay = sharded.plan_global_layout(ends, 0, 8)
-    assert lay[2]["prev_key_bits"] == 4 and lay[2]["prev_F"] == 2 and lay[1]["has_prev"] == 1
-    assert lay[2]["base"] == 3 and lay[2]["n_global"] == 5
+    ends = np.array([[1, 4, 2, 3, 0], [0, 0, 0, 0, 0], [7, 8, 1, 2, 0]], dtype=np.uint64)
+    for lay in both_rules(layout_tool, ends, api.KEY_U64, 8):
+        assert lay[2]["prev_key_bits"] == 4 and lay[2]["prev_F"] == 2 and lay[1]["has_prev"] == 1
+        assert lay[2]["base"] == 3 and lay[2]["n_global"] == 5
 
 
-def test_layout_planner_compares_f64_keys_at_the_cuts_by_value():
+def test_layout_planner_compares_f64_keys_at_the_cuts_by_value(layout_tool):
     """-0.0 == 0.0: a cut between them separates two equal keys (the data set has duplicates, so the leaf kernel
     must track runs) and a slab of zeros continues the run of a -0.0 before it, whatever the zeros' signs."""
-    from rmi_b200 import api, sharded
 
     def b(x):
         return int(np.array([x], dtype=np.float64).view(np.uint64)[0])
@@ -162,49 +197,83 @@ def test_layout_planner_compares_f64_keys_at_the_cuts_by_value():
         return np.array([[b(f), b(l), s, n, d] for f, l, s, n, d in rows], dtype=np.uint64)
 
     def planned(*rows):
-        return sharded.plan_global_layout(ends(*rows), api.KEY_F64, 16)
+        return both_rules(layout_tool, ends(*rows), api.KEY_F64, 16)
 
     # [-1.0, -0.5, -0.0] | [0.0, 0.5, 1.0] and [-1.0, -0.5, 0.0] | [-0.0, 0.5, 1.0]: no equal keys inside a slab
     for z0, z1 in ((-0.0, 0.0), (0.0, -0.0)):
-        lay = planned((-1.0, z0, 2, 3, 1), (z1, 1.0, 2, 3, 1))
-        assert lay[0]["no_dups"] == 0
-        assert lay[1]["has_prev"] == 1 and lay[1]["prev_key_bits"] == b(z0) and lay[1]["prev_F"] == 2
-        assert lay[0]["last_F"] == 5
+        for lay in planned((-1.0, z0, 2, 3, 1), (z1, 1.0, 2, 3, 1)):
+            assert lay[0]["no_dups"] == 0
+            assert lay[1]["has_prev"] == 1 and lay[1]["prev_key_bits"] == b(z0) and lay[1]["prev_F"] == 2
+            assert lay[0]["last_F"] == 5
     # [-1.0, -0.5, -0.0] | [0.0, -0.0, 0.0] | [2.0, 3.0]: the middle slab is one run that began at global index 2
-    lay = planned((-1.0, -0.0, 2, 3, 1), (0.0, 0.0, 0, 3, 0), (2.0, 3.0, 1, 2, 1))
-    assert [d["base"] for d in lay] == [0, 3, 6] and lay[0]["no_dups"] == 0
-    assert lay[1]["prev_F"] == 2 and lay[1]["prev_key_bits"] == b(-0.0)
-    assert lay[2]["prev_F"] == 2 and lay[2]["prev_key_bits"] == b(0.0)
-    assert lay[0]["last_F"] == 7
+    for lay in planned((-1.0, -0.0, 2, 3, 1), (0.0, 0.0, 0, 3, 0), (2.0, 3.0, 1, 2, 1)):
+        assert [d["base"] for d in lay] == [0, 3, 6] and lay[0]["no_dups"] == 0
+        assert lay[1]["prev_F"] == 2 and lay[1]["prev_key_bits"] == b(-0.0)
+        assert lay[2]["prev_F"] == 2 and lay[2]["prev_key_bits"] == b(0.0)
+        assert lay[0]["last_F"] == 7
     # the last slab is the zeros: the data set's last run starts on rank 0
-    lay = planned((-1.0, -0.0, 1, 2, 1), (0.0, -0.0, 0, 4, 0))
-    assert lay[1]["prev_F"] == 1 and lay[0]["last_F"] == 1 and lay[0]["no_dups"] == 0
+    for lay in planned((-1.0, -0.0, 1, 2, 1), (0.0, -0.0, 0, 4, 0)):
+        assert lay[1]["prev_F"] == 1 and lay[0]["last_F"] == 1 and lay[0]["no_dups"] == 0
     # [-1.0, -0.0] | (empty) | [0.0, 1.0]: the empty slab does not separate the two zeros
-    lay = planned((-1.0, -0.0, 1, 2, 1), (0.0, 0.0, 0, 0, 1), (0.0, 1.0, 1, 2, 1))
-    assert lay[0]["no_dups"] == 0 and [d["base"] for d in lay] == [0, 2, 2]
-    assert lay[1]["has_prev"] == 1 and lay[1]["prev_F"] == 1 and lay[1]["prev_key_bits"] == b(-0.0)
-    assert lay[2]["prev_F"] == 1 and lay[2]["prev_key_bits"] == b(-0.0) and lay[0]["last_F"] == 3
+    for lay in planned((-1.0, -0.0, 1, 2, 1), (0.0, 0.0, 0, 0, 1), (0.0, 1.0, 1, 2, 1)):
+        assert lay[0]["no_dups"] == 0 and [d["base"] for d in lay] == [0, 2, 2]
+        assert lay[1]["has_prev"] == 1 and lay[1]["prev_F"] == 1 and lay[1]["prev_key_bits"] == b(-0.0)
+        assert lay[2]["prev_F"] == 1 and lay[2]["prev_key_bits"] == b(-0.0) and lay[0]["last_F"] == 3
     # [-1.0, -0.0] | (empty) | [0.0, -0.0] | [1.0]: a slab of zeros continues a run across the empty slab
-    lay = planned((-1.0, -0.0, 1, 2, 1), (0.0, 0.0, 0, 0, 1), (0.0, -0.0, 0, 2, 0), (1.0, 1.0, 0, 1, 1))
-    assert lay[3]["prev_F"] == 1 and lay[3]["prev_key_bits"] == b(-0.0) and lay[0]["last_F"] == 4
+    for lay in planned((-1.0, -0.0, 1, 2, 1), (0.0, 0.0, 0, 0, 1), (0.0, -0.0, 0, 2, 0), (1.0, 1.0, 0, 1, 1)):
+        assert lay[3]["prev_F"] == 1 and lay[3]["prev_key_bits"] == b(-0.0) and lay[0]["last_F"] == 4
     # distinct keys whose bits differ only in the sign stay distinct: [-1.0, -0.5] | [0.5, 1.0]
-    lay = planned((-1.0, -0.5, 1, 2, 1), (0.5, 1.0, 1, 2, 1))
-    assert lay[0]["no_dups"] == 1 and lay[1]["prev_F"] == 1 and lay[0]["last_F"] == 3
+    for lay in planned((-1.0, -0.5, 1, 2, 1), (0.5, 1.0, 1, 2, 1)):
+        assert lay[0]["no_dups"] == 1 and lay[1]["prev_F"] == 1 and lay[0]["last_F"] == 3
 
 
-def test_layout_planner_u32_keys_compare_as_32_bit_values():
-    from rmi_b200 import api, sharded
+def test_layout_planner_u32_keys_compare_as_32_bit_values(layout_tool):
     # rank 1 is one run of 0xFFFFFFF0 (negative in int32 storage) that began on rank 0
     ends = np.array([[5, 0xFFFFFFF0, 3, 10, 1], [0xFFFFFFF0, 0xFFFFFFF0, 0, 4, 0], [0xFFFFFFF0, 0xFFFFFFFF, 2, 6, 0]],
                     dtype=np.uint64)
-    lay = sharded.plan_global_layout(ends, api.KEY_U32, 64)
-    assert lay[1]["prev_F"] == 3 and lay[2]["prev_F"] == 3 and lay[2]["prev_key_bits"] == 0xFFFFFFF0
-    assert lay[0]["last_F"] == 16 and lay[0]["no_dups"] == 0
+    for lay in both_rules(layout_tool, ends, api.KEY_U32, 64):
+        assert lay[1]["prev_F"] == 3 and lay[2]["prev_F"] == 3 and lay[2]["prev_key_bits"] == 0xFFFFFFF0
+        assert lay[0]["last_F"] == 16 and lay[0]["no_dups"] == 0
     ends[:, 4] = 1
     ends[1] = [0xFFFFFFF1, 0xFFFFFFF2, 1, 2, 1]
     ends[2] = [0xFFFFFFF3, 0xFFFFFFFF, 5, 6, 1]
-    lay = sharded.plan_global_layout(ends, api.KEY_U32, 64)
-    assert lay[0]["no_dups"] == 1 and lay[2]["prev_F"] == 11 and lay[0]["last_F"] == 17
+    for lay in both_rules(layout_tool, ends, api.KEY_U32, 64):
+        assert lay[0]["no_dups"] == 1 and lay[2]["prev_F"] == 11 and lay[0]["last_F"] == 17
+
+
+def _random_ends(rng, key_type):
+    """The ends table rmi_shard_ends_get would give for a small sorted key set with long runs, cut at random places
+    (empty slabs included); a slab's no_dups may under-report, as it does for slabs of fewer than two keys."""
+    pool = {api.KEY_U64: np.array([0, 1, 5, 1 << 40, (1 << 63) + 3, (1 << 64) - 1], dtype=np.uint64),
+            api.KEY_U32: np.array([0, 1, 7, 0x7FFFFFFF, 0x80000000, 0xFFFFFFF0, 0xFFFFFFFF], dtype=np.uint32),
+            api.KEY_F64: np.array([-2.0, -1.0, -0.0, 0.0, 0.5, 1.0, 3.0])}[key_type]
+    keys = np.sort(rng.choice(pool, int(rng.integers(1, 14))), kind="stable")
+    bits = keys.view(np.uint64) if key_type == api.KEY_F64 else keys.astype(np.uint64)
+    world = int(rng.integers(1, 6))
+    cuts = [0] + sorted(int(c) for c in rng.integers(0, keys.size + 1, world - 1)) + [keys.size]
+    rows = []
+    for lo, hi in zip(cuts, cuts[1:]):
+        if hi == lo:
+            rows.append([0, 0, 0, 0, int(rng.integers(0, 2))])
+            continue
+        slab = keys[lo:hi]
+        unique = np.unique(slab).size == slab.size
+        rows.append([int(bits[lo]), int(bits[hi - 1]), int(np.searchsorted(slab, slab[-1], "left")), hi - lo,
+                     int(unique and rng.random() < 0.8)])
+    return np.array(rows, dtype=np.uint64)
+
+
+def test_layout_rules_of_the_library_and_the_stand_in_agree(layout_tool):
+    """The numpy stand-in carries its own copy of the layout rule: on many small random ends tables (runs across cuts,
+    empty slabs, -0.0 next to 0.0, u32 keys with the top bit set) it must give every rank the layout the library does."""
+    rng = np.random.default_rng(2024)
+    tables = [(_random_ends(rng, kt), kt, int(rng.integers(1, 1000))) for kt in _KEY_NAME for _ in range(300)]
+    for (ends, kt, N), got in zip(tables, tool_layouts(layout_tool, tables)):
+        want = plan_global_layout(ends, kt, N)
+        for rank, (g, w) in enumerate(zip(got, want)):
+            for k, v in w.items():
+                same = g[k].hex() == v.hex() if isinstance(v, float) else g[k] == v
+                assert same, (kt, N, ends.tolist(), rank, k, g[k], v)
 
 
 def test_halo_planner():
