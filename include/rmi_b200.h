@@ -446,6 +446,53 @@ int rmi_cache_fix_device(const rmi_dataset* ds, uint64_t line_size, rmi_spline_p
                          uint64_t* out_count, rmi_cache_fix_stats* stats);
 void rmi_spline_free(rmi_spline_point* points);
 
+/* ---- rmi_cache_fix_device over a range-partitioned data set (DESIGN.md section 16: method, measured cost) ---------
+ * Every rank holds its slab `local` (u64 keys) and, behind it in the same device array, the first halo_keys keys of
+ * the following ranks.  The knots of all ranks, in rank order, are rmi_cache_fix_device(concatenation of the slabs),
+ * knot for knot.  The point stream is section 12's with global indices: point (global key index g, sub) has pid
+ * 2g + sub (sub 0: (key - 1, g), sub 1: (key, g), both at the first index of a run of equal keys only).  A rank's
+ * chain starts at an ENTRY pid E: the first point at or after E.  Its EXIT X(E) is the first knot of that chain at or
+ * past 2 x (the next rank's base), RMI_SHARD_CACHE_FIX_PID_END when the last segment stays open to the end of the
+ * data.  An entry at or past the slab's end, or an empty slab, passes straight through: no knots, X = E, no key read.
+ *
+ * rmi_shard_cache_fix_create refuses, before any device work, in this order: a null argument (RMI_ERR_INVALID); the
+ * ends-table checks of rmi_shard_index_create (world / rank, ends_all[rank] not describing local, slabs out of key
+ * order); a dataset that is not u64 and a halo that reaches past the end of the data (RMI_ERR_INVALID); then
+ * rmi_cache_fix_device's panics with its messages, decided from ends_all so that every rank fails alike: fewer keys in
+ * all slabs than the line size, line size 0, a local dataset that is not sorted, a first key of 0 (RMI_ERR_PANIC).
+ * local must outlive the object; its device scratch is about 24 words per 256 local keys.
+ *
+ * Joining the ranks (the caller issues the collectives; rmi_b200/sharded.py cache_fix_sharded does it with
+ * torch.distributed):
+ *   1. every rank scans with E = 2 x its base (its own first point); rank 0's entry is the true first knot;
+ *   2. all-gather every rank's (E, X, status);
+ *   3. every rank r >= 1 whose E differs from X of rank r - 1 scans again with E = that X;
+ *   4. repeat 2 and 3 until no entry changes (at most world - 1 more rounds: after round k, ranks 0..k have true
+ *      entries);
+ *   5. every rank emits its num_knots knots; the counts give the offsets of a gather.
+ * scan runs on cuda_stream and waits for it (its result is read on the host).  The first scan runs the speculation
+ * and every chunk's stitch; a later one re-runs only the stitch of the slab's first chunk and the resolve.  Status
+ * RMI_SHARD_CACHE_FIX_HALO_TOO_SMALL: the chain needs keys past the halo, which does not reach the end of the data;
+ * reach is the global index of the first key it could not read.  Nothing may be emitted then: build a new object
+ * over a larger halo and start again.  emit writes the knots of the last scan's chain whose pids lie in the slab,
+ * then, on the last non-empty rank, finish()'s point (the last key and the global index of its run's first key), to
+ * d_out (device memory, num_knots entries), enqueued on cuda_stream without a host synchronisation. */
+#define RMI_SHARD_CACHE_FIX_PID_END 0xFFFFFFFFFFFFFFFFull
+#define RMI_SHARD_CACHE_FIX_HALO_TOO_SMALL 1u
+typedef struct {
+  uint64_t exit_pid;    /* X(E) */
+  uint64_t num_knots;   /* knots emit writes for this entry, finish()'s point included */
+  uint64_t reach;       /* with RMI_SHARD_CACHE_FIX_HALO_TOO_SMALL: the global index of the first key the walk lacked */
+  uint32_t status;      /* 0 or RMI_SHARD_CACHE_FIX_HALO_TOO_SMALL */
+  uint32_t _pad;
+} rmi_shard_cache_fix_scan_result;
+typedef struct rmi_shard_cache_fix rmi_shard_cache_fix;
+int rmi_shard_cache_fix_create(const rmi_dataset* local, const rmi_shard_ends* ends_all, int world, int rank,
+                               uint64_t line_size, uint64_t halo_keys, void* cuda_stream, rmi_shard_cache_fix** out);
+int rmi_shard_cache_fix_scan(rmi_shard_cache_fix* cf, uint64_t entry_pid, rmi_shard_cache_fix_scan_result* out);
+int rmi_shard_cache_fix_emit(rmi_shard_cache_fix* cf, rmi_spline_point* d_out);
+void rmi_shard_cache_fix_destroy(rmi_shard_cache_fix* cf);
+
 /* ---- The rest of rmi_lib's public surface (host-side code, no device work of their own) ---------
  * rmi_lib::rmi_size (codegen.rs:375-394): bytes of the model's parameters (+ 8 per leaf with the
  * last-layer errors, + 16 per spline knot of a bounded RMI). */

@@ -2798,3 +2798,145 @@ int rmi_shard_evaluate(rmi_shard_eval* e, rmi_shard_comm* c, uint32_t flags, rmi
 }
 
 }  // extern "C"
+
+// ---- the cache-fix spline over a range-partitioned data set (DESIGN.md section 16) ---------------------------------
+struct rmi_shard_cache_fix {
+  const rmi_dataset* ds = nullptr;
+  CacheFixSlab slab{};
+  uint64_t line = 0, nch = 0;
+  int is_last = 0;
+  rmi_spline_point finish{};       // finish()'s point, written by the last non-empty rank
+  cudaStream_t st = nullptr;
+  int num_sms = 0;
+  void* d_mem = nullptr;
+  ShardCacheFixScratch s{};
+  bool speculated = false;         // speculation and the stitches of chunks 1.. are in s
+  bool scanned = false, passed = false;
+  uint64_t slab_knots = 0;         // knots of the last scan's chain inside the slab
+};
+
+extern "C" {
+
+int rmi_shard_cache_fix_create(const rmi_dataset* local, const rmi_shard_ends* ends_all, int world, int rank,
+                               uint64_t line_size, uint64_t halo_keys, void* cuda_stream, rmi_shard_cache_fix** out) {
+  const std::string fn = "rmi_shard_cache_fix_create";
+  g_last_error.clear();
+  if (!local || !ends_all || !out) return fail(RMI_ERR_INVALID, fn + ": null argument");
+  uint64_t total = 0, base = 0;
+  if (int rc = check_slabs(fn, local, ends_all, world, rank, &base, &total)) return rc;
+  if (local->key_type != RMI_KEY_U64) return fail(RMI_ERR_INVALID, fn + ": Can only construct a bounded RMI on u64 data");
+  if (base + local->n + halo_keys > total)
+    return fail(RMI_ERR_INVALID, fn + ": the halo reaches past the end of the data");
+  // rmi_cache_fix_device's panics, in its order, decided from the ends table so that every rank fails alike
+  if (!(total > line_size)) return fail(RMI_ERR_PANIC, "Cannot apply a cachefix with fewer items than the line size");
+  if (line_size == 0) return fail(RMI_ERR_PANIC, "attempt to divide by zero");
+  if (!local->sorted) return fail(RMI_ERR_PANIC, "keys are not sorted in ascending order");
+  const SlabLayout lay = rmihost::slab_layout<uint64_t>(ends_all, world, rank, 1);
+  if (lay.first_key_bits == 0) return fail(RMI_ERR_PANIC, "When source x is 18446744073709551615, cannot set dest x to 0");
+  CUDA_TRY(cudaSetDevice(local->device));
+  DeviceInfo di;
+  if (int rc = device_info(local->device, &di)) return rc;
+  auto* cf = new rmi_shard_cache_fix();
+  cf->ds = local;
+  cf->line = line_size;
+  cf->st = (cudaStream_t)cuda_stream;
+  cf->num_sms = di.num_sms;
+  cf->is_last = lay.is_last;
+  cf->finish = rmi_spline_point{lay.last_key_bits, lay.last_F};
+  CacheFixSlab& S = cf->slab;
+  S.keys = (const u64*)local->d_keys;
+  S.base = base;
+  S.n_local = local->n;
+  S.n_avail = local->n + halo_keys;
+  S.prev_key = lay.has_prev ? lay.prev_key_bits : 0;
+  S.has_prev = lay.has_prev;
+  S.at_end = base + S.n_avail == total;
+  const u64 nch = cf->nch = (local->n + CACHEFIX_CHUNK - 1) / CACHEFIX_CHUNK;
+  if (nch) {
+    const size_t words = nch * CACHEFIX_TARGETS + 3 * nch + (nch + 1) / 2 + 4 * nch + (nch + 1) + 4;
+    if (cudaMalloc(&cf->d_mem, sizeof(u64) * words) != cudaSuccess) {
+      cudaGetLastError();
+      delete cf;
+      return fail(RMI_ERR_CUDA, fn + ": device allocation failed");
+    }
+    u64* p = (u64*)cf->d_mem;
+    ShardCacheFixScratch& s = cf->s;
+    s.targets = p; p += nch * CACHEFIX_TARGETS;
+    s.spec_count = p; p += nch;
+    s.spec_exit = p; p += nch;
+    s.stitch_exit = p; p += nch;
+    s.stitch_ok = (u32*)p; p += (nch + 1) / 2;
+    s.st_entry = p; p += 2 * nch;
+    s.entry = p; p += 2 * nch;
+    s.offsets = p; p += nch + 1;
+    s.res = p;
+  }
+  *out = cf;
+  return RMI_OK;
+}
+
+void rmi_shard_cache_fix_destroy(rmi_shard_cache_fix* cf) {
+  if (!cf) return;
+  if (cf->d_mem) {
+    cudaStreamSynchronize(cf->st);
+    cudaFree(cf->d_mem);
+  }
+  delete cf;
+}
+
+int rmi_shard_cache_fix_scan(rmi_shard_cache_fix* cf, uint64_t entry_pid, rmi_shard_cache_fix_scan_result* out) {
+  const std::string fn = "rmi_shard_cache_fix_scan";
+  g_last_error.clear();
+  if (!cf || !out) return fail(RMI_ERR_INVALID, fn + ": null argument");
+  const CacheFixSlab& S = cf->slab;
+  if (entry_pid < 2 * S.base)
+    return fail(RMI_ERR_INVALID, fn + ": entry pid " + std::to_string(entry_pid) + " lies before the slab (first pid " +
+                                     std::to_string(2 * S.base) + ")");
+  *out = rmi_shard_cache_fix_scan_result{};
+  cf->scanned = true;
+  cf->passed = entry_pid >= 2 * (S.base + S.n_local);   // a segment spanning the whole slab, or an empty slab
+  if (cf->passed) {
+    cf->slab_knots = 0;
+    out->exit_pid = entry_pid;
+  } else {
+    CUDA_TRY(cudaSetDevice(cf->ds->device));
+    Launch L{cf->st, cf->num_sms};
+    if (!cf->speculated) shard_cache_fix_speculate(L, S, cf->line, CACHEFIX_CHUNK, cf->s);
+    shard_cache_fix_join(L, S, cf->line, CACHEFIX_CHUNK, entry_pid, cf->speculated, cf->s);
+    u64 res[4] = {};
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaMemcpyAsync(res, cf->s.res, sizeof res, cudaMemcpyDeviceToHost, cf->st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(cf->st);
+    if (e != cudaSuccess) { cf->scanned = false; return fail(RMI_ERR_CUDA, fn + ": " + cudaGetErrorString(e)); }
+    cf->speculated = true;
+    cf->slab_knots = res[1];
+    out->exit_pid = res[0];
+    out->status = res[2] ? RMI_SHARD_CACHE_FIX_HALO_TOO_SMALL : 0;
+    out->reach = res[3];
+    if (out->status) cf->scanned = false;
+  }
+  out->num_knots = cf->slab_knots + (cf->is_last ? 1 : 0);
+  return RMI_OK;
+}
+
+int rmi_shard_cache_fix_emit(rmi_shard_cache_fix* cf, rmi_spline_point* d_out) {
+  const std::string fn = "rmi_shard_cache_fix_emit";
+  g_last_error.clear();
+  if (!cf) return fail(RMI_ERR_INVALID, fn + ": null argument");
+  if (!cf->scanned) return fail(RMI_ERR_INVALID, fn + ": no complete scan to emit");
+  const uint64_t total = cf->slab_knots + (cf->is_last ? 1 : 0);
+  if (!total) return RMI_OK;
+  if (!d_out) return fail(RMI_ERR_INVALID, fn + ": null output");
+  CUDA_TRY(cudaSetDevice(cf->ds->device));
+  if (!cf->passed && cf->slab_knots) {
+    Launch L{cf->st, cf->num_sms};
+    shard_cache_fix_emit(L, cf->slab, cf->line, CACHEFIX_CHUNK, cf->s, d_out);
+    CUDA_TRY(cudaGetLastError());
+  }
+  // finish() (cache_fix.rs:91-93): from pageable memory, staged before the call returns
+  if (cf->is_last) CUDA_TRY(cudaMemcpyAsync(d_out + cf->slab_knots, &cf->finish, sizeof(rmi_spline_point),
+                                            cudaMemcpyHostToDevice, cf->st));
+  return RMI_OK;
+}
+
+}  // extern "C"

@@ -252,6 +252,39 @@ void cache_fix_scan(const Launch& L, const u64* keys, u64 n, u64 line, u64 chunk
 void cache_fix_emit(const Launch& L, const u64* keys, u64 n, u64 line, u64 chunk, const CacheFixScratch& s,
                     void* d_out);
 
+// ---- the cache-fix scan over one rank's slab of range-partitioned keys (kernels_shard_cachefix.cu, section 16) ----
+// The keys a rank's walks read: its own keys [0, n_local), then the halo up to n_avail.  Point ids are global.
+struct CacheFixSlab {
+  const u64* keys;
+  u64 base;        // global index of local key 0
+  u64 n_local;     // the slab's own keys (> 0)
+  u64 n_avail;     // own keys + halo keys
+  u64 prev_key;    // the last key of the previous non-empty rank; 0 when there is none
+  int has_prev;
+  int at_end;      // base + n_avail is the end of the data
+};
+// Device scratch of one rank's scan, nch = ceil(n_local / chunk) chunks.
+struct ShardCacheFixScratch {
+  u64* targets;       // nch x CACHEFIX_TARGETS
+  u64* spec_count;    // nch
+  u64* spec_exit;     // nch
+  u64* stitch_exit;   // nch
+  u32* stitch_ok;     // nch
+  u64* st_entry;      // 2 x nch: the stitch's entries | counts (kept across scans: they do not depend on the entry)
+  u64* entry;         // 2 x nch: the resolved entries | counts of the last scan
+  u64* offsets;       // nch + 1
+  u64* res;           // 4: exit pid, knots in the slab, status (1: halo too small), global index the walk lacked
+};
+// Speculation of every chunk (once per slab and line size).
+void shard_cache_fix_speculate(const Launch& L, const CacheFixSlab& S, u64 line, u64 chunk, const ShardCacheFixScratch& s);
+// Stitch (every chunk, or chunk 0 alone when the other chunks' stitches are in s.st_entry already) from entry_pid
+// (a pid in the slab: the chain starts at the first point at or after it), then the resolve; fills s.res.
+void shard_cache_fix_join(const Launch& L, const CacheFixSlab& S, u64 line, u64 chunk, u64 entry_pid, bool chunk0_only,
+                          const ShardCacheFixScratch& s);
+// Writes the res[1] knots of the last join to d_out as {key, offset} pairs.
+void shard_cache_fix_emit(const Launch& L, const CacheFixSlab& S, u64 line, u64 chunk, const ShardCacheFixScratch& s,
+                          void* d_out);
+
 // ---- range-partitioned build phases (kernels_shard.cu) ---------------------------------------
 size_t shard_scratch_bytes();
 template <class T>

@@ -23,6 +23,9 @@ its lower bound, is searched there, and its global answer comes back.
 
 evaluate_sharded measures a given RMI's error bounds over the same slabs (DESIGN.md section 15): every rank streams
 only its own keys, and one all-reduce MAX of per-leaf maxima combines them.
+
+cache_fix_sharded fits the `--bounded` cache-fix spline over the same slabs (DESIGN.md section 16), knot for knot the
+single-GPU scan's, and train_bounded_sharded builds the bounded RMI over the knots without gathering them on one GPU.
 """
 from __future__ import annotations
 
@@ -239,6 +242,9 @@ class CudaShardEngine:
 
     def evaluator(self, trained, ends_all: np.ndarray, world: int, rank: int) -> "CudaShardEval":
         return CudaShardEval(self, trained, ends_all, world, rank)
+
+    def cache_fixer(self, ends_all: np.ndarray, world: int, rank: int, line_size: int, halo_keys: int) -> "CudaShardCacheFix":
+        return CudaShardCacheFix(self, ends_all, world, rank, line_size, halo_keys)
 
     def end(self):
         if self._build is not None:
@@ -786,3 +792,180 @@ class ShardedRMIIndex:
     def close(self):
         if hasattr(self.index, "close"):
             self.index.close()
+
+
+# ---- the cache-fix spline over the slabs (include/rmi_b200.h rmi_shard_cache_fix_*, DESIGN.md section 16) -----------
+
+class _CacheFixScan(C.Structure):
+    _fields_ = [("exit_pid", C.c_uint64), ("num_knots", C.c_uint64), ("reach", C.c_uint64), ("status", C.c_uint32),
+                ("_pad", C.c_uint32)]
+
+
+PID_END = (1 << 64) - 1            # RMI_SHARD_CACHE_FIX_PID_END: the last segment stays open to the end of the data
+CACHE_FIX_HALO_TOO_SMALL = 1       # RMI_SHARD_CACHE_FIX_HALO_TOO_SMALL
+
+
+class CudaShardCacheFix:
+    """One rank's side of cache_fix_sharded on librmi_b200.so (rmi_shard_cache_fix_*), on the current torch stream of
+    the data's device.  scan(entry) -> (exit pid, status, reach, knots to emit); emit() -> the knots as a (K, 2) int64
+    tensor (uint64 key, offset) on the device."""
+
+    def __init__(self, eng: CudaShardEngine, ends_all: np.ndarray, world: int, rank: int, line_size: int,
+                 halo_keys: int):
+        L = self.lib = api.load_library()
+        L.rmi_shard_cache_fix_create.argtypes = [C.c_void_p, C.POINTER(_Ends), C.c_int, C.c_int, C.c_uint64, C.c_uint64,
+                                                 C.c_void_p, C.POINTER(C.c_void_p)]
+        L.rmi_shard_cache_fix_scan.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(_CacheFixScan)]
+        L.rmi_shard_cache_fix_emit.argtypes = [C.c_void_p, C.c_void_p]
+        L.rmi_shard_cache_fix_destroy.argtypes = [C.c_void_p]
+        self.device = eng.device
+        self._ds = eng.ds             # the slab and its halo are read at every scan: kept alive with it
+        self.num_knots = 0
+        self._h = C.c_void_p()
+        stream = torch.cuda.current_stream(self.device).cuda_stream or None
+        api._check(L.rmi_shard_cache_fix_create(eng.ds._h, _ends_array(ends_all), world, rank, int(line_size),
+                                                int(halo_keys), C.c_void_p(stream), C.byref(self._h)))
+
+    def scan(self, entry: int):
+        r = _CacheFixScan()
+        api._check(self.lib.rmi_shard_cache_fix_scan(self._h, int(entry), C.byref(r)))
+        self.num_knots = int(r.num_knots)
+        return int(r.exit_pid), int(r.status), int(r.reach), int(r.num_knots)
+
+    def emit(self) -> torch.Tensor:
+        out = torch.empty((self.num_knots, 2), dtype=torch.int64, device=self.device)
+        api._check(self.lib.rmi_shard_cache_fix_emit(self._h, out.data_ptr() if self.num_knots else None))
+        return out
+
+    def close(self):
+        if getattr(self, "_h", None) and self._h.value:
+            self.lib.rmi_shard_cache_fix_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def _gather_rows(row: list[int], world: int, group, dev, stage: bool) -> list[list[int]]:
+    """Every rank's row of u64 words, in rank order (a tiny all-gather; through the host under gloo)."""
+    t = torch.from_numpy(np.array(row, dtype=np.uint64).view(np.int64))
+    if world <= 1:
+        return [list(row)]
+    t = t if stage else t.to(dev)
+    out = [torch.empty_like(t) for _ in range(world)]
+    dist.all_gather(out, t, group=group)
+    return [[int(v) for v in o.cpu().numpy().view(np.uint64)] for o in out]
+
+
+def cache_fix_sharded(data, line_size: int, group=None, root_only: bool = False, engine=None,
+                      timings: dict | None = None):
+    """api.cache_fix of the concatenated slabs (u64 keys), fitted where the keys live (DESIGN.md section 16).  Returns
+    the (K, 2) uint64 knot array on every rank, or on rank 0 only with root_only (None elsewhere); collective.  Each
+    rank also keeps its own knots on its device as ``data.cache_fix_knots = (line_size, (K_r, 2) int64 tensor)``: a
+    sorted slab of the knot set.  Raises the reference's panics (RMIPanic) on every rank alike, and RMIError for keys
+    that are not u64.
+
+    Every rank scans its slab from an entry point and reports its exit, the first knot at or past the next slab; ranks
+    whose entry is not their predecessor's exit scan again from it until every entry agrees (at most world - 1 more
+    rounds), then emit their knots.  A chain that needs keys past the halo fetched behind the slabs grows the halo
+    and starts again.  timings: filled with the rounds and the host times (s) of the scans, rounds, emit and gather."""
+    import time
+    eng = engine if engine is not None else data.engine
+    group = group if group is not None else getattr(data, "group", None)
+    rank, world = _world(group)
+    dev = eng.device
+    ends_all = gather_ends(data, eng, group)
+    bases = [0]
+    for n_local in ends_all[:, 3]:
+        bases.append(bases[-1] + int(n_local))
+    n_global = bases[-1]
+    if world > 1 and getattr(data, "_halo_have", None) is None:
+        cap = _min_halo_capacity(data, group, world, dev)
+        moves = plan_halo(bases, [bases[g + 1] + cap - 1 for g in range(world)], n_global)
+        data._halo_have = _exchange_halo(eng, moves, rank, group, dev)
+    stage = world > 1 and dev.type == "cuda" and dist.get_backend(group) == "gloo"
+
+    def sync():
+        if dev.type == "cuda":
+            torch.cuda.synchronize(dev)
+
+    t = {} if timings is None else timings
+    cf = eng.cache_fixer(ends_all, world, rank, line_size, getattr(data, "_halo_have", 0) or 0)
+    try:
+        t0 = time.perf_counter()
+        entry = 2 * bases[rank]                      # this rank's own first point
+        exit_pid, status, reach, count = cf.scan(entry)
+        t["first_scan_s"] = time.perf_counter() - t0
+        rounds, t0 = 0, time.perf_counter()
+        while True:
+            table = _gather_rows([entry, exit_pid, status, reach, count], world, group, dev, stage)
+            if any(row[2] & CACHE_FIX_HALO_TOO_SMALL for row in table):
+                cf.close()
+                return _cache_fix_with_larger_halo(data, line_size, group, root_only, engine, timings, table, bases)
+            moved = False
+            for r in range(1, world):
+                if table[r][0] != table[r - 1][1]:
+                    moved = True
+                    if r == rank:
+                        entry = table[r - 1][1]
+                        exit_pid, status, reach, count = cf.scan(entry)
+            if not moved:
+                break
+            rounds += 1
+        t["join_rounds"] = rounds
+        t["join_s"] = time.perf_counter() - t0
+        t0 = time.perf_counter()
+        local = cf.emit()
+        sync()
+        t["emit_s"] = time.perf_counter() - t0
+    finally:
+        cf.close()
+    data.cache_fix_knots = (int(line_size), local)
+    t0 = time.perf_counter()
+    counts = [row[4] for row in table]
+    if world <= 1:
+        knots = local.cpu()
+    else:
+        # equal-sized pieces for the collective: every rank's knots padded to the largest count
+        send = torch.zeros((max(counts), 2), dtype=torch.int64, device="cpu" if stage else dev)
+        send[: counts[rank]].copy_(local)
+        if root_only:
+            parts = [torch.empty_like(send) for _ in range(world)] if rank == 0 else None
+            dist.gather(send, parts, dst=dist.get_global_rank(group, 0) if group is not None else 0, group=group)
+        else:
+            parts = [torch.empty_like(send) for _ in range(world)]
+            dist.all_gather(parts, send, group=group)
+        knots = torch.cat([p[:c] for p, c in zip(parts, counts)]).cpu() if parts is not None else None
+    t["gather_s"] = time.perf_counter() - t0
+    if knots is None or (root_only and rank != 0):
+        return None
+    return knots.numpy().view(np.uint64).reshape(-1, 2)
+
+
+def _cache_fix_with_larger_halo(data, line_size, group, root_only, engine, timings, table, bases):
+    # A chain reaches past the halo.  Every rank saw the same table: grow every halo past the furthest walk and redo.
+    if not hasattr(data, "grow_halo"):
+        raise api.RMIError("the cache-fix spline reaches past the halo copied from the next ranks")
+    need = max(row[3] - bases[r + 1] for r, row in enumerate(table) if row[2] & CACHE_FIX_HALO_TOO_SMALL)
+    data.grow_halo(2 * max(need, data.halo_capacity) + 256)
+    return cache_fix_sharded(data, line_size, group, root_only, None, timings)
+
+
+def train_bounded_sharded(data, model_spec: str, num_leaves: int, line_size: int, flags: int = 0, group=None,
+                          halo_capacity: int = 1 << 20):
+    """api.train_bounded over range-partitioned keys: returns (TrainedRMI with num_data_rows = the keys of all slabs,
+    knots), the pair api.train_bounded returns for the concatenated keys, on every rank; collective.  The spline is
+    fitted by cache_fix_sharded, then train_sharded builds the RMI over every rank's slab of knot keys (a
+    ShardedTrainingData with halo_capacity keys of room), so no knot table has to fit on one GPU.
+    api.output_rmi(..., cache_fix_knots=knots, line_size=line_size) then writes the reference's `--bounded` artefact."""
+    group = group if group is not None else getattr(data, "group", None)
+    knots = cache_fix_sharded(data, line_size, group)
+    _, local = data.cache_fix_knots
+    kdata = ShardedTrainingData(local[:, 0].contiguous(), key_type=api.KEY_U64, halo_capacity=halo_capacity,
+                                group=group)
+    rmi = train_sharded(kdata, model_spec, num_leaves, flags, group)
+    rmi.num_data_rows = int(gather_ends(data, data.engine, group)[:, 3].astype(np.uint64).sum())
+    return rmi, knots
