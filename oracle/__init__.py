@@ -31,6 +31,15 @@ def build(force: bool = False) -> str:
     return _LIB_PATH
 
 
+def build_variant(out_dir: str, *defines: str):
+    """A test-only variant of the oracle, compiled into out_dir with the given -D macros (e.g. ORACLE_FIT_LN_NOISE)
+    and loaded: pass it to train(..., library=...)."""
+    so = os.path.join(os.path.abspath(out_dir), "librmi_oracle.so")
+    subprocess.run(["make", "-C", _HERE, f"OUT={so}", "DEFINES=" + " ".join(f"-D{d}" for d in defines)], check=True,
+                   stdout=subprocess.DEVNULL)
+    return _bind(C.CDLL(so))
+
+
 _lib = None
 
 
@@ -38,39 +47,42 @@ def lib():
     global _lib
     if _lib is None:
         build()
-        L = C.CDLL(_LIB_PATH)
-        L.rmi_oracle_train.restype = C.c_void_p
-        L.rmi_oracle_train.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.c_char_p, C.c_uint64,
-                                       C.c_void_p, C.c_int, C.c_int]
-        L.rmi_oracle_last_error.restype = C.c_char_p
-        L.rmi_oracle_free.argtypes = [C.c_void_p]
-        L.rmi_oracle_summary.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-        L.rmi_oracle_l0_sizes.argtypes = [C.c_void_p, C.c_void_p]
-        L.rmi_oracle_l0_get.argtypes = [C.c_void_p] + [C.c_void_p] * 5
-        L.rmi_oracle_l1_params_per_model.restype = C.c_uint32
-        L.rmi_oracle_l1_params_per_model.argtypes = [C.c_void_p]
-        L.rmi_oracle_l1_get.argtypes = [C.c_void_p] + [C.c_void_p] * 3
-        L.rmi_oracle_lookup.restype = C.c_uint64
-        L.rmi_oracle_lookup.argtypes = [C.c_void_p, C.c_int, C.c_uint64, C.c_double, C.c_void_p]
-        L.rmi_oracle_lookup_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_void_p, C.c_void_p]
-        L.rmi_oracle_model_train.restype = C.c_void_p
-        L.rmi_oracle_model_train.argtypes = [C.c_char_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_double]
-        L.rmi_oracle_model_free.argtypes = [C.c_void_p]
-        L.rmi_oracle_model_predict_int.restype = C.c_uint64
-        L.rmi_oracle_model_predict_int.argtypes = [C.c_void_p, C.c_int, C.c_uint64, C.c_double]
-        L.rmi_oracle_model_predict_float.restype = C.c_double
-        L.rmi_oracle_model_predict_float.argtypes = [C.c_void_p, C.c_int, C.c_uint64, C.c_double]
-        L.rmi_oracle_model_sizes.argtypes = [C.c_void_p, C.c_void_p]
-        L.rmi_oracle_model_get.argtypes = [C.c_void_p] + [C.c_void_p] * 5
-        L.rmi_oracle_model_high.restype = C.c_int
-        L.rmi_oracle_model_high.argtypes = [C.c_void_p]
-        L.rmi_oracle_scale_offset.restype = C.c_uint64
-        L.rmi_oracle_scale_offset.argtypes = [C.c_uint64, C.c_double]
-        L.rmi_oracle_set_trailing_repeat.argtypes = [C.c_int]
-        L.rmi_oracle_common_prefix_u64.restype = C.c_uint8
-        L.rmi_oracle_common_prefix_u64.argtypes = [C.c_void_p, C.c_uint64]
-        _lib = L
+        _lib = _bind(C.CDLL(_LIB_PATH))
     return _lib
+
+
+def _bind(L):
+    L.rmi_oracle_train.restype = C.c_void_p
+    L.rmi_oracle_train.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.c_char_p, C.c_uint64,
+                                   C.c_void_p, C.c_int, C.c_int]
+    L.rmi_oracle_last_error.restype = C.c_char_p
+    L.rmi_oracle_free.argtypes = [C.c_void_p]
+    L.rmi_oracle_summary.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    L.rmi_oracle_l0_sizes.argtypes = [C.c_void_p, C.c_void_p]
+    L.rmi_oracle_l0_get.argtypes = [C.c_void_p] + [C.c_void_p] * 5
+    L.rmi_oracle_l1_params_per_model.restype = C.c_uint32
+    L.rmi_oracle_l1_params_per_model.argtypes = [C.c_void_p]
+    L.rmi_oracle_l1_get.argtypes = [C.c_void_p] + [C.c_void_p] * 3
+    L.rmi_oracle_lookup.restype = C.c_uint64
+    L.rmi_oracle_lookup.argtypes = [C.c_void_p, C.c_int, C.c_uint64, C.c_double, C.c_void_p]
+    L.rmi_oracle_lookup_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_void_p, C.c_void_p]
+    L.rmi_oracle_model_train.restype = C.c_void_p
+    L.rmi_oracle_model_train.argtypes = [C.c_char_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_double]
+    L.rmi_oracle_model_free.argtypes = [C.c_void_p]
+    L.rmi_oracle_model_predict_int.restype = C.c_uint64
+    L.rmi_oracle_model_predict_int.argtypes = [C.c_void_p, C.c_int, C.c_uint64, C.c_double]
+    L.rmi_oracle_model_predict_float.restype = C.c_double
+    L.rmi_oracle_model_predict_float.argtypes = [C.c_void_p, C.c_int, C.c_uint64, C.c_double]
+    L.rmi_oracle_model_sizes.argtypes = [C.c_void_p, C.c_void_p]
+    L.rmi_oracle_model_get.argtypes = [C.c_void_p] + [C.c_void_p] * 5
+    L.rmi_oracle_model_high.restype = C.c_int
+    L.rmi_oracle_model_high.argtypes = [C.c_void_p]
+    L.rmi_oracle_scale_offset.restype = C.c_uint64
+    L.rmi_oracle_scale_offset.argtypes = [C.c_uint64, C.c_double]
+    L.rmi_oracle_set_trailing_repeat.argtypes = [C.c_int]
+    L.rmi_oracle_common_prefix_u64.restype = C.c_uint8
+    L.rmi_oracle_common_prefix_u64.argtypes = [C.c_void_p, C.c_uint64]
+    return L
 
 
 class OraclePanic(RuntimeError):
@@ -120,11 +132,12 @@ class OracleRMI:
     l1_counts: np.ndarray        # (N,) uint64
     could_not_replace: bool = False
     _handle: int = field(default=0, repr=False)
+    _lib: object = field(default=None, repr=False)   # the library that made it (a build_variant one, or None)
 
     def lookup(self, key) -> tuple[int, int]:
         err = C.c_uint64(0)
         isf = isinstance(key, float)
-        pos = lib().rmi_oracle_lookup(self._handle, int(isf), 0 if isf else int(key), float(key) if isf else 0.0,
+        pos = (self._lib or lib()).rmi_oracle_lookup(self._handle, int(isf), 0 if isf else int(key), float(key) if isf else 0.0,
                                       C.byref(err))
         return int(pos), int(err.value)
 
@@ -132,12 +145,12 @@ class OracleRMI:
         keys = np.ascontiguousarray(keys)
         pos = np.zeros(keys.size, dtype=np.uint64)
         err = np.zeros(keys.size, dtype=np.uint64)
-        lib().rmi_oracle_lookup_batch(self._handle, _ptr(keys), keys.size, key_type_of(keys), _ptr(pos), _ptr(err))
+        (self._lib or lib()).rmi_oracle_lookup_batch(self._handle, _ptr(keys), keys.size, key_type_of(keys), _ptr(pos), _ptr(err))
         return pos, err
 
     def close(self):
         if self._handle:
-            lib().rmi_oracle_free(self._handle)
+            (self._lib or lib()).rmi_oracle_free(self._handle)
             self._handle = 0
 
     def __del__(self):
@@ -159,11 +172,13 @@ def _get_model(sizes_fn, get_fn, h, kind, high=True) -> ModelParams:
     return ModelParams(kind, fp, ip, t32, a1, a2, high)
 
 
-def train(keys: np.ndarray, model_spec: str, branch_factor: int, l0_override=None, threads: int = 2) -> OracleRMI:
-    """rmi_lib::train (train/mod.rs:100) on an in-memory sorted key array."""
+def train(keys: np.ndarray, model_spec: str, branch_factor: int, l0_override=None, threads: int = 2,
+          library=None) -> OracleRMI:
+    """rmi_lib::train (train/mod.rs:100) on an in-memory sorted key array (with `library` from build_variant: the
+    variant's train)."""
     keys = np.ascontiguousarray(keys)
     kt = key_type_of(keys)
-    L = lib()
+    L = library or lib()
     ov = None if l0_override is None else np.ascontiguousarray(l0_override, dtype=np.float64)
     h = L.rmi_oracle_train(_ptr(keys), keys.size, kt, model_spec.encode(), int(branch_factor),
                            _ptr(ov), 0 if ov is None else ov.size, threads)
@@ -182,7 +197,7 @@ def train(keys: np.ndarray, model_spec: str, branch_factor: int, l0_override=Non
     return OracleRMI(n=int(scal[0]), branching_factor=N, max_error=int(scal[2]), max_error_idx=int(scal[3]),
                      avg_error=float(stats[0]), avg_l2_error=float(stats[1]), avg_log2_error=float(stats[2]),
                      max_log2_error=float(stats[3]), l0=l0, l1_kind=KINDS[int(scal[5])], l1_params=params,
-                     l1_errors=errors, l1_counts=counts, could_not_replace=bool(scal[7]), _handle=h)
+                     l1_errors=errors, l1_counts=counts, could_not_replace=bool(scal[7]), _handle=h, _lib=library)
 
 
 class OracleModel:

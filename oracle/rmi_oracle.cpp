@@ -51,6 +51,22 @@ inline uint64_t f64_to_u64(double v) {
   if (v >= 18446744073709551616.0) return UINT64_MAX;
   return (uint64_t)v;
 }
+// ln at fit time (loglinear's ln y, lognormal's ln x).  Compiled with -DORACLE_FIT_LN_NOISE (a test-only variant,
+// never the default build) it is moved by -1, 0 or +1 ulp, chosen by a hash of the argument: how far the fitted
+// parameters move when two libms' ln disagree in the last place.
+inline double fit_ln(double x) {
+  double l = std::log(x);
+#ifdef ORACLE_FIT_LN_NOISE
+  if (std::isfinite(l) && l != 0.0) {
+    uint64_t b;
+    std::memcpy(&b, &x, sizeof b);
+    const int step = (int)(((b * 0x9E3779B97F4A7C15ull) >> 40) % 3) - 1;
+    if (step) l = std::nextafter(l, step > 0 ? INFINITY : -INFINITY);
+  }
+#endif
+  return l;
+}
+
 // Rust f64::max(a, b): returns the non-NaN operand if one is NaN.
 inline double rust_fmax(double a, double b) {
   if (std::isnan(a)) return b;
@@ -358,7 +374,7 @@ template <class T> Model loglinear_new(const Data<T>& data) {
   FixDupsIter<T> it(data);
   T k; size_t y;
   while (it.next(k, y)) {
-    double ly = std::log((double)y);
+    double ly = fit_ln((double)y);
     if (!std::isfinite(ly)) continue;
     s.push(KeyTraits<T>::as_float(k), ly);
   }
@@ -487,7 +503,7 @@ template <class T> Model normal_new(const Data<T>& data, bool lognormal) {
     FixDupsIter<T> it(data);
     while (it.next(k, y)) {
       double x = KeyTraits<T>::as_float(k);
-      if (lognormal) { double l = std::log(x); x = std::isfinite(l) ? l : 0.0; }
+      if (lognormal) { double l = fit_ln(x); x = std::isfinite(l) ? l : 0.0; }
       mean += x / n;
       scale = rust_fmax(scale, (double)y);
     }
@@ -496,7 +512,7 @@ template <class T> Model normal_new(const Data<T>& data, bool lognormal) {
     FixDupsIter<T> it(data);
     while (it.next(k, y)) {
       double x = KeyTraits<T>::as_float(k);
-      if (lognormal) { double l = std::log(x); x = std::isfinite(l) ? l : 0.0; }
+      if (lognormal) { double l = fit_ln(x); x = std::isfinite(l) ? l : 0.0; }
       stdev += (x - mean) * (x - mean);
     }
   }

@@ -1053,9 +1053,14 @@ template <int LEAF> __device__ __forceinline__ bool set_constant(double* f, u64 
 // Leaf predictions are clamped to n by error_between.  With 32-bit indices (n < 2^32 - 1) the
 // conversion saturates at 2^32 - 1 >= n, which the clamp to n makes equivalent to
 // leaf_predict64 (models.cuh).
-// NANCHECK: leaf parameters (hence predictions) can only be NaN for float keys or for the
-// normal / lognormal / loglinear leaves; integer keys with linear / spline / cubic leaves
-// always give finite parameters, so the select is compiled out there.
+// NANCHECK: a NaN prediction must become 0, as the reference's saturating `as` cast makes it;
+// the conversion does not do that by itself (on sm_90 it gives at least n).  Predictions can be
+// NaN for float keys, for the normal / lognormal / loglinear leaves, and for linear_spline /
+// cubic leaves over uint64 keys: above 2^53 distinct keys can round onto one double, and a
+// leaf whose first and last keys do gets a slope of -inf and an intercept of +inf (the
+// reference tests the raw keys for equality but divides by their doubles' difference).  Linear
+// and robust_linear leaves keep finite parameters (a zero variance gives a constant model), as
+// do all leaves over uint32 keys (exact in double), so the select is compiled out there.
 template <int LEAF, class I, bool NANCHECK>
 __device__ __forceinline__ I leaf_predict_clamped(const double* f, double x, I n) {
   double p = predict_float<LEAF>(f, x);
@@ -1325,7 +1330,8 @@ k_leaf(const T* __restrict__ keys, const Shard<T> sh, u64 N, const u64* __restri
   const u64 j = long_mode == 1 ? (threadIdx.x == 0 ? (u64)long_list[1 + blockIdx.x] : N)
                                : group * blockDim.x + threadIdx.x;
   constexpr int PPM = leaf_params_per_model(LEAF);
-  constexpr bool NANCHECK = Key<T>::is_float || LEAF == M_LOGLINEAR || LEAF == M_NORMAL || LEAF == M_LOGNORMAL;
+  constexpr bool NANCHECK = Key<T>::is_float || LEAF == M_LOGLINEAR || LEAF == M_NORMAL || LEAF == M_LOGNORMAL ||
+                           (sizeof(T) == 8 && (LEAF == M_LINEAR_SPLINE || LEAF == M_CUBIC));
   const u64 n = sh.n_global;
   const I nI = (I)n;
   const I baseI = (I)sh.base;

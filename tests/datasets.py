@@ -51,14 +51,18 @@ def lognormal_f64(n: int, seed: int = 11, sigma: float = 2.0) -> np.ndarray:
     return k
 
 
-def designed_leaves(counts, shift: int, dtype=np.uint64, runs=(), seed: int = 17) -> np.ndarray:
+def designed_leaves(counts, shift: int, dtype=np.uint64, runs=(), seed: int = 17, base: int = 0) -> np.ndarray:
     """Keys with a chosen number of keys per leaf: counts[j] distinct sorted keys in [j*2^shift, (j+1)*2^shift)
     for every j, then each (start, length) of `runs` (global indices) overwritten with copies of its first key.
 
     A top model that maps x to x / 2^shift (an injected linear top with l0 params [0, 2^-shift], or a radix top
     when len(counts) is a power of two and the last leaf is non-empty) then puts exactly counts[j] keys into
     leaf j.  Without runs no two keys are equal.  Every run must lie inside one leaf (equal keys always share
-    a leaf)."""
+    a leaf).
+
+    `base` (uint64 keys only) is added to every key.  Above 2^53 distinct keys can share one double: at base 2^63
+    a double covers 2^11 integers, so a leaf of at most 2^11 values holds keys that round onto a few doubles.  The
+    radix top works on the integers and still reproduces the design; a linear top on the doubles does not."""
     counts = np.asarray(counts, dtype=np.int64)
     span = 1 << shift
     if counts.min(initial=0) < 0 or counts.max(initial=0) > span:
@@ -67,6 +71,8 @@ def designed_leaves(counts, shift: int, dtype=np.uint64, runs=(), seed: int = 17
         raise ValueError(f"{counts.size} leaves of 2^{shift} values do not fit uint32 keys")
     if np.dtype(dtype) == np.float64 and counts.size * span > 1 << 53:
         raise ValueError("keys beyond 2^53 are not exact in float64")
+    if base and (np.dtype(dtype) != np.uint64 or base < 0 or base + counts.size * span > 1 << 64):
+        raise ValueError(f"a key base of {base} needs uint64 keys that stay below 2^64")
     rng = np.random.Generator(np.random.MT19937(seed))
     n = int(counts.sum())
     leaf = np.repeat(np.arange(counts.size, dtype=np.int64), counts)
@@ -85,6 +91,8 @@ def designed_leaves(counts, shift: int, dtype=np.uint64, runs=(), seed: int = 17
         k[s:s + length] = k[s]
     if np.dtype(dtype) == np.float64:
         return k.astype(np.float64)
+    if base:
+        return k.astype(np.uint64) + np.uint64(base)
     return k.astype(dtype)
 
 

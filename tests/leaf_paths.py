@@ -53,9 +53,9 @@ def _thresholds():
 
 K = _thresholds()
 
-LEAVES = ("linear", "linear_spline", "cubic", "robust_linear")
+LEAVES = ("linear", "linear_spline", "cubic", "robust_linear", "loglinear", "normal", "lognormal")
 DTYPES = (np.uint64, np.uint32, np.float64)
-ANY_LEAF = LEAVES + ("normal",)
+ANY_LEAF = LEAVES
 # leaf types with a DUPS = false instantiation (launch_leaf's SPECIALISED)
 NO_DUPS_LEAVES = ("linear", "linear_spline", "cubic")
 
@@ -64,8 +64,8 @@ PATHS = {
     "all_short": ("linear",),            # fit: every vector of the warp below the shared reciprocal table
     "ring": ("linear",),                 # fit: per-warp reciprocal ring
     "solo": ("linear",),                 # fit: one lane's chain handed to the whole warp (solo_chain)
-    "rcp_global": ("robust_linear",),    # general step: counts past the shared table, from the global table
-    "rcp_divide": ("robust_linear",),    # general step: counts past the global table, by division
+    "rcp_global": ("robust_linear", "loglinear"),   # general step: counts past the shared table, from the global table
+    "rcp_divide": ("robust_linear", "loglinear"),   # general step: counts past the global table, by division
     "lane_serial_fwd": ANY_LEAF,         # forward pass: every lane walks its own leaf
     "coop_fwd": ANY_LEAF,                # forward pass: the warp walks its (few) long leaves together
     "coop_fwd_all_long": ("cubic",),     # forward pass: (nearly) all lanes long, cubic leaves
@@ -80,10 +80,12 @@ def _kpp(dtype):
     return 16 // np.dtype(dtype).itemsize
 
 
-def census(counts, leaf, dtype, stats_only=False):
+def census(counts, leaf, dtype, stats_only=False, first_run=1):
     """Which paths of k_leaf a single-GPU build over leaves of these key counts takes: a Counter of
     path -> warps (fit and forward paths), leaves (long_kernel, long_in_bulk, rcp_*) or 1 (sliced_copy).
-    The fit paths follow fit_leaf() and stream_pass(); the forward paths the selection of long_fwd in k_leaf."""
+    The fit paths follow fit_leaf() and stream_pass(); the forward paths the selection of long_fwd in k_leaf.
+    `first_run` is the length of the data set's first run of equal keys (its items have offset 0, which a
+    loglinear leaf does not push: ln 0 is not finite)."""
     c = np.asarray(counts, dtype=np.int64)
     N = c.size
     kpp = _kpp(dtype)
@@ -129,11 +131,15 @@ def census(counts, leaf, dtype, stats_only=False):
                 out["long_lane_serial"] += 1
         if (own_w[w] & ~(long_w[w] & (p <= K["FWD_FEW"] or (leaf == "cubic" and p >= K["FWD_ALL_LONG"])))).any():
             out["lane_serial_fwd"] += 1
-    if leaf == "robust_linear":
+    if leaf in ("robust_linear", "loglinear"):
         # the general step fetches 1/count for counts 1 .. items + 1 (one step ahead): the shared table up to
         # RCP_TABLE - 1, the global table below RCP_FAR, a division beyond
-        bnd = np.maximum(np.floor(L.astype(np.float64) * 0.0001).astype(np.int64), 1)
-        items = np.where(L > 2 * bnd + 1, L - 2 * bnd, 0)
+        if leaf == "robust_linear":   # skip(bnd).take(len - 2*bnd) of the vector
+            bnd = np.maximum(np.floor(L.astype(np.float64) * 0.0001).astype(np.int64), 1)
+            items = np.where(L > 2 * bnd + 1, L - 2 * bnd, 0)
+        else:   # the vector and the drained repeat of its final item, less the items with offset 0
+            zero = np.clip(np.minimum(ve, first_run) - vs, 0, None)
+            items = L - zero + ((L > 0) & (ve - 1 >= first_run))
         top = np.where(items > 0, items + 1, 0)
         out["rcp_global"] += int(((top >= K["RCP_TABLE"]) & (top < K["RCP_FAR"])).sum())
         out["rcp_divide"] += int((top >= K["RCP_FAR"]).sum())
@@ -174,6 +180,19 @@ def training_vectors(counts):
     return vs, ve
 
 
+def leaf_ends(counts, keys):
+    """Per leaf, the doubles of its first and last key (of its training vector where it owns no key; NaN where that
+    is empty too): where loglinear leaves' ln-space predictions are compared (parity.loglinear_discrepancy)."""
+    c = np.asarray(counts, dtype=np.int64)
+    S = np.concatenate([[0], np.cumsum(c)])
+    vs, ve = training_vectors(c)
+    lo, hi = np.where(c > 0, S[:-1], vs), np.where(c > 0, S[1:], ve) - 1
+    x = np.asarray(keys).astype(np.float64)
+    ends = np.stack([x[np.clip(lo, 0, x.size - 1)], x[np.clip(hi, 0, x.size - 1)]], axis=1)
+    ends[(c == 0) & (ve <= vs)] = np.nan
+    return ends
+
+
 def solo_handoff(rlen, sw):
     """stream_pass(SOLO = true) over a warp whose lanes stream `rlen` keys each: the (lane, chunk) at which one
     lane is left with at least SOLO_MIN keys and every other lane is done, or None."""
@@ -199,13 +218,25 @@ class Profile:
     runs: tuple = ()       # (start, length) runs of equal keys
     avoids: tuple = ()     # paths it must not take (the other side of a threshold)
     sliced: bool = False   # a sliced-copy profile (built with a decoy first)
+    base: int = 0          # added to every key (uint64 keys, radix top only): datasets.designed_leaves
 
     @property
     def N(self):
         return len(self.counts)
 
+    @property
+    def first_run(self):
+        """Length of the data set's first run of equal keys."""
+        return max([ln for s, ln in self.runs if s == 0], default=1)
+
+    def dtypes(self):
+        return DTYPES if not self.base else (np.uint64,)
+
     def keys(self, dtype, seed=17):
-        return datasets.designed_leaves(self.counts, self.shift, dtype, runs=self.runs, seed=seed)
+        return datasets.designed_leaves(self.counts, self.shift, dtype, runs=self.runs, seed=seed, base=self.base)
+
+    def census(self, leaf, dtype, stats_only=False):
+        return census(self.counts, leaf, dtype, stats_only=stats_only, first_run=self.first_run)
 
     def expected_counts(self):
         """The oracle's l1_counts: the design, plus the drained iterator's repeated final item on the leaf that
@@ -215,8 +246,9 @@ class Profile:
         return e
 
     def tops(self, dtype):
-        """'linear' (injected top x / 2^shift) always; 'radix' where it reproduces the design."""
-        t = ["linear"]
+        """'linear' (injected top x / 2^shift) wherever the keys are exact doubles; 'radix' where it reproduces the
+        design."""
+        t = [] if self.base else ["linear"]
         if np.dtype(dtype) != np.float64 and self.N & (self.N - 1) == 0 and self.counts[-1] > 0:
             t.append("radix")
         return t
@@ -233,8 +265,10 @@ class Profile:
         return tuple(l for l in LEAVES if l != "robust_linear" or robust_ok)
 
     def cubic_exact(self):
-        """Leaf key spans below 2^15: (xmax - xmin)^3 is exact in libm's pow and the device's cube."""
-        return self.shift <= 15
+        """Leaf key spans below 2^15 doubles apart: (xmax - xmin)^3 is exact in libm's pow and the device's cube.
+        Above 2^53 the keys' doubles are 2^(bits - 53) apart."""
+        top = self.base + (self.N << self.shift)
+        return self.shift - max(0, top.bit_length() - 53) <= 15
 
 
 FILL = (3, 7, 12, 5, 9, 4)
@@ -394,6 +428,15 @@ def _with_runs(p, runs):
     return Profile(p.name + "+runs", p.counts, p.shift, p.drives, runs=tuple(runs), avoids=p.avoids, sliced=p.sliced)
 
 
+def _at_base(p, log2_base):
+    return Profile(f"{p.name}@2^{log2_base}", p.counts, p.shift, p.drives, runs=p.runs, avoids=p.avoids,
+                   base=1 << log2_base)
+
+
+# profiles that also get the 2^60 base (shift 6: doubles 2^8 apart, so many leaves' first and last keys share one)
+AT_2E60 = ("solo", "alignment", "empties_tail", "empties_head")
+
+
 def _catalogue():
     base = [_table_edge(), _solo(), _fwd_walk(), _long(15, True), _long(16, False), _long(17, False), _rcp(),
             _align()] + _empties() + _sliced()
@@ -401,7 +444,15 @@ def _catalogue():
     for p in base:
         out.append(p)
         out.append(_with_runs(p, _solo_runs(p.counts) if p.name == "solo" else _auto_runs(p.counts)))
-    return out
+    # uint64 keys above 2^53, wherever the radix top reproduces the design (the injected linear top does not: the
+    # keys' doubles cross the designed boundaries)
+    high = []
+    for p in out:
+        if "radix" in p.tops(np.uint64):
+            high.append(_at_base(p, 63))
+            if p.name.split("+")[0] in AT_2E60:
+                high.append(_at_base(p, 60))
+    return out + high
 
 
 PROFILES = _catalogue()
@@ -424,9 +475,9 @@ def census_table(profiles=PROFILES):
                     if leaf in kinds:
                         table[(path, np.dtype(dt).name, leaf, dups)] = 0
     for p in profiles:
-        for dt in DTYPES:
+        for dt in p.dtypes():
             for leaf in p.leaves():
-                for path, v in census(p.counts, leaf, dt).items():
+                for path, v in p.census(leaf, dt).items():
                     table[(path, np.dtype(dt).name, leaf, bool(p.runs))] += v
     return table
 

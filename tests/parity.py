@@ -1,4 +1,7 @@
 """Shared comparison helpers: GPU result (rmi_b200.TrainedRMI) vs oracle result (oracle.OracleRMI)."""
+import math
+from fractions import Fraction
+
 import numpy as np
 
 # Tolerances, as stated in BASELINE.json's north_star and DESIGN.md:
@@ -14,6 +17,11 @@ import numpy as np
 #    the GPU sums in a fixed tree).
 COEF_RTOL = 1e-9
 STAT_RTOL = 1e-10
+# Leaf parameters fitted through ln (loglinear's ln y, lognormal's ln x): libm's ln and the device's may differ in the
+# last place or two, so these are compared by what they predict (loglinear: ln-space predictions at the leaf's ends;
+# lognormal: mean and stdev) within 2^-40 relative.  tests/test_leaf_path_census.py measures how far one ulp of ln
+# noise moves them and holds this bound to a 2^5 margin over that.
+LN_RTOL = 2.0 ** -40
 
 
 def bits(a):
@@ -117,3 +125,135 @@ def assert_same_rmi(g, o, top_exact=True, leaf_exact=True):
     assert_leaves_equal(g, o, params_exact=leaf_exact)
     if leaf_exact:
         assert_stats_equal(g, o)
+
+
+# ------------------------------------------------------------------------------------------------
+# One rule for every leaf type: parameters by leaf type, error bounds and statistics by the oracle's error pass over
+# the GPU's own tables (tests/evaluate_oracle.py)
+# ------------------------------------------------------------------------------------------------
+def _nan_or_bits_equal(a, b):
+    """Per element: bit-equal, or both NaN (NaN payloads may differ between libm and the device)."""
+    a, b = np.asarray(a, dtype=np.float64), np.asarray(b, dtype=np.float64)
+    return (bits(a) == bits(b)) | (np.isnan(a) & np.isnan(b))
+
+
+def loglinear_discrepancy(got, want, xs):
+    """Per leaf: max |u_got(x) - u_want(x)| / max(1, |u_want(x)|) over the points x of xs[j] (NaN points skipped), where
+    u(x) = alpha + beta x is the leaf's prediction in ln space, computed exactly.  0 where the parameters are bit-equal;
+    inf where they are not and a parameter is not finite, or the leaf has no points to compare at."""
+    got, want = np.asarray(got, dtype=np.float64), np.asarray(want, dtype=np.float64)
+    out = np.zeros(got.shape[0])
+    for j in np.flatnonzero(~_nan_or_bits_equal(got, want).all(axis=1)):
+        pts = [x for x in np.asarray(xs[j], dtype=np.float64) if not math.isnan(x)]
+        if not pts or not (np.isfinite(got[j]).all() and np.isfinite(want[j]).all()):
+            out[j] = math.inf
+            continue
+        ga, gb, wa, wb = (Fraction(float(v)) for v in (got[j, 0], got[j, 1], want[j, 0], want[j, 1]))
+        worst = Fraction(0)
+        for x in pts:
+            fx = Fraction(float(x))
+            uw = wa + wb * fx
+            worst = max(worst, abs(ga + gb * fx - uw) / max(Fraction(1), abs(uw)))
+        out[j] = float(worst)
+    return out
+
+
+def lognormal_discrepancy(got, want):
+    """Per leaf: max(|d mean|, |d stdev|) / max(1, |mean|); inf where `scale` differs or NaN-ness differs."""
+    got, want = np.asarray(got, dtype=np.float64), np.asarray(want, dtype=np.float64)
+    same = _nan_or_bits_equal(got, want)
+    nan_ok = (np.isnan(got) == np.isnan(want)).all(axis=1)
+    with np.errstate(invalid="ignore"):
+        d = np.maximum(np.abs(got[:, 0] - want[:, 0]), np.abs(got[:, 1] - want[:, 1])) / np.maximum(1.0, np.abs(want[:, 0]))
+    d = np.where(same[:, :2].all(axis=1), 0.0, np.nan_to_num(d, nan=0.0))
+    return np.where(same[:, 2] & nan_ok, d, np.inf)
+
+
+def assert_leaf_params(g, o, leaf, xs=None, cubic_exact=True, out_range=None):
+    """Leaf parameters of a GPU build against the oracle's, by leaf type:
+      linear, linear_spline, robust_linear, normal: bit-exact (NaN-ness equal where either is NaN);
+      cubic: bit-exact when cubic_exact; otherwise (pow(x, 3.0) in libm vs the device's double-double cube) almost
+        always bit-equal, and within COEF_RTOL where not;
+      loglinear: ln-space predictions at the points xs[j] (the leaf's first and last key) within LN_RTOL;
+      lognormal: scale bit-exact, mean and stdev within LN_RTOL * max(1, |mean|)."""
+    assert g.l1_model == o.l1_kind == leaf
+    assert g.l1_params.shape == o.l1_params.shape
+    gp, op = g.l1_params, o.l1_params
+    if leaf == "loglinear":
+        d = loglinear_discrepancy(gp, op, xs)
+        bad = np.flatnonzero(~(d <= LN_RTOL))
+        assert bad.size == 0, ("loglinear predictions differ", bad[:5], d[bad[:5]], gp[bad[:3]], op[bad[:3]])
+    elif leaf == "lognormal":
+        d = lognormal_discrepancy(gp, op)
+        bad = np.flatnonzero(~(d <= LN_RTOL))
+        assert bad.size == 0, ("lognormal parameters differ", bad[:5], d[bad[:5]], gp[bad[:3]], op[bad[:3]])
+    elif leaf == "cubic" and not cubic_exact:
+        same = (bits(gp) == bits(op)).all(axis=1)
+        assert same.mean() > 0.99
+        for j in np.flatnonzero(~same):
+            assert_coef_close("cubic", gp[j], op[j], out_range)
+    else:
+        mism = ~_nan_or_bits_equal(gp, op)
+        assert not mism.any(), ("leaf params differ", int(mism.sum()), np.argwhere(mism)[:5],
+                                gp[np.argwhere(mism)[:3, 0]], op[np.argwhere(mism)[:3, 0]])
+
+
+def assert_evaluation_equal(g, want, leaves=None):
+    """g's error bounds, counts and statistics against an error pass over g's own tables (want: evaluate_oracle's
+    Evaluated): integers exactly, the two summed statistics within STAT_RTOL (the oracle sums the leaves serially,
+    the GPU in a fixed tree).  With a leaf mask `leaves`, only those leaves' bounds and no statistics."""
+    assert np.array_equal(g.l1_counts, want.counts), "leaf key counts differ"
+    e, w = g.last_layer_max_l1s, want.errors
+    if leaves is not None:
+        e, w = e[leaves], w[leaves]
+    d = np.flatnonzero(e != w)
+    assert d.size == 0, ("leaf errors differ", d[:5], e[d[:5]], w[d[:5]])
+    if leaves is None:
+        assert (g.model_max_error, g.model_max_error_idx) == (want.max_error, want.max_error_idx)
+        assert g.model_avg_error == want.avg_error and g.model_max_log2_error == want.max_log2_error
+        for a, b in ((g.model_avg_l2_error, want.avg_l2_error), (g.model_avg_log2_error, want.avg_log2_error)):
+            assert abs(a - b) <= STAT_RTOL * max(abs(b), 1e-300), (a, b)
+
+
+STATS = ("model_max_error", "model_max_error_idx", "model_avg_error", "model_avg_l2_error", "model_avg_log2_error",
+         "model_max_log2_error")
+
+
+def assert_same_evaluation(g, e):
+    """Two GPU results with the same error bounds, counts and statistics, bit for bit (e.g. a build and
+    rmi.evaluate over its tables)."""
+    assert np.array_equal(g.last_layer_max_l1s, e.last_layer_max_l1s)
+    assert np.array_equal(g.l1_counts, e.l1_counts)
+    for f in STATS:
+        assert np.array_equal(bits(getattr(g, f)), bits(getattr(e, f))), (f, getattr(g, f), getattr(e, f))
+
+
+def _exp1(v):
+    x = 1.0 + v / 64.0
+    for _ in range(6):
+        x = x * x
+    return x
+
+
+def lognormal_stable_leaves(params, keys, counts, ulps=2):
+    """Leaves none of whose keys' prediction floor changes when ln x moves by up to `ulps` ulp either way: there the
+    device's ln and libm's give the same error bound.  Keys are assigned to leaves by `counts` (the design);
+    the prediction restates the lognormal predict (models/normal.rs:163-167) in numpy, ln by math.log."""
+    params = np.asarray(params, dtype=np.float64)
+    x = np.asarray(keys).astype(np.float64)
+    ln = np.array([math.log(v) if v > 0 else -math.inf for v in x])
+    leaf = np.repeat(np.arange(len(counts)), np.asarray(counts, dtype=np.int64))
+    mean, stdev, scale = params[leaf, 0], params[leaf, 1], params[leaf, 2]
+
+    def floor_pred(lv):
+        with np.errstate(all="ignore"):
+            p = 1.0 / (1.0 + _exp1(-1.65451 * ((np.maximum(lv, 0.0) - mean) / stdev))) * scale
+            return np.where(p > 0, np.floor(np.minimum(p, 2.0 ** 64)), 0.0)
+
+    at = floor_pred(ln)
+    flips = np.zeros(x.size, dtype=bool)
+    lo, hi = ln, ln
+    for _ in range(ulps):   # every step: exp1 is not monotone far below its range
+        lo, hi = np.nextafter(lo, -np.inf), np.nextafter(hi, np.inf)
+        flips |= (floor_pred(lo) != at) | (floor_pred(hi) != at)
+    return np.bincount(leaf[flips], minlength=len(counts)) == 0

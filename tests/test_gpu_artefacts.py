@@ -92,17 +92,6 @@ def changed_keys(name, a):
     return np.sort(rng.integers(int(a[0]), int(a[a.size // 2]), a.size // 2, dtype=np.uint64))
 
 
-def compare_with_oracle(e, want):
-    """Integer outputs exactly; the two summed statistics within parity.STAT_RTOL (the oracle sums the N leaves
-    serially, the GPU in a fixed tree)."""
-    assert np.array_equal(e.last_layer_max_l1s, want.errors)
-    assert np.array_equal(e.l1_counts, want.counts)
-    assert (e.model_max_error, e.model_max_error_idx) == (want.max_error, want.max_error_idx)
-    assert e.model_avg_error == want.avg_error and e.model_max_log2_error == want.max_log2_error
-    for a, b in ((e.model_avg_l2_error, want.avg_l2_error), (e.model_avg_log2_error, want.avg_log2_error)):
-        assert abs(a - b) <= parity.STAT_RTOL * max(abs(b), 1e-300), (a, b)
-
-
 @pytest.mark.parametrize("spec", ["linear,linear", "cubic,linear", "radix,linear", "radix18,linear", "histogram,linear",
                                   "linear,cubic", "linear,lognormal", "normal,linear"])
 @pytest.mark.parametrize("change", ["churn", "lognormal", "empties"])
@@ -125,7 +114,7 @@ def test_evaluate_on_changed_keys_equals_oracle(rmi, oracle, evo, spec, change):
     e = rmi.evaluate(g, ds_b)
     assert_same_tables(e, g)
     assert e.num_rmi_rows == b.size
-    compare_with_oracle(e, want)
+    parity.assert_evaluation_equal(e, want)
     if change == "empties":
         assert (e.l1_counts == 0).sum() > 0
 
