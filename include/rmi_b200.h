@@ -54,11 +54,14 @@ typedef enum {
 enum {
   RMI_FLAG_STATS_ONLY = 1u,     /* do not copy leaf parameters/errors to the host (optimizer use:
                                    only the statistics are consumed, optimizer.rs:163-171) */
-  RMI_FLAG_TOP_FIT_EXACT = 2u,  /* fit linear/robust_linear/loglinear/normal/lognormal TOP models
-                                   with the reference's order-dependent serial recurrence
-                                   (linear.rs:12-59) on one device thread: bit-identical to the
-                                   reference, seconds at 200 M keys.  Default is the parallel fit
-                                   (tree reduction, coefficients equal within 1e-9 relative). */
+  RMI_FLAG_TOP_FIT_EXACT = 2u,  /* fit linear/robust_linear/loglinear/normal TOP models with the
+                                   reference's order-dependent serial chain (linear.rs:12-59,
+                                   normal.rs:28-50) on one device warp, or on a host core for
+                                   linear/robust_linear/normal at 2^20 keys and more: bit-identical
+                                   to the reference, seconds at 200 M keys.  Default is the parallel
+                                   fit (tree reduction, coefficients equal within 1e-9 relative).
+                                   lognormal, cubic and the integer tops ignore the flag;
+                                   rmi_result.top_fit_exact says whether it took effect. */
   RMI_FLAG_NO_ERRORS = 4u,      /* reserved for --no-errors (main.rs:84-86); errors are still computed */
   RMI_FLAG_LEAF_COUNTS = 8u,    /* also return l1_counts (keys per leaf as the error pass counts them,
                                    two_layer.rs:207-217); not part of TrainedRMI, used by parity checks */

@@ -1145,6 +1145,9 @@ unsigned host_exact_top(const rmi_dataset* ds, int kind, uint64_t N, double* out
   if (!ok) return 0x80000000u;   // CUDA failure marker (decoded by the caller)
   return status;
 }
+inline bool serial_top_kind(int kind) {
+  return kind == M_LINEAR || kind == M_ROBUST_LINEAR || kind == M_LOGLINEAR || kind == M_NORMAL;
+}
 inline bool host_exact_kind(int kind) { return kind == M_LINEAR || kind == M_ROBUST_LINEAR || kind == M_NORMAL; }
 // exact serial tops on at least this many keys run on a host core (host_exact_top); smaller sets keep the one-warp
 // device chain (no PCIe round trip, and the CPU tests of the chain itself stay meaningful)
@@ -1257,7 +1260,9 @@ int train_typed(const rmi_dataset* ds, const ModelName& top, const ModelName& le
         R.device_time_ns = elapsed_ns(ev0, ev1);
         cudaEvent_t seq[5] = {ev0, evp[0], evp[1], evp[2], ev1};
         for (int q = 0; q < 4; ++q) R.phase_device_ns[q] = elapsed_ns(seq[q], seq[q + 1]);
-        R.top_fit_exact = (exact && !l0_over) ? 1 : 0;
+        // only the tops the flag switches to a serial chain (k_slr_exact, k_normal_exact or host_exact_top) were fitted
+        // bit for bit as the reference fits them; lognormal, cubic and the integer tops ignore the flag
+        R.top_fit_exact = (exact && !l0_over && serial_top_kind(top.kind)) ? 1 : 0;
       }
     }
   }   // arena frees (stream-ordered)
@@ -1347,7 +1352,7 @@ int train_batch_typed(const rmi_dataset* ds, const ModelName& top, const std::ve
           // the top tables stay on the device: the result holds their lengths (rmi_model_size) without them
           fill_result(boxes[k], top, *leaves[k], tables, n, N);
           boxes[k]->pub.device_time_ns = (uint64_t)((double)ms * 1e6 / (double)K);   // the batch's device time, shared out evenly
-          boxes[k]->pub.top_fit_exact = exact ? 1 : 0;
+          boxes[k]->pub.top_fit_exact = exact && serial_top_kind(top.kind) ? 1 : 0;
         }
       }
     }

@@ -178,7 +178,14 @@ __global__ void k_split(const T* __restrict__ keys, u64 n, const TopModel* __res
                         const u64* __restrict__ S, BuildAux* aux, int searched) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
   TopModel m = *top_ptr;
-  if (searched && TOP == M_LINEAR && !(m.f[1] >= 0.0)) set_status(aux, ST_NON_MONOTONE);   // slope < 0 or NaN
+  // A slope that is not >= 0 (negative, -inf or NaN) makes the predictions non-increasing in the key, so they are
+  // monotone over the sorted keys only if they are constant: the first and the last key predict the same leaf.  That
+  // happens, e.g., for a linear_spline over keys whose ends round to the same double: slope -inf, every prediction NaN,
+  // every key in leaf 0 — the reference builds that RMI, and the search above finds it.
+  if (searched && TOP == M_LINEAR && !(m.f[1] >= 0.0) && n > 0) {
+    const u64 p0 = top_predict<TOP>(m, keys[0]), p1 = top_predict<TOP>(m, keys[n - 1]);
+    if ((p0 < N - 1 ? p0 : N - 1) != (p1 < N - 1 ? p1 : N - 1)) set_status(aux, ST_NON_MONOTONE);
+  }
   if (!top_needs_bounds_check(TOP) && n > 0 && top_predict<TOP>(m, keys[n - 1]) >= N)
     set_status(aux, ST_TOP_OUT_OF_BOUNDS);
   u64 split = S[N / 2];

@@ -88,6 +88,10 @@ template <int KIND, class T> __device__ __forceinline__ u64 top_predict(const To
     unsigned prefix = (unsigned)m.ip[0], bits = (unsigned)m.table_bits;
     unsigned nb = (prefix + bits > 64u) ? 0u : 64u - (prefix + bits);
     u64 res = shr64(shr64(shl64(as_int, prefix), prefix), nb);
+    // res < 2^bits for every table RadixTable::new accepts.  Only all-equal keys (prefix 64: the masked shifts leave
+    // the key whole) give a larger radix; the reference panics there ("current_radix out of range"), and the build
+    // reports ST_RADIX_TABLE_OOB, but the kernels behind the fit still predict with the table: stay inside it.
+    if (res >> bits) res = 0;
     return (u64)__ldg(m.t32 + res);
   } else {                                 // histogram.rs:57-61: upper_bound(pivots, key) - 1 (wrapping)
     u64 val = Key<T>::as_int(key);
