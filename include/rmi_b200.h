@@ -546,9 +546,10 @@ typedef struct {
 int rmi_find_pareto_efficient_configs(const rmi_dataset* const* replicas, int num_replicas, uint64_t restrict_to,
                                       uint32_t flags, rmi_config_stats* out, uint64_t capacity, uint64_t* out_count);
 
-/* rmi_train keeps one CUDA stream set per host thread and device (created on first use, reused by later builds).
- * A worker thread that will not build again releases them with this call before it exits (the optimizer's per-replica
- * workers do); the main thread's are reclaimed at process exit. */
+/* rmi_train keeps one CUDA stream set and one device scratch buffer per host thread and device (created on first use,
+ * grown to the largest build and reused by later builds; results never live in it).  A worker thread that will not
+ * build again releases them with this call before it exits (the optimizer's per-replica workers do); the main
+ * thread's are reclaimed at process exit. */
 void rmi_thread_release(void);
 
 /* Message of the last failure on the calling thread ("" if none). */

@@ -1,10 +1,11 @@
 // api.cu — the C ABI of librmi_b200.so (include/rmi_b200.h): datasets in HBM, the
 // rmi_lib::train replacement, result marshalling, error text.
 //
-// One rmi_train call = one CUDA stream + one stream-ordered scratch arena; the dataset is
-// read-only and may be shared by concurrent calls (reference optimizer.rs:224 trains many
-// configurations on one shared RMITrainingData).  No host synchronisation happens between
-// the first kernel and the final result copy.
+// One rmi_train call = the calling thread's build stream and device scratch (BuildContext,
+// reused by that thread's later calls); the dataset is read-only and may be shared by
+// concurrent calls (reference optimizer.rs:224 trains many configurations on one shared
+// RMITrainingData).  No host synchronisation happens between the first kernel and the final
+// result copy, and a call synchronises once.
 #include <algorithm>
 #include <fcntl.h>
 #include <sys/mman.h>
@@ -944,7 +945,11 @@ int rmi_index_lookup_host(const rmi_index* idx, const void* host_queries, uint64
 namespace {
 
 // Streams / events of the sliced leaf launch (kernels.h: LeafCopyOut), created once per host
-// thread and device and reused by every rmi_train call of that thread.
+// thread and device and reused by every rmi_train call of that thread.  Slice c's stream has a
+// higher priority than slice c + 1's (below the long-leaf side stream's): the block scheduler
+// then hands out the slices' blocks in slice order, so the small slices at the end of the taper
+// are the last to finish (at equal priorities it picks among the pending slices in no fixed
+// order, and a full-size slice, whose copy is then exposed, often runs last).
 struct SliceResources {
   int device = -1;
   LeafCopyOut co;
@@ -962,9 +967,11 @@ struct SliceResources {
   LeafCopyOut* get(int dev) {
     if (device == dev) return &co;
     release();
+    int least = 0, greatest = 0;   // numerically: greatest <= least
+    cudaDeviceGetStreamPriorityRange(&least, &greatest);
     bool ok = cudaEventCreateWithFlags(&co.ev_ready, cudaEventDisableTiming) == cudaSuccess;
     for (int c = 0; c < LEAF_SLICES && ok; ++c)
-      ok = cudaStreamCreateWithFlags(&co.streams[c], cudaStreamNonBlocking) == cudaSuccess &&
+      ok = cudaStreamCreateWithPriority(&co.streams[c], cudaStreamNonBlocking, std::min(least, greatest + 1 + c)) == cudaSuccess &&
            cudaEventCreateWithFlags(&co.ev_kernel[c], cudaEventDisableTiming) == cudaSuccess &&
            cudaEventCreateWithFlags(&co.ev_copied[c], cudaEventDisableTiming) == cudaSuccess;
     device = dev;
@@ -977,13 +984,23 @@ thread_local SliceResources t_slices;
 
 // The build's own stream, the high-priority side stream of the long-leaf kernel and the timing
 // events, likewise kept per host thread and device (creating and destroying two streams and
-// seven events per call cost more host time than the launches of a small build).
+// seven events per call cost more host time than the launches of a small build).  Also the
+// device scratch of the thread's builds (BuildScratch) and the pinned slot a build's initial
+// TopModel and zeroed BuildAux are uploaded from.
 struct BuildContext {
   int device = -1;
   cudaStream_t st = nullptr, side = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr, evp[3] = {nullptr, nullptr, nullptr}, ev_fork = nullptr, ev_join = nullptr;
+  char* scratch = nullptr;   // device, scratch_cap bytes
+  size_t scratch_cap = 0;
+  char* h_init = nullptr;    // pinned, kInitBytes
+  static constexpr size_t kInitBytes = sizeof(TopModel) + sizeof(BuildAux);
+  // builds that need more scratch than this take the excess from the pool per call rather than keep it for the thread
+  static constexpr size_t kScratchKeepMax = (size_t)1 << 30;
   void release() {
     if (device < 0) return;
+    if (scratch) cudaFree(scratch);   // builds are synchronous: nothing in flight still uses it
+    if (h_init) cudaFreeHost(h_init);
     if (st) cudaStreamDestroy(st);
     if (side) cudaStreamDestroy(side);
     for (cudaEvent_t e : {ev0, ev1, evp[0], evp[1], evp[2], ev_fork, ev_join}) if (e) cudaEventDestroy(e);
@@ -999,14 +1016,61 @@ struct BuildContext {
               cudaEventCreate(&evp[0]) == cudaSuccess && cudaEventCreate(&evp[1]) == cudaSuccess &&
               cudaEventCreate(&evp[2]) == cudaSuccess &&
               cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming) == cudaSuccess &&
-              cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming) == cudaSuccess;
+              cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming) == cudaSuccess &&
+              cudaMallocHost((void**)&h_init, kInitBytes) == cudaSuccess;
     if (ok && cudaStreamCreateWithPriority(&side, cudaStreamNonBlocking, hi_prio) != cudaSuccess) { side = nullptr; cudaGetLastError(); }
     device = dev;
     if (!ok) { release(); cudaGetLastError(); return nullptr; }
     return this;
   }
+  // Issues the upload of a build's starting state on st: top to d_init[0, sizeof(TopModel)), a zeroed BuildAux after
+  // it.  One copy from page-locked memory (a pageable copy stages through the driver on the calling thread).  The slot
+  // is rewritten only by the next build of this thread, which starts after this one has synchronised.
+  void upload_init(void* d_init, const TopModel& top) {
+    memcpy(h_init, &top, sizeof(TopModel));
+    memset(h_init + sizeof(TopModel), 0, sizeof(BuildAux));
+    cudaMemcpyAsync(d_init, h_init, kInitBytes, cudaMemcpyHostToDevice, st);
+  }
+  // After a build that needed `bytes` of scratch (its stream synchronised): a larger buffer for the next ones.
+  void grow_scratch(size_t bytes) {
+    if (bytes <= scratch_cap || bytes > kScratchKeepMax) return;
+    if (scratch) cudaFreeAsync(scratch, st);
+    scratch = nullptr;
+    scratch_cap = 0;
+    if (cudaMallocAsync((void**)&scratch, bytes, st) == cudaSuccess) scratch_cap = bytes;
+    else { scratch = nullptr; cudaGetLastError(); }
+  }
 };
 thread_local BuildContext t_build_ctx;
+static_assert(sizeof(TopModel) % alignof(BuildAux) == 0, "the BuildAux after a TopModel in one upload must be aligned");
+
+// A build's device scratch, carved from its thread's BuildContext buffer: once that buffer has grown to the largest
+// build the thread runs, a build allocates and frees nothing on the device.  A build that needs more takes the excess
+// from the stream-ordered pool for itself, and once it has synchronised the buffer grows to what it needed.  Reuse is
+// safe because builds are synchronous: every stream a build uses is joined into bc->st before the build's one
+// synchronisation, so nothing of a build is in flight when the next build of the same thread carves the buffer again.
+// Results never live here: they go to pinned host buffers of their own (ResultBox).
+struct BuildScratch {
+  BuildContext* bc;
+  size_t used = 0;
+  std::vector<void*> extra;   // the excess of a build larger than the buffer
+  cudaError_t err = cudaSuccess;
+  explicit BuildScratch(BuildContext* c) : bc(c) {}
+  template <class P> P* get(size_t count) {
+    const size_t bytes = (std::max<size_t>(count * sizeof(P), 16) + 255) & ~(size_t)255;   // cudaMallocAsync's alignment
+    used += bytes;
+    if (used <= bc->scratch_cap) return (P*)(bc->scratch + used - bytes);
+    void* p = nullptr;
+    cudaError_t e = cudaMallocAsync(&p, bytes, bc->st);
+    if (e != cudaSuccess) { err = e; return nullptr; }
+    extra.push_back(p);
+    return (P*)p;
+  }
+  ~BuildScratch() {   // runs after the build's synchronisation (or before anything was launched)
+    for (void* p : extra) cudaFreeAsync(p, bc->st);
+    if (err == cudaSuccess) bc->grow_scratch(used);
+  }
+};
 
 struct Arena {   // stream-ordered scratch; everything is released when the call ends
   cudaStream_t st;
@@ -1171,13 +1235,14 @@ int train_typed(const rmi_dataset* ds, const ModelName& top, const ModelName& le
   int rc = RMI_OK;
   auto box = new ResultBox();
   {
-    Arena A(st);
+    BuildScratch A(bc);
     Launch L{st, di.num_sms};
     L.side = bc->side; L.ev_fork = bc->ev_fork; L.ev_join = bc->ev_join;
     L.d_long = A.get<u32>(LONG_LEAF_CAP + 1);
     const int ppm = leaf_params_per_model(leaf.kind);
-    TopModel* d_top = A.get<TopModel>(1);
-    BuildAux* d_aux = A.get<BuildAux>(1);
+    char* d_init = A.get<char>(BuildContext::kInitBytes);   // TopModel, then BuildAux (BuildContext::upload_init)
+    TopModel* d_top = reinterpret_cast<TopModel*>(d_init);
+    BuildAux* d_aux = reinterpret_cast<BuildAux*>(d_init + sizeof(TopModel));
     u64* d_S = A.get<u64>(N + 1);
     double* d_params = A.get<double>(N * ppm);
     u64* d_errors = A.get<u64>(N);
@@ -1209,8 +1274,7 @@ int train_typed(const rmi_dataset* ds, const ModelName& top, const ModelName& le
         if (hs == 0x80000000u) rc = fail(RMI_ERR_CUDA, "exact top fit: copying the keys back to the host failed");
         else { host_status |= hs; host_top = true; }
       }
-      cudaMemcpyAsync(d_top, &h_top, sizeof(h_top), cudaMemcpyHostToDevice, st);
-      cudaMemsetAsync(d_aux, 0, sizeof(BuildAux), st);
+      bc->upload_init(d_init, h_top);
       bool leaf_results_copied = false;
       if (!l0_over && !host_top && rc == RMI_OK)
         host_status |= fit_top_model<T>(L, keys, n, top.kind, top.table_bits, N, exact, d_top, d_aux, d_scratch, tables.t32,
@@ -1265,9 +1329,8 @@ int train_typed(const rmi_dataset* ds, const ModelName& top, const ModelName& le
         R.top_fit_exact = (exact && !l0_over && serial_top_kind(top.kind)) ? 1 : 0;
       }
     }
-  }   // arena frees (stream-ordered)
-  cudaStreamSynchronize(st);
-  if (rc != RMI_OK) { delete box; return rc; }
+  }
+  if (rc != RMI_OK) { cudaStreamSynchronize(st); delete box; return rc; }
   box->pub.build_time_ns =
       (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t_start).count();
   *out = &box->pub;
@@ -1293,14 +1356,15 @@ int train_batch_typed(const rmi_dataset* ds, const ModelName& top, const std::ve
   std::vector<ResultBox*> boxes(K, nullptr);
   int rc = RMI_OK;
   {
-    Arena A(st);
+    BuildScratch A(bc);
     Launch L{st, di.num_sms};
     L.side = bc->side; L.ev_fork = bc->ev_fork; L.ev_join = bc->ev_join;
     L.d_long = A.get<u32>(LONG_LEAF_CAP + 1);
     int max_ppm = 2;
     for (auto* lf : leaves) max_ppm = std::max(max_ppm, leaf_params_per_model(lf->kind));
-    TopModel* d_top = A.get<TopModel>(1);
-    BuildAux* d_aux0 = A.get<BuildAux>(1);
+    char* d_init = A.get<char>(BuildContext::kInitBytes);   // TopModel, then BuildAux (BuildContext::upload_init)
+    TopModel* d_top = reinterpret_cast<TopModel*>(d_init);
+    BuildAux* d_aux0 = reinterpret_cast<BuildAux*>(d_init + sizeof(TopModel));
     BuildAux* d_auxk = A.get<BuildAux>(K);
     u64* d_S = A.get<u64>(N + 1);
     double* d_params = A.get<double>(N * max_ppm);
@@ -1322,8 +1386,7 @@ int train_batch_typed(const rmi_dataset* ds, const ModelName& top, const std::ve
     else {
       const TopModel h_top = tables.initial(top);
       cudaEventRecord(bc->ev0, st);
-      cudaMemcpyAsync(d_top, &h_top, sizeof(h_top), cudaMemcpyHostToDevice, st);
-      cudaMemsetAsync(d_aux0, 0, sizeof(BuildAux), st);
+      bc->upload_init(d_init, h_top);
       const bool exact = (flags & RMI_FLAG_TOP_FIT_EXACT) != 0;
       unsigned host_status = fit_top_model<T>(L, keys, n, top.kind, top.table_bits, N, exact, d_top, d_aux0, d_scratch,
                                               tables.t32, tables.pivots, tables.radix_index, d_sample);
@@ -1357,8 +1420,7 @@ int train_batch_typed(const rmi_dataset* ds, const ModelName& top, const std::ve
       }
     }
   }
-  cudaStreamSynchronize(st);
-  if (rc != RMI_OK) { for (auto* b : boxes) delete b; return rc; }
+  if (rc != RMI_OK) { cudaStreamSynchronize(st); for (auto* b : boxes) delete b; return rc; }
   const uint64_t wall = (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t_start).count();
   for (size_t k = 0; k < K; ++k) { boxes[k]->pub.build_time_ns = wall / K; out[k] = &boxes[k]->pub; }
   return RMI_OK;
@@ -1418,10 +1480,11 @@ int evaluate_typed(const rmi_dataset* ds, const rmi_result* r, const ModelName& 
   int rc = RMI_OK;
   auto box = new ResultBox();
   {
-    Arena A(st);
+    BuildScratch A(bc);
     Launch L{st, di.num_sms};
-    TopModel* d_top = A.get<TopModel>(1);
-    BuildAux* d_aux = A.get<BuildAux>(1);
+    char* d_init = A.get<char>(BuildContext::kInitBytes);   // TopModel, then BuildAux (BuildContext::upload_init)
+    TopModel* d_top = reinterpret_cast<TopModel*>(d_init);
+    BuildAux* d_aux = reinterpret_cast<BuildAux*>(d_init + sizeof(TopModel));
     u64* d_S = A.get<u64>(N + 1);
     double* d_params = A.get<double>(N * ppm);
     u64* d_errors = A.get<u64>(N);
@@ -1440,9 +1503,8 @@ int evaluate_typed(const rmi_dataset* ds, const rmi_result* r, const ModelName& 
       rc = fail(RMI_ERR_CUDA, kPinnedFailed);
     } else {
       const TopModel h_top = tables.given(*r);
-      cudaMemcpyAsync(d_top, &h_top, sizeof(h_top), cudaMemcpyHostToDevice, st);
+      bc->upload_init(d_init, h_top);
       cudaMemcpyAsync(d_params, r->l1_params, sizeof(double) * N * ppm, cudaMemcpyHostToDevice, st);
-      cudaMemsetAsync(d_aux, 0, sizeof(BuildAux), st);
       cudaEventRecord(evp[0], st);
       // the streaming pass: the given top is not known to be monotone on these keys
       compute_leaf_bounds<T>(L, keys, n, top.kind, d_top, N, d_S, d_aux, /*allow_search=*/false, nullptr);
@@ -1470,9 +1532,8 @@ int evaluate_typed(const rmi_dataset* ds, const rmi_result* r, const ModelName& 
         for (int q = 0; q < 4; ++q) R.phase_device_ns[q] = elapsed_ns(seq[q], seq[q + 1]);
       }
     }
-  }   // arena frees (stream-ordered)
-  cudaStreamSynchronize(st);
-  if (rc != RMI_OK) { delete box; return rc; }
+  }
+  if (rc != RMI_OK) { cudaStreamSynchronize(st); delete box; return rc; }
   box->pub.build_time_ns =
       (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t_start).count();
   *out = &box->pub;

@@ -67,7 +67,8 @@ template <class T> inline Shard<T> whole_array(u64 n) {
 // after the kernel they would be fully exposed).  The bulk leaf kernel is launched as
 // LEAF_SLICES consecutive block ranges on separate streams (so a slice's tail overlaps the next
 // slice's start); each slice's parameter / error (/ count) ranges are copied to pinned host
-// memory on the slice's stream as soon as the slice is done.
+// memory on the slice's stream as soon as the slice is done.  streams[c] must have a higher
+// priority than streams[c + 1], so that the slices are scheduled, and finish, in order.
 constexpr int LEAF_SLICES = 5;
 struct LeafCopyOut {
   double* h_params = nullptr;   // N x ppm (pinned)
