@@ -377,6 +377,54 @@ typedef struct {
 } rmi_shard_lookup_stats;
 int rmi_shard_index_last_stats(const rmi_shard_index* idx, rmi_shard_lookup_stats* out);
 
+/* ---- `--bounded` lookups over a range-partitioned data set (DESIGN.md section 17) ----------------------------------
+ * r is the RMI over the K knots of a `--bounded` RMI's cache-fix spline (train_bounded, or the range-partitioned
+ * build); every rank holds its slab `local` of the u64 keys and its KNOT SLAB: the knots whose key routes to it by the
+ * rule above (the last non-empty rank whose first key is < the knot's key, or the first non-empty rank), global knots
+ * [a0, a1) with a0 = the sum of knot_counts over the earlier ranks.  `knots` (num_knots of them) is that slab with a halo:
+ * halo_before knots before it and num_knots - halo_before - (a1 - a0) after it, each at least h = 2 e_max + 2 knots or
+ * up to the end of the knots, where e_max is r's largest leaf error bound.  The knots are copied to the device.
+ *
+ * rmi_shard_index_create_bounded returns an rmi_shard_index: rmi_shard_index_route, _search, _gather, the one-call
+ * rmi_shard_index_lower_bound and rmi_shard_index_last_stats take it as they take a plain one; rmi_shard_index_predict
+ * refuses it (RMI_ERR_INVALID), because no rank holds every knot.  Refused before any device work, in this order: a
+ * null argument (RMI_ERR_INVALID); every result rmi_index_create refuses; a dataset that is not u64, line_size 0,
+ * num_knots 0; the ends-table checks of rmi_shard_index_create; a rank holding knots but no keys, more ranks holding
+ * knots than the route takes; the sum of knot_counts != r->num_rmi_rows; a slab and halo that do not fit knot_counts, a
+ * halo below h on a side; knots out of order (keys strictly increasing, offsets non-decreasing) or with offsets past
+ * the keys of all slabs; slab knots whose keys route to another rank.  local must outlive the index.
+ *
+ * lower_bound (routed by key, as for a plain index): the owner evaluates the knot RMI, (start, e), and the knot window
+ *              [lower, upper) of rmi_index_create_bounded's predict.  If the closed range [lower, upper] meets
+ *              [a0, a1], the answer knot lies in the slab or is the first knot after it and the window lies in the
+ *              halo: pos is the single-GPU one, bit for bit, and the line [pos, pos + line_size] is searched inside the
+ *              slab.  Otherwise the query is FAR: its answer knot is the window's edge, which may lie past the halo, so
+ *              the owner does not evaluate the spline; it searches its whole slab, exactly, and counts the query as a
+ *              fallback.  *d_fallbacks grows by the far queries and by the others whose line [pos, pos + line_size]
+ *              does not hold their lower bound (the single-GPU count).  Always exact.
+ * predict      collective, routed by KNOT INDEX: the querying rank evaluates the knot RMI (start, e) and sends the query
+ *              to the rank whose knot slab holds knot max(start - e, 0); that rank holds the whole window and the knot
+ *              before it, so d_pos receives rmi_index_predict of the single-GPU bounded index, bit for bit, for every
+ *              query, and d_err (may be NULL) line_size.  Phases, with the exchanges of rmi_shard_index_route's:
+ *   predict_route   as rmi_shard_index_route, grouped by knot index (five kernel launches; none for n == 0, where
+ *                   d_send_counts is zeroed)
+ *   predict_search  pos of the m received queries, in received order (one launch; none for m == 0; a rank without
+ *                   knots receives none, m > 0 there is refused)
+ *   rmi_shard_index_gather
+ * rmi_shard_index_predict_collective: the whole predict in one call over c, as rmi_shard_index_lower_bound (phase times
+ * in rmi_shard_index_last_stats, which reports the last one-call form of either kind).  The phase calls and the
+ * predict calls refuse a plain index (RMI_ERR_INVALID). */
+int rmi_shard_index_create_bounded(const rmi_result* r, const rmi_spline_point* knots, uint64_t num_knots,
+                                   uint64_t halo_before, const uint64_t* knot_counts, uint64_t line_size,
+                                   const rmi_dataset* local, const rmi_shard_ends* ends_all, int world, int rank,
+                                   rmi_shard_index** out);
+int rmi_shard_index_predict_route(const rmi_shard_index* idx, const uint64_t* d_queries, uint64_t n, uint64_t* d_send,
+                                  uint64_t* d_slot, uint64_t* d_send_counts, void* cuda_stream);
+int rmi_shard_index_predict_search(const rmi_shard_index* idx, const uint64_t* d_received, uint64_t m, uint64_t* d_pos,
+                                   void* cuda_stream);
+int rmi_shard_index_predict_collective(rmi_shard_index* idx, rmi_shard_comm* c, const uint64_t* d_queries, uint64_t n,
+                                       uint64_t* d_pos, uint64_t* d_err, void* cuda_stream);
+
 /* ---- rmi_evaluate over a range-partitioned data set (DESIGN.md section 15) ----------------------------------------
  * Every rank holds the whole model r and its own slab `local`; the result is rmi_evaluate(concatenation of the slabs, r),
  * bit for bit in every field but the timings, on every rank.  Each rank reads only its own keys: the per-key errors,

@@ -19,6 +19,7 @@
 #include <memory>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/rmi_b200.h"
@@ -2402,10 +2403,18 @@ struct rmi_shard_index {
   uint64_t first_bits[SHARD_ROUTE_MAX] = {};
   unsigned char route_rank[SHARD_ROUTE_MAX] = {};
   int route_count = 0;
-  uint64_t* h_counts = nullptr;   // world x world, pinned: the one host read of rmi_shard_index_lower_bound
+  uint64_t* h_counts = nullptr;   // world x world, pinned: the one host read of the one-call forms
   cudaEvent_t ev[SHARD_LOOKUP_EVENTS] = {};
   rmi_shard_lookup_stats last = {};
   bool ran = false;
+  // a bounded index (rmi_shard_index_create_bounded, DESIGN.md section 17): idx is the RMI over the knots (predicting
+  // over K positions), ks this rank's knot slab with its halo (ks.knots: device memory owned here); the route by knot
+  // index holds the knot base of every rank that holds knots.  Null / 0 for a plain index.
+  void* d_knots = nullptr;
+  BoundedKnotSlab ks = {};
+  uint64_t knot_first[SHARD_ROUTE_MAX] = {};
+  unsigned char knot_rank[SHARD_ROUTE_MAX] = {};
+  int knot_route_count = 0;
 };
 
 namespace {
@@ -2451,6 +2460,15 @@ int shard_lookup_search(const rmi_shard_index* si, const T* d_recv, uint64_t m, 
   const rmi_dataset* ds = idx->ds;
   if (ds->n == 0)
     return fail(RMI_ERR_INVALID, "rmi_shard_index_search: this rank holds no keys, so no query is routed to it");
+  if constexpr (std::is_same<T, u64>::value) {
+    if (si->d_knots) {
+      Launch L{st, idx->num_sms};
+      shard_bounded_search(L, idx->top, idx->leaf_kind, idx->d_records, idx->N, si->ks, (const u64*)ds->d_keys, ds->n,
+                           si->base, si->n_global, d_recv, m, d_answers, d_fallbacks, true);
+      CUDA_TRY(cudaGetLastError());
+      return RMI_OK;
+    }
+  }
   PoolScratch s{nullptr, st};
   CUDA_TRY(cudaMallocAsync(&s.p, 2 * sizeof(u64) * m, st));
   uint64_t* pos = (uint64_t*)s.p;   // m predictions, then their error bounds
@@ -2462,9 +2480,52 @@ int shard_lookup_search(const rmi_shard_index* si, const T* d_recv, uint64_t m, 
   return RMI_OK;
 }
 
-template <class T>
-int shard_lookup_one_call(rmi_shard_index* si, rmi_shard_comm* c, const T* d_q, uint64_t n, u64* d_out, u64* d_fallbacks,
-                          cudaStream_t st) {
+// The bounded index's predict route: the knot RMI's (start, e) per query, the route by knot index over lower + 1
+// (written over start in place), then the queries themselves into the route's positions (over the routed values).
+int shard_predict_route(const rmi_shard_index* si, const u64* d_q, uint64_t n, u64* d_send, u64* d_slot, u64* d_counts,
+                        cudaStream_t st) {
+  PoolScratch s{nullptr, st};
+  if (n) CUDA_TRY(cudaMallocAsync(&s.p, 2 * sizeof(u64) * n, st));
+  uint64_t* pos = (uint64_t*)s.p;   // n predictions, then their error bounds
+  if (int rc = index_launch(si->idx, d_q, n, pos, pos + n, nullptr, st, false)) return rc;
+  Launch L{st, si->idx->num_sms};
+  shard_knot_route_keys(L, (const u64*)pos, (const u64*)pos + n, n, (u64*)pos);
+  ShardRoute<u64> route;
+  memset(&route, 0, sizeof(route));
+  for (int k = 0; k < si->knot_route_count; ++k) {
+    route.first[k] = si->knot_first[k];
+    route.rank[k] = si->knot_rank[k];
+  }
+  route.count = si->knot_route_count;
+  const u64 nb = shard_route_blocks(n), W = (u64)si->world;
+  PoolScratch s2{nullptr, st};
+  if (n) CUDA_TRY(cudaMallocAsync(&s2.p, nb * W * (sizeof(u64) + sizeof(u32)), st));
+  shard_route<u64>(L, route, si->world, (const u64*)pos, n, (u32*)((u64*)s2.p + nb * W), (u64*)s2.p, d_send, d_slot,
+                   d_counts);
+  shard_scatter_queries(L, d_q, d_slot, n, d_send);
+  CUDA_TRY(cudaGetLastError());
+  return RMI_OK;
+}
+
+int shard_predict_search(const rmi_shard_index* si, const u64* d_recv, uint64_t m, u64* d_pos, cudaStream_t st) {
+  if (m == 0) return RMI_OK;
+  const rmi_index* idx = si->idx;
+  if (si->ks.a1 == si->ks.a0)
+    return fail(RMI_ERR_INVALID, "rmi_shard_index_predict_search: this rank holds no knots, so no query is routed to it");
+  Launch L{st, idx->num_sms};
+  shard_bounded_search(L, idx->top, idx->leaf_kind, idx->d_records, idx->N, si->ks, (const u64*)idx->ds->d_keys,
+                       idx->ds->n, si->base, si->n_global, d_recv, m, d_pos, nullptr, false);
+  CUDA_TRY(cudaGetLastError());
+  return RMI_OK;
+}
+
+// The one-call exchange of rmi_shard_index_lower_bound and rmi_shard_index_predict_collective: route(d_send, d_slot,
+// d_counts) groups the n queries by destination; the world x world counts are all-gathered and read once on the host;
+// the queries go to their ranks, search(d_recv, m, d_ans) answers the m received ones, the answers come back and are
+// gathered into d_out.  Events around every phase for rmi_shard_index_last_stats.
+template <class T, class Route, class Search>
+int shard_one_call(rmi_shard_index* si, rmi_shard_comm* c, uint64_t n, u64* d_out, cudaStream_t st, const char* fn,
+                   Route&& route, Search&& search) {
   const NcclApi& nc = nccl_api();
   const int W = si->world, me = si->rank;
   const size_t kb = sizeof(T);
@@ -2476,7 +2537,7 @@ int shard_lookup_one_call(rmi_shard_index* si, rmi_shard_comm* c, const T* d_q, 
   u64* d_slot = (u64*)((char*)s1.p + send_b);
   u64* d_mat = (u64*)((char*)s1.p + send_b + slot_b);
   cudaEventRecord(si->ev[0], st);
-  if (int rc = shard_lookup_route<T>(si, d_q, n, d_send, d_slot, d_mat + (size_t)me * W, st)) return rc;
+  if (int rc = route(d_send, d_slot, d_mat + (size_t)me * W)) return rc;
   cudaEventRecord(si->ev[1], st);
   NCCL_TRY(nc.AllGather(d_mat + (size_t)me * W, d_mat, W, ncclUint64, c->comm, st));
   CUDA_TRY(cudaMemcpyAsync(si->h_counts, d_mat, mat_b, cudaMemcpyDeviceToHost, st));
@@ -2490,7 +2551,7 @@ int shard_lookup_one_call(rmi_shard_index* si, rmi_shard_comm* c, const T* d_q, 
     soff[p + 1] = soff[p] + scount[p];
     roff[p + 1] = roff[p] + rcount[p];
   }
-  if (soff[W] != n) return fail(RMI_ERR_CUDA, "rmi_shard_index_lower_bound: the route's counts do not add up to the queries");
+  if (soff[W] != n) return fail(RMI_ERR_CUDA, std::string(fn) + ": the route's counts do not add up to the queries");
   const u64 m = roff[W];
   // received queries | their answers | the answers returned to this rank
   PoolScratch s2{nullptr, st};
@@ -2506,7 +2567,7 @@ int shard_lookup_one_call(rmi_shard_index* si, rmi_shard_comm* c, const T* d_q, 
   }
   NCCL_TRY(nc.GroupEnd());
   cudaEventRecord(si->ev[3], st);
-  if (int rc = shard_lookup_search<T>(si, d_recv, m, d_ans, d_fallbacks, st)) return rc;
+  if (int rc = search((const T*)d_recv, m, d_ans)) return rc;
   cudaEventRecord(si->ev[4], st);
   NCCL_TRY(nc.GroupStart());
   for (int p = 0; p < W; ++p) {
@@ -2526,21 +2587,29 @@ int shard_lookup_one_call(rmi_shard_index* si, rmi_shard_comm* c, const T* d_q, 
   return RMI_OK;
 }
 
-}  // namespace
+template <class T>
+int shard_lookup_one_call(rmi_shard_index* si, rmi_shard_comm* c, const T* d_q, uint64_t n, u64* d_out, u64* d_fallbacks,
+                          cudaStream_t st) {
+  return shard_one_call<T>(
+      si, c, n, d_out, st, "rmi_shard_index_lower_bound",
+      [&](T* d_send, u64* d_slot, u64* d_counts) { return shard_lookup_route<T>(si, d_q, n, d_send, d_slot, d_counts, st); },
+      [&](const T* d_recv, u64 m, u64* d_ans) { return shard_lookup_search<T>(si, d_recv, m, d_ans, d_fallbacks, st); });
+}
 
-extern "C" {
+// The checks of a call that takes a communicator (the one-call forms).
+int shard_check_comm(const rmi_shard_index* si, const rmi_shard_comm* c, const std::string& fn) {
+  if (c->world != si->world || c->rank != si->rank)
+    return fail(RMI_ERR_INVALID, fn + ": the communicator is rank " + std::to_string(c->rank) + " of " +
+                                     std::to_string(c->world) + ", the index rank " + std::to_string(si->rank) + " of " +
+                                     std::to_string(si->world));
+  const NcclApi& nc = nccl_api();
+  if (!nc.ok) return fail(RMI_ERR_UNSUPPORTED, nc.error);
+  return RMI_OK;
+}
 
-int rmi_shard_index_create(const rmi_result* r, const rmi_dataset* local, const rmi_shard_ends* ends_all, int world,
-                           int rank, rmi_shard_index** out) {
-  const std::string fn = "rmi_shard_index_create";
-  g_last_error.clear();
-  if (!r || !local || !ends_all || !out) return fail(RMI_ERR_INVALID, fn + ": null argument");
-  if (int rc = check_result(r, true, fn)) return rc;
-  uint64_t total = 0, base = 0;
-  if (int rc = check_slabs(fn, local, ends_all, world, rank, &base, &total)) return rc;
-  if (int rc = index_check_tables(r, total, "the slabs hold ", total, fn)) return rc;
-  rmi_index* idx = nullptr;
-  if (int rc = index_upload(r, local, total, nullptr, 0, 0, fn, &idx)) return rc;
+// The part of creating a shard index after its checks: binds the uploaded tables to the route of ends_all.
+int shard_index_make(rmi_index* idx, const rmi_shard_ends* ends_all, int world, int rank, uint64_t base, uint64_t total,
+                     const std::string& fn, rmi_shard_index** out) {
   auto* si = new rmi_shard_index();
   si->idx = idx;
   si->world = world;
@@ -2562,8 +2631,30 @@ int rmi_shard_index_create(const rmi_result* r, const rmi_dataset* local, const 
   return RMI_OK;
 }
 
+}  // namespace
+
+extern "C" {
+
+int rmi_shard_index_create(const rmi_result* r, const rmi_dataset* local, const rmi_shard_ends* ends_all, int world,
+                           int rank, rmi_shard_index** out) {
+  const std::string fn = "rmi_shard_index_create";
+  g_last_error.clear();
+  if (!r || !local || !ends_all || !out) return fail(RMI_ERR_INVALID, fn + ": null argument");
+  if (int rc = check_result(r, true, fn)) return rc;
+  uint64_t total = 0, base = 0;
+  if (int rc = check_slabs(fn, local, ends_all, world, rank, &base, &total)) return rc;
+  if (int rc = index_check_tables(r, total, "the slabs hold ", total, fn)) return rc;
+  rmi_index* idx = nullptr;
+  if (int rc = index_upload(r, local, total, nullptr, 0, 0, fn, &idx)) return rc;
+  return shard_index_make(idx, ends_all, world, rank, base, total, fn, out);
+}
+
 void rmi_shard_index_destroy(rmi_shard_index* si) {
   if (!si) return;
+  if (si->d_knots) {
+    cudaSetDevice(si->idx->ds->device);
+    cudaFree(si->d_knots);
+  }
   rmi_index_destroy(si->idx);
   if (si->h_counts) cudaFreeHost(si->h_counts);
   for (cudaEvent_t e : si->ev) if (e) cudaEventDestroy(e);
@@ -2573,6 +2664,9 @@ void rmi_shard_index_destroy(rmi_shard_index* si) {
 int rmi_shard_index_predict(const rmi_shard_index* si, const void* d_queries, uint64_t n, uint64_t* d_pos,
                             uint64_t* d_err, void* cuda_stream) {
   if (!si) return fail(RMI_ERR_INVALID, "rmi_shard_index_predict: null index");
+  if (si->d_knots)
+    return fail(RMI_ERR_INVALID, "rmi_shard_index_predict: a bounded index predicts collectively "
+                                 "(rmi_shard_index_predict_collective, or its phases)");
   if (int rc = index_check_call(si->idx, d_queries, n, d_pos, "rmi_shard_index_predict")) return rc;
   return index_launch(si->idx, d_queries, n, d_pos, d_err, nullptr, cuda_stream, false);
 }
@@ -2619,12 +2713,7 @@ int rmi_shard_index_lower_bound(rmi_shard_index* si, rmi_shard_comm* c, const vo
   g_last_error.clear();
   if (!si || !c) return fail(RMI_ERR_INVALID, std::string(fn) + ": null index or communicator");
   if (n && (!d_queries || !d_out)) return fail(RMI_ERR_INVALID, std::string(fn) + ": null query or output pointer");
-  if (c->world != si->world || c->rank != si->rank)
-    return fail(RMI_ERR_INVALID, std::string(fn) + ": the communicator is rank " + std::to_string(c->rank) + " of " +
-                                     std::to_string(c->world) + ", the index rank " + std::to_string(si->rank) + " of " +
-                                     std::to_string(si->world));
-  const NcclApi& nc = nccl_api();
-  if (!nc.ok) return fail(RMI_ERR_UNSUPPORTED, nc.error);
+  if (int rc = shard_check_comm(si, c, fn)) return rc;
   CUDA_TRY(cudaSetDevice(si->idx->ds->device));
   return with_key_type(si->idx->ds->key_type, [&](auto k) {
     using T = decltype(k);
@@ -2640,6 +2729,141 @@ int rmi_shard_index_last_stats(const rmi_shard_index* si, rmi_shard_lookup_stats
   *out = si->last;
   for (int q = 0; q + 1 < SHARD_LOOKUP_EVENTS; ++q) CUDA_TRY(cudaEventElapsedTime(&out->phase_ms[q], si->ev[q], si->ev[q + 1]));
   return RMI_OK;
+}
+
+// ---- `--bounded` lookups over a range-partitioned data set (DESIGN.md section 17) ----------------------------------
+
+int rmi_shard_index_create_bounded(const rmi_result* r, const rmi_spline_point* knots, uint64_t num_knots,
+                                   uint64_t halo_before, const uint64_t* knot_counts, uint64_t line_size,
+                                   const rmi_dataset* local, const rmi_shard_ends* ends_all, int world, int rank,
+                                   rmi_shard_index** out) {
+  const std::string fn = "rmi_shard_index_create_bounded";
+  g_last_error.clear();
+  if (!r || !knots || !knot_counts || !local || !ends_all || !out) return fail(RMI_ERR_INVALID, fn + ": null argument");
+  if (int rc = check_result(r, true, fn)) return rc;
+  if (local->key_type != RMI_KEY_U64) return fail(RMI_ERR_INVALID, fn + ": Can only construct a bounded RMI on u64 data");
+  if (line_size == 0) return fail(RMI_ERR_INVALID, fn + ": line size 0");
+  if (num_knots == 0) return fail(RMI_ERR_INVALID, fn + ": no spline knots");
+  uint64_t total = 0, base = 0;
+  if (int rc = check_slabs(fn, local, ends_all, world, rank, &base, &total)) return rc;
+  // the knot slabs: rank p holds global knots [kbase[p], kbase[p] + knot_counts[p])
+  std::vector<uint64_t> kbase(world + 1, 0);
+  int knot_ranks = 0;
+  for (int p = 0; p < world; ++p) {
+    if (knot_counts[p] && !ends_all[p].n_local)
+      return fail(RMI_ERR_INVALID, fn + ": rank " + std::to_string(p) + " holds " + std::to_string(knot_counts[p]) +
+                                       " knots and no keys (a knot goes to the rank its key routes to)");
+    knot_ranks += knot_counts[p] ? 1 : 0;
+    kbase[p + 1] = kbase[p] + knot_counts[p];
+  }
+  if (knot_ranks > SHARD_ROUTE_MAX)
+    return fail(RMI_ERR_INVALID, fn + ": more ranks hold knots than the route takes (" + std::to_string(SHARD_ROUTE_MAX) + ")");
+  const uint64_t K = kbase[world], a0 = kbase[rank], a1 = kbase[rank + 1];
+  if (int rc = index_check_tables(r, K, "the knot slabs hold ", total, fn)) return rc;
+  // the slab and its halo: halo_before knots before it, the rest after it, each at least h = 2 e_max + 2 knots (or up
+  // to the end of the knots), so that every window the lookups search lies inside (DESIGN.md section 17)
+  uint64_t e_max = 0;
+  for (uint64_t j = 0; j < r->branching_factor; ++j) e_max = std::max<uint64_t>(e_max, ((const uint64_t*)r->l1_errors)[j]);
+  const uint64_t h = e_max >= (UINT64_MAX - 2) / 2 ? UINT64_MAX : 2 * e_max + 2;
+  if (halo_before > a0 || a1 - a0 > num_knots - std::min(num_knots, halo_before) ||
+      num_knots - halo_before - (a1 - a0) > K - a1)
+    return fail(RMI_ERR_INVALID, fn + ": " + std::to_string(num_knots) + " knots with " + std::to_string(halo_before) +
+                                     " before the slab do not fit knot slab [" + std::to_string(a0) + ", " +
+                                     std::to_string(a1) + ") of " + std::to_string(K));
+  const uint64_t halo_after = num_knots - halo_before - (a1 - a0);
+  if (halo_before < std::min(h, a0) || halo_after < std::min(h, K - a1))
+    return fail(RMI_ERR_INVALID, fn + ": the halo (" + std::to_string(halo_before) + " knots before the slab, " +
+                                     std::to_string(halo_after) + " after) is below 2 x the largest leaf error + 2 = " +
+                                     std::to_string(h) + " knots on a side");
+  for (uint64_t i = 0; i < num_knots; ++i) {
+    if (knots[i].offset >= total)
+      return fail(RMI_ERR_INVALID, fn + ": knot " + std::to_string(i) + " has offset " + std::to_string(knots[i].offset) +
+                                       ", the slabs hold " + std::to_string(total) + " keys");
+    if (i && !(knots[i - 1].key < knots[i].key && knots[i - 1].offset <= knots[i].offset))
+      return fail(RMI_ERR_INVALID, fn + ": knots " + std::to_string(i - 1) + " and " + std::to_string(i) +
+                                       " are out of order (keys must increase strictly, offsets must not decrease)");
+  }
+  // the slab's knots route to this rank: above its first key (unless it is the first rank with keys), not above the
+  // next non-empty rank's first key
+  if (a1 > a0) {
+    int first_rank = 0, next = -1;
+    while (!ends_all[first_rank].n_local) ++first_rank;
+    for (int p = rank + 1; p < world && next < 0; ++p)
+      if (ends_all[p].n_local) next = p;
+    const uint64_t lo_key = knots[halo_before].key, hi_key = knots[halo_before + (a1 - a0) - 1].key;
+    if ((rank != first_rank && !(lo_key > ends_all[rank].first_key_bits)) ||
+        (next >= 0 && hi_key > ends_all[next].first_key_bits))
+      return fail(RMI_ERR_INVALID, fn + ": the knot slab holds knots whose keys route to other ranks");
+  }
+  rmi_index* idx = nullptr;
+  if (int rc = index_upload(r, local, K, nullptr, 0, 0, fn, &idx)) return rc;
+  rmi_shard_index* si = nullptr;
+  if (int rc = shard_index_make(idx, ends_all, world, rank, base, total, fn, &si)) return rc;
+  for (int p = 0; p < world; ++p) {
+    if (!knot_counts[p]) continue;
+    si->knot_first[si->knot_route_count] = kbase[p];
+    si->knot_rank[si->knot_route_count++] = (unsigned char)p;
+  }
+  cudaError_t e = cudaMalloc(&si->d_knots, sizeof(rmi_spline_point) * num_knots);
+  if (e == cudaSuccess) e = cudaMemcpy(si->d_knots, knots, sizeof(rmi_spline_point) * num_knots, cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {
+    rmi_shard_index_destroy(si);
+    return fail(RMI_ERR_CUDA, fn + ": " + cudaGetErrorString(e));
+  }
+  si->ks = BoundedKnotSlab{si->d_knots, a0 - halo_before, num_knots, K, a0, a1, line_size};
+  *out = si;
+  return RMI_OK;
+}
+
+static int shard_check_bounded(const rmi_shard_index* si, const char* fn) {
+  if (!si) return fail(RMI_ERR_INVALID, std::string(fn) + ": null index");
+  if (!si->d_knots)
+    return fail(RMI_ERR_INVALID, std::string(fn) + ": not a bounded index (a plain index predicts locally: "
+                                                   "rmi_shard_index_predict)");
+  return RMI_OK;
+}
+
+int rmi_shard_index_predict_route(const rmi_shard_index* si, const uint64_t* d_queries, uint64_t n, uint64_t* d_send,
+                                  uint64_t* d_slot, uint64_t* d_send_counts, void* cuda_stream) {
+  const char* fn = "rmi_shard_index_predict_route";
+  if (int rc = shard_check_bounded(si, fn)) return rc;
+  if (!d_send_counts) return fail(RMI_ERR_INVALID, std::string(fn) + ": null count pointer");
+  if (n && (!d_queries || !d_send || !d_slot)) return fail(RMI_ERR_INVALID, std::string(fn) + ": null query, send or slot pointer");
+  CUDA_TRY(cudaSetDevice(si->idx->ds->device));
+  return shard_predict_route(si, (const u64*)d_queries, n, (u64*)d_send, (u64*)d_slot, (u64*)d_send_counts,
+                             (cudaStream_t)cuda_stream);
+}
+
+int rmi_shard_index_predict_search(const rmi_shard_index* si, const uint64_t* d_received, uint64_t m, uint64_t* d_pos,
+                                   void* cuda_stream) {
+  const char* fn = "rmi_shard_index_predict_search";
+  if (int rc = shard_check_bounded(si, fn)) return rc;
+  if (m && (!d_received || !d_pos)) return fail(RMI_ERR_INVALID, std::string(fn) + ": null query or output pointer");
+  CUDA_TRY(cudaSetDevice(si->idx->ds->device));
+  return shard_predict_search(si, (const u64*)d_received, m, (u64*)d_pos, (cudaStream_t)cuda_stream);
+}
+
+int rmi_shard_index_predict_collective(rmi_shard_index* si, rmi_shard_comm* c, const uint64_t* d_queries, uint64_t n,
+                                       uint64_t* d_pos, uint64_t* d_err, void* cuda_stream) {
+  const char* fn = "rmi_shard_index_predict_collective";
+  g_last_error.clear();
+  if (int rc = shard_check_bounded(si, fn)) return rc;
+  if (!c) return fail(RMI_ERR_INVALID, std::string(fn) + ": null communicator");
+  if (n && (!d_queries || !d_pos)) return fail(RMI_ERR_INVALID, std::string(fn) + ": null query or output pointer");
+  if (int rc = shard_check_comm(si, c, fn)) return rc;
+  CUDA_TRY(cudaSetDevice(si->idx->ds->device));
+  const cudaStream_t st = (cudaStream_t)cuda_stream;
+  const u64* d_q = (const u64*)d_queries;
+  int rc = shard_one_call<u64>(
+      si, c, n, (u64*)d_pos, st, fn,
+      [&](u64* d_send, u64* d_slot, u64* d_counts) { return shard_predict_route(si, d_q, n, d_send, d_slot, d_counts, st); },
+      [&](const u64* d_recv, u64 m, u64* d_ans) { return shard_predict_search(si, d_recv, m, d_ans, st); });
+  if (rc == RMI_OK && d_err) {
+    Launch L{st, si->idx->num_sms};
+    shard_fill(L, si->ks.line, n, (u64*)d_err);
+    CUDA_TRY(cudaGetLastError());
+  }
+  return rc;
 }
 
 }  // extern "C"

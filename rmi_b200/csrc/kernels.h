@@ -227,6 +227,28 @@ void shard_search(const Launch& L, const T* keys, u64 n_local, u64 base, u64 n_g
 // d_out[i] = d_returned[d_slot[i]].  One launch (none for n == 0).
 void shard_gather(const Launch& L, const u64* d_slot, const u64* d_returned, u64 n, u64* d_out);
 
+// ---- `--bounded` lookups over a range-partitioned data set (kernels_shard_bounded.cu, DESIGN.md section 17) --------
+// A rank's knots: global knots [k_lo, k_lo + k_len) at `knots` ({key, offset} pairs), its own knot slab [a0, a1) among
+// them, K knots in all, line_size `line`.
+struct BoundedKnotSlab {
+  const void* knots;
+  u64 k_lo, k_len, K, a0, a1, line;
+};
+// One launch (none for m == 0).  lower_bound = true: exact global lower bounds of m queries routed to this rank by key
+// (slab keys[0, n_local) at global index base, n_local >= 1); *d_fallbacks (may be null) grows by the far queries and
+// by the others whose global line missed.  lower_bound = false: the single-GPU bounded pos of m queries routed to this
+// rank by knot index.  The RMI (d_records, N leaves, `top` by value) runs over the K knots.
+void shard_bounded_search(const Launch& L, const TopModel& top, int leaf_kind, const void* d_records, u64 N,
+                          const BoundedKnotSlab& ks, const u64* keys, u64 n_local, u64 base, u64 n_global,
+                          const u64* d_queries, u64 m, u64* d_out, u64* d_fallbacks, bool lower_bound);
+// d_out[i] = max(d_pos[i] - d_err[i], 0) + 1 (d_out may be d_pos): the value shard_route<u64> routes by knot index
+// (a route whose "first keys" are the knot bases of the ranks that hold knots).  One launch (none for n == 0).
+void shard_knot_route_keys(const Launch& L, const u64* d_pos, const u64* d_err, u64 n, u64* d_out);
+// d_send[d_slot[i]] = d_q[i].  One launch (none for n == 0).
+void shard_scatter_queries(const Launch& L, const u64* d_q, const u64* d_slot, u64 n, u64* d_send);
+// d_out[i] = value.  One launch (none for n == 0).
+void shard_fill(const Launch& L, u64 value, u64 n, u64* d_out);
+
 // ---- the `--bounded` cache-fix scan (kernels_cachefix.cu, DESIGN.md section 12) ----------------------------------
 // Key indices per speculation chunk, and how many of a chunk's speculative knots the stitch can join.
 // (DESIGN.md section 12.3 gives the sweep.)

@@ -35,26 +35,6 @@ constexpr int LOOKUP_Q = 1;
 constexpr int LOOKUP_THREADS = 128;
 constexpr int LOOKUP_MAX_BLOCKS_PER_SM = 32;   // grid cap; beyond it the blocks stride over the tiles
 
-// The packed leaf record (pack_leaf_records): parameters, then the error bound, in 16-byte vectors.
-//   32 B: {f0, f1}, {f2, err}               linear family, loglinear, normal, lognormal (f2 = 0 for 2 params)
-//   64 B: {f0, f1}, {f2, f3}, {err, 0}, pad  cubic
-template <int LEAF> struct Rec {
-  static constexpr int VECS = LEAF == M_CUBIC ? 4 : 2;   // stride in 16-byte vectors
-  static constexpr int LOADS = LEAF == M_CUBIC ? 3 : 2;  // vectors a lookup reads
-  __device__ __forceinline__ static void unpack(const ulonglong2 (&v)[LOADS], double* f, u64& err) {
-    f[0] = __longlong_as_double((long long)v[0].x);
-    f[1] = __longlong_as_double((long long)v[0].y);
-    f[2] = __longlong_as_double((long long)v[1].x);
-    if (LEAF == M_CUBIC) {
-      f[3] = __longlong_as_double((long long)v[1].y);
-      err = v[LOADS - 1].x;
-    } else {
-      f[3] = 0.0;
-      err = v[1].y;
-    }
-  }
-};
-
 template <class T, int TOP, int LEAF>
 __global__ void __launch_bounds__(LOOKUP_THREADS)
 k_lookup(const __grid_constant__ TopModel top, const ulonglong2* __restrict__ recs, const T* __restrict__ keys, u64 n,
@@ -148,11 +128,8 @@ void lookup_leaf(const Launch& L, const TopModel& top, int leaf_kind, const void
 // position, rounded down to its line (codegen.rs:410-437).  lower_bound: the answer lies in [pos, pos + line]
 // for every key of the data set (the spline's construction), so the kernel searches that window only.
 //
-// Windows of up to BOUNDED_COUNT_MAX keys are searched by loading every key independently and counting those
-// below q (no dependent probe chain); longer ones by the branchless binary search.  The keys just outside the
-// window are read only when the search ends on that edge, so a present key touches its own line alone unless its
-// lower bound is the line's first index.
-constexpr u64 BOUNDED_COUNT_MAX = 16;
+// The knot-window search and the key-line step are lookup_search.cuh's (knot_window_search, RMI_LINE_SEARCH), shared
+// with the search over a rank's slab of a range-partitioned data set (kernels_shard_bounded.cu).
 
 template <int TOP, int LEAF>
 __global__ void __launch_bounds__(LOOKUP_THREADS)
@@ -177,13 +154,7 @@ k_lookup_bounded(const __grid_constant__ TopModel top, const ulonglong2* __restr
     // knot window [lower, upper); upper saturates where start + e would pass K
     const u64 lower = e > start ? 0 : start - e;
     const u64 upper = e >= K - start ? K : start + e;
-    u64 b = lower, len = upper - lower;
-    while (len > 1) {
-      const u64 h = len >> 1;
-      b = knots[b + h].x < q ? b + h : b;
-      len -= h;
-    }
-    const u64 res = len == 1 && knots[b].x < q ? b + 1 : b;
+    const u64 res = knot_window_search(knots, lower, upper, q);
     u64 pos;
     if (res == K) {
       pos = n - 1;
@@ -200,26 +171,8 @@ k_lookup_bounded(const __grid_constant__ TopModel top, const ulonglong2* __restr
     }
     const u64 lo = pos < n ? pos : n;
     const u64 hi = line >= n - lo ? n : lo + line;
-    u64 r = lo;
-    if (line <= BOUNDED_COUNT_MAX) {
-#pragma unroll
-      for (u64 j = 0; j < BOUNDED_COUNT_MAX; ++j)
-        if (lo + j < hi) r += keys[lo + j] < q ? 1 : 0;
-    } else {
-      u64 kb = lo, klen = hi - lo;
-      while (klen > 1) {
-        const u64 h = klen >> 1;
-        kb = keys[kb + h] < q ? kb + h : kb;
-        klen -= h;
-      }
-      r = klen == 1 && keys[kb] < q ? kb + 1 : kb;
-    }
-    const bool left_ok = r > lo || lo == 0 || keys[lo - 1] < q;
-    const bool right_ok = r < hi || hi == n || !(keys[hi] < q);
-    if (!(left_ok && right_ok)) {
-      ++misses;
-      r = lookup_fallback(keys, n, q, lo, hi, left_ok);
-    }
+    u64 r;
+    RMI_LINE_SEARCH(keys, n, q, lo, hi, line, misses, r);
     __stcs(out + i, r);
   }
   if (fallbacks) {

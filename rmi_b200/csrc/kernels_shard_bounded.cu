@@ -1,0 +1,178 @@
+// kernels_shard_bounded.cu — `--bounded` lookups over a range-partitioned data set (DESIGN §17).
+//
+// Rank r holds its key slab (global keys [base, base + n_local)) and its knot slab: the knots whose key routes to r by
+// §14's rule, global knots [a0, a1), with a halo of knots on each side, global knots [k_lo, k_lo + k_len) in all.
+//
+// search   lower bounds of queries routed to r BY KEY.  The knot RMI gives (start, e) and the knot window
+//          [lower, upper) as on one GPU.  When the closed window [lower, upper] meets [a0, a1], the answer knot lies in
+//          the knot slab or is the first knot after it, and the window lies inside the halo: the single-GPU knot search
+//          and spline step over the extended knots give the single-GPU pos, bit for bit.  The key line [pos, pos + line]
+//          is shifted by -base and clamped to the slab, and searched with the single-GPU key-line step; the slab's edges
+//          confirm themselves (§14).  A "far" query, whose window misses [a0, a1], may need knots past the halo: it
+//          searches the whole slab instead, exactly, and is always counted as a fallback.  Any other query is counted
+//          when its global line [pos, pos + line] does not hold its lower bound, as on one GPU.
+// predict  pos of queries routed to r BY KNOT INDEX (the rank whose knot slab holds lower = start - e): the window and
+//          the knot before it lie inside the halo, so every pos is the single-GPU one.
+// The route by knot index reuses §14's route over the values lower + 1 (knot_route_keys), then moves the queries
+// themselves to the positions the route gave (scatter_queries).
+#include "kernels.h"
+#include "lookup_search.cuh"
+#include "spline.cuh"
+
+namespace rmi {
+
+namespace {
+
+constexpr int SB_THREADS = 128;
+constexpr int SB_MAX_BLOCKS_PER_SM = 32;
+
+template <int TOP, int LEAF>
+__global__ void __launch_bounds__(SB_THREADS)
+k_shard_bounded(const __grid_constant__ TopModel top, const ulonglong2* __restrict__ recs, u64 N,
+                const __grid_constant__ BoundedKnotSlab ks, const u64* __restrict__ keys, u64 n_local, u64 base,
+                u64 n_global, const u64* __restrict__ qs, u64 m, u64* __restrict__ out, u64* fallbacks,
+                int lower_bound) {
+  using R = Rec<LEAF>;
+  const ulonglong2* __restrict__ kext = (const ulonglong2*)ks.knots;
+  const u64 K = ks.K, line = ks.line;
+  unsigned misses = 0, local_misses = 0;
+  for (u64 i = (u64)blockIdx.x * SB_THREADS + threadIdx.x; i < m; i += (u64)gridDim.x * SB_THREADS) {
+    const u64 q = __ldcs(qs + i);
+    u64 t = top_predict<TOP>(top, q);
+    t = t < N - 1 ? t : N - 1;
+    ulonglong2 v[R::LOADS];
+#pragma unroll
+    for (int k = 0; k < R::LOADS; ++k) v[k] = __ldg(recs + t * R::VECS + k);
+    double f[4];
+    u64 e;
+    R::unpack(v, f, e);
+    u64 start = leaf_predict64<LEAF>(f, Key<u64>::as_float(q));
+    start = start < K - 1 ? start : K - 1;
+    const u64 lower = e > start ? 0 : start - e;
+    const u64 upper = e >= K - start ? K : start + e;
+    u64 r;
+    if (lower_bound && (upper < ks.a0 || lower > ks.a1)) {
+      // far: the whole slab, whose edges confirm themselves
+      RMI_LINE_SEARCH(keys, n_local, q, (u64)0, n_local, n_local, local_misses, r);
+      ++misses;
+      __stcs(out + i, base + r);
+      continue;
+    }
+    const u64 res = knot_window_search(kext, lower - ks.k_lo, upper - ks.k_lo, q) + ks.k_lo;
+    u64 pos;
+    if (res == K) {
+      pos = n_global - 1;
+    } else if (res == 0) {
+      pos = 0;
+    } else {
+      const ulonglong2 p0 = kext[res - ks.k_lo - 1], p1 = kext[res - ks.k_lo];
+      pos = cache_fix_interp(q, p0.x, p0.y, p1.x, p1.y) / line * line;
+    }
+    if (!lower_bound) {
+      __stcs(out + i, pos);
+      continue;
+    }
+    // the global line, then its part inside this slab
+    const u64 glo = pos < n_global ? pos : n_global;
+    const u64 ghi = line >= n_global - glo ? n_global : glo + line;
+    const u64 lo = glo <= base ? 0 : (glo - base < n_local ? glo - base : n_local);
+    const u64 hi = ghi <= base ? 0 : (ghi - base < n_local ? ghi - base : n_local);
+    RMI_LINE_SEARCH(keys, n_local, q, lo, hi, line, local_misses, r);
+    if (base + r < glo || base + r > ghi) ++misses;
+    __stcs(out + i, base + r);
+  }
+  if (fallbacks) {
+    misses = __reduce_add_sync(0xffffffffu, misses);
+    if ((threadIdx.x & 31) == 0 && misses) atomicAdd((unsigned long long*)fallbacks, (unsigned long long)misses);
+  }
+}
+
+template <int TOP, int LEAF>
+void launch_shard_bounded(const Launch& L, const TopModel& top, const void* recs, u64 N, const BoundedKnotSlab& ks,
+                          const u64* keys, u64 n_local, u64 base, u64 n_global, const u64* q, u64 m, u64* out,
+                          u64* fallbacks, bool lb) {
+  u64 blocks = (m + SB_THREADS - 1) / SB_THREADS;
+  const u64 cap = (u64)L.num_sms * SB_MAX_BLOCKS_PER_SM;
+  if (blocks > cap) blocks = cap;
+  k_shard_bounded<TOP, LEAF><<<(unsigned)blocks, SB_THREADS, 0, L.stream>>>(
+      top, (const ulonglong2*)recs, N, ks, keys, n_local, base, n_global, q, m, out, fallbacks, lb ? 1 : 0);
+  count_launch();
+}
+
+#define RMI_SB_ARGS recs, N, ks, keys, n_local, base, n_global, q, m, out, fallbacks, lb
+template <int TOP>
+void shard_bounded_leaf(const Launch& L, const TopModel& top, int leaf_kind, const void* recs, u64 N,
+                        const BoundedKnotSlab& ks, const u64* keys, u64 n_local, u64 base, u64 n_global, const u64* q,
+                        u64 m, u64* out, u64* fallbacks, bool lb) {
+  switch (lookup_leaf_group(leaf_kind)) {
+    case M_LINEAR: launch_shard_bounded<TOP, M_LINEAR>(L, top, RMI_SB_ARGS); break;
+    case M_CUBIC: launch_shard_bounded<TOP, M_CUBIC>(L, top, RMI_SB_ARGS); break;
+    case M_LOGLINEAR: launch_shard_bounded<TOP, M_LOGLINEAR>(L, top, RMI_SB_ARGS); break;
+    case M_NORMAL: launch_shard_bounded<TOP, M_NORMAL>(L, top, RMI_SB_ARGS); break;
+    default: launch_shard_bounded<TOP, M_LOGNORMAL>(L, top, RMI_SB_ARGS); break;
+  }
+}
+
+__global__ void __launch_bounds__(256)
+k_knot_route_keys(const u64* pos, const u64* err, u64 n, u64* out) {   // out may be pos (in place)
+  for (u64 i = (u64)blockIdx.x * 256 + threadIdx.x; i < n; i += (u64)gridDim.x * 256) {
+    const u64 p = __ldcs(pos + i), e = __ldcs(err + i);
+    __stcs(out + i, (p >= e ? p - e : 0) + 1);
+  }
+}
+
+__global__ void __launch_bounds__(256)
+k_scatter_queries(const u64* __restrict__ q, const u64* __restrict__ slot, u64 n, u64* __restrict__ send) {
+  for (u64 i = (u64)blockIdx.x * 256 + threadIdx.x; i < n; i += (u64)gridDim.x * 256)
+    send[__ldcs(slot + i)] = __ldcs(q + i);
+}
+
+__global__ void __launch_bounds__(256) k_fill(u64 v, u64 n, u64* __restrict__ out) {
+  for (u64 i = (u64)blockIdx.x * 256 + threadIdx.x; i < n; i += (u64)gridDim.x * 256) __stcs(out + i, v);
+}
+
+unsigned elementwise_blocks(const Launch& L, u64 n) {
+  u64 blocks = (n + 255) / 256;
+  const u64 cap = (u64)L.num_sms * 16;
+  return (unsigned)(blocks > cap ? cap : blocks);
+}
+
+}  // namespace
+
+void shard_bounded_search(const Launch& L, const TopModel& top, int leaf_kind, const void* recs, u64 N,
+                          const BoundedKnotSlab& ks, const u64* keys, u64 n_local, u64 base, u64 n_global, const u64* q,
+                          u64 m, u64* out, u64* fallbacks, bool lb) {
+  if (m == 0) return;
+  switch (lookup_top_group(top.kind)) {
+    case M_LINEAR: shard_bounded_leaf<M_LINEAR>(L, top, leaf_kind, RMI_SB_ARGS); break;
+    case M_CUBIC: shard_bounded_leaf<M_CUBIC>(L, top, leaf_kind, RMI_SB_ARGS); break;
+    case M_LOGLINEAR: shard_bounded_leaf<M_LOGLINEAR>(L, top, leaf_kind, RMI_SB_ARGS); break;
+    case M_NORMAL: shard_bounded_leaf<M_NORMAL>(L, top, leaf_kind, RMI_SB_ARGS); break;
+    case M_LOGNORMAL: shard_bounded_leaf<M_LOGNORMAL>(L, top, leaf_kind, RMI_SB_ARGS); break;
+    case M_RADIX: shard_bounded_leaf<M_RADIX>(L, top, leaf_kind, RMI_SB_ARGS); break;
+    case M_RADIX_TABLE: shard_bounded_leaf<M_RADIX_TABLE>(L, top, leaf_kind, RMI_SB_ARGS); break;
+    case M_BRADIX: shard_bounded_leaf<M_BRADIX>(L, top, leaf_kind, RMI_SB_ARGS); break;
+    default: shard_bounded_leaf<M_HISTOGRAM>(L, top, leaf_kind, RMI_SB_ARGS); break;
+  }
+}
+#undef RMI_SB_ARGS
+
+void shard_knot_route_keys(const Launch& L, const u64* d_pos, const u64* d_err, u64 n, u64* d_out) {
+  if (n == 0) return;
+  k_knot_route_keys<<<elementwise_blocks(L, n), 256, 0, L.stream>>>(d_pos, d_err, n, d_out);
+  count_launch();
+}
+
+void shard_scatter_queries(const Launch& L, const u64* d_q, const u64* d_slot, u64 n, u64* d_send) {
+  if (n == 0) return;
+  k_scatter_queries<<<elementwise_blocks(L, n), 256, 0, L.stream>>>(d_q, d_slot, n, d_send);
+  count_launch();
+}
+
+void shard_fill(const Launch& L, u64 value, u64 n, u64* d_out) {
+  if (n == 0) return;
+  k_fill<<<elementwise_blocks(L, n), 256, 0, L.stream>>>(value, n, d_out);
+  count_launch();
+}
+
+}  // namespace rmi

@@ -19,7 +19,8 @@ The orchestration below is engine-agnostic: `CudaShardEngine` drives librmi_b200
 CPU tests (gloo, world_size 2) plug in a numpy engine to exercise exactly this host logic.
 
 ShardedRMIIndex serves lookups over the same slabs (DESIGN.md section 14): a query goes to the rank whose slab holds
-its lower bound, is searched there, and its global answer comes back.
+its lower bound, is searched there, and its global answer comes back.  ShardedBoundedRMIIndex serves a `--bounded` RMI
+the same way (DESIGN.md section 17), with every rank holding only its slab of the spline's knots and a small halo.
 
 evaluate_sharded measures a given RMI's error bounds over the same slabs (DESIGN.md section 15): every rank streams
 only its own keys, and one all-reduce MAX of per-leaf maxima combines them.
@@ -239,6 +240,10 @@ class CudaShardEngine:
 
     def lookup_index(self, trained, ends_all: np.ndarray, world: int, rank: int) -> "CudaShardIndex":
         return CudaShardIndex(self, trained, ends_all, world, rank)
+
+    def bounded_lookup_index(self, trained, knots: np.ndarray, halo_before: int, knot_counts: list[int], line_size: int,
+                             ends_all: np.ndarray, world: int, rank: int) -> "CudaShardBoundedIndex":
+        return CudaShardBoundedIndex(self, trained, knots, halo_before, knot_counts, line_size, ends_all, world, rank)
 
     def evaluator(self, trained, ends_all: np.ndarray, world: int, rank: int) -> "CudaShardEval":
         return CudaShardEval(self, trained, ends_all, world, rank)
@@ -559,6 +564,11 @@ class CudaShardIndex:
     the current torch stream of the data's device and returns device tensors."""
 
     def __init__(self, eng: CudaShardEngine, trained, ends_all: np.ndarray, world: int, rank: int):
+        L = self._bind(eng, trained, world)
+        api._check(L.rmi_shard_index_create(api._result_ptr(trained), eng.ds._h, _ends_array(ends_all), world, rank,
+                                            C.byref(self._h)))
+
+    def _bind(self, eng: CudaShardEngine, trained, world: int):
         L = self.lib = api.load_library()
         L.rmi_shard_index_create.argtypes = [C.POINTER(api._Result), C.c_void_p, C.POINTER(_Ends), C.c_int, C.c_int,
                                              C.POINTER(C.c_void_p)]
@@ -576,8 +586,7 @@ class CudaShardIndex:
         self._ds = eng.ds            # the slab the index searches: kept alive with it
         self._trained = trained
         self._h = C.c_void_p()
-        api._check(L.rmi_shard_index_create(api._result_ptr(trained), eng.ds._h, _ends_array(ends_all), world, rank,
-                                            C.byref(self._h)))
+        return L
 
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream or None)
@@ -767,10 +776,15 @@ class ShardedRMIIndex:
         return (out, int(fb)) if return_fallbacks else out
 
     def _lower_bound_phases(self, q: torch.Tensor):
+        return self._phases(q, self.index.route, self.index.search)
+
+    def _phases(self, q: torch.Tensor, route, search):
+        """route -> count exchange -> query exchange -> search -> answer exchange -> gather, the exchanges through
+        torch.distributed.  search(received) -> (answers, fallbacks)."""
         idx, group = self.index, self.group
-        send, slot, counts = idx.route(q)
+        send, slot, counts = route(q)
         if self.world <= 1:
-            answers, fb = idx.search(send)
+            answers, fb = search(send)
             return idx.gather(slot, answers), fb
         # gloo cannot exchange device memory (one-GPU test boxes): stage through the host there
         stage = self.device.type == "cuda" and dist.get_backend(group) == "gloo"
@@ -779,7 +793,7 @@ class ShardedRMIIndex:
         dist.all_to_all_single(c_recv, c_send, group=group)
         scount, rcount = c_send.tolist(), c_recv.tolist()      # the one host read of the counts
         recv = self._exchange(send, rcount, scount, stage)
-        answers, fb = idx.search(recv)
+        answers, fb = search(recv)
         returned = self._exchange(answers, scount, rcount, stage)
         return idx.gather(slot, returned), fb
 
@@ -969,3 +983,217 @@ def train_bounded_sharded(data, model_spec: str, num_leaves: int, line_size: int
     rmi = train_sharded(kdata, model_spec, num_leaves, flags, group)
     rmi.num_data_rows = int(gather_ends(data, data.engine, group)[:, 3].astype(np.uint64).sum())
     return rmi, knots
+
+
+# ---- `--bounded` lookups over the slabs (include/rmi_b200.h rmi_shard_index_create_bounded, DESIGN.md section 17) -------
+
+def knot_halo_width(trained) -> int:
+    """h = 2 e_max + 2 knots on each side of a rank's knot slab, e_max the largest leaf error bound of the knot RMI
+    (its last_layer_max_l1s: a loaded artefact holds no statistics).  DESIGN.md section 17 gives the bound."""
+    errs = getattr(trained, "last_layer_max_l1s", None)
+    if errs is None:
+        raise api.RMIError("the knot RMI holds no error bounds (a --bounded artefact without errors cannot be served)")
+    return 2 * int(np.max(np.asarray(errs, dtype=np.uint64))) + 2
+
+
+def knot_owners(knot_keys: np.ndarray, ends_all: np.ndarray) -> np.ndarray:
+    """The rank every knot key routes to by DESIGN.md section 14's rule: the last non-empty key slab whose first key is
+    below it, or the first non-empty slab.  Pure function of the knot keys and gather_ends' table."""
+    nonempty = np.flatnonzero(ends_all[:, 3].astype(np.uint64) > 0)
+    firsts = ends_all[nonempty, 0].astype(np.uint64)
+    below = np.searchsorted(firsts, np.asarray(knot_keys, dtype=np.uint64), "left")
+    return nonempty[np.maximum(below.astype(np.int64) - 1, 0)]
+
+
+def plan_knot_halo(counts: list[int], rank: int, h: int) -> tuple[list[tuple[int, int, int, int]], list[tuple[int, int, int, int]]]:
+    """Where rank's knot halo comes from, given every rank's knot count and the halo width h.  Rank p publishes its
+    first and its last min(h, counts[p]) knots (its head and tail); the halo is global knots [max(a0 - h, 0), a0)
+    before the slab [a0, a1) and [a1, min(a1 + h, K)) after it.  Returns (before, after): pieces (src rank, side, offset,
+    count) in global order, side 0 = src's head, 1 = its tail, offset into that side.  Every knot within h of a slab
+    lies in its owner's head or tail, so the pieces cover both ranges, across any number of ranks with few or no knots."""
+    bases = [0]
+    for c in counts:
+        bases.append(bases[-1] + int(c))
+    K, a0, a1 = bases[-1], bases[rank], bases[rank + 1]
+    before, after = [], []
+    for p in range(len(counts)):
+        lo, hi, w = bases[p], bases[p + 1], min(h, int(counts[p]))
+        if p < rank:                                   # from p's tail: global [hi - w, hi)
+            g0, g1 = max(hi - w, a0 - h, 0), min(hi, a0)
+            if g1 > g0:
+                before.append((p, 1, g0 - (hi - w), g1 - g0))
+        elif p > rank:                                 # from p's head: global [lo, lo + w)
+            g0, g1 = max(lo, a1), min(lo + w, a1 + h, K)
+            if g1 > g0:
+                after.append((p, 0, g0 - lo, g1 - g0))
+    return before, after
+
+
+def _all_gather_u64(row: np.ndarray, world: int, group, dev, stage: bool) -> np.ndarray:
+    """Every rank's equal-length row of u64 words as a (world, len) array (a small all-gather; through the host under
+    gloo)."""
+    t = torch.from_numpy(np.ascontiguousarray(row, dtype=np.uint64).view(np.int64))
+    if world <= 1:
+        return np.ascontiguousarray(row, dtype=np.uint64)[None, :]
+    t = t if stage else t.to(dev)
+    out = [torch.empty_like(t) for _ in range(world)]
+    dist.all_gather(out, t, group=group)
+    return torch.stack(out).cpu().numpy().view(np.uint64)
+
+
+def _route_local_knots(local: np.ndarray, ends_all: np.ndarray, world: int, rank: int, group, dev, stage: bool):
+    """From the knot slabs cache_fix_sharded leaves (partitioned by point index), every rank's knot slab by the routing
+    rule.  The knots that route elsewhere (a few at the cuts: the minus and key points of a slab's first key, and the
+    final point when a slab is one repeated key) travel in one all-gather, padded to the most any rank sends, after one
+    of every rank's (staying, moving) counts.  Returns (this rank's slab, every rank's knot count)."""
+    dest = knot_owners(local[:, 0], ends_all) if len(local) else np.zeros(0, dtype=np.int64)
+    stay, moving, mdest = local[dest == rank], local[dest != rank], dest[dest != rank]
+    sizes = _all_gather_u64(np.array([len(stay), len(moving)], dtype=np.uint64), world, group, dev, stage)
+    counts = [int(x) for x in sizes[:, 0]]
+    width = int(sizes[:, 1].max())
+    incoming = []
+    if width:
+        row = np.zeros((width, 3), dtype=np.uint64)
+        row[: len(moving), :2] = moving
+        row[: len(moving), 2] = mdest
+        table = _all_gather_u64(row.reshape(-1), world, group, dev, stage).reshape(world, width, 3)
+        for p in range(world):
+            moved = table[p, : int(sizes[p, 1])]
+            for d in moved[:, 2]:
+                counts[int(d)] += 1
+            incoming.append(moved[moved[:, 2] == rank, :2])
+    slab = np.concatenate([stay] + incoming) if incoming else stay
+    slab = slab[np.argsort(slab[:, 0], kind="stable")]
+    return np.ascontiguousarray(slab, dtype=np.uint64).reshape(-1, 2), counts
+
+
+def _assemble_halo(slab: np.ndarray, counts: list[int], h: int, world: int, rank: int, group, dev, stage: bool):
+    """This rank's knot slab with its halo (plan_knot_halo) from one all-gather of every rank's head and tail of h
+    knots.  Returns (knots, halo_before)."""
+    w = min(h, len(slab))
+    row = np.zeros(4 * h, dtype=np.uint64)
+    row[: 2 * w] = slab[:w].reshape(-1)
+    row[2 * h: 2 * h + 2 * w] = slab[len(slab) - w:].reshape(-1)
+    table = _all_gather_u64(row, world, group, dev, stage)
+    before, after = plan_knot_halo(counts, rank, h)
+
+    def piece(src, side, off, cnt):
+        return table[src, 2 * h * side:].reshape(-1, 2)[off: off + cnt]
+
+    parts = [piece(*x) for x in before] + [slab] + [piece(*x) for x in after]
+    return np.ascontiguousarray(np.concatenate(parts), dtype=np.uint64).reshape(-1, 2), sum(x[3] for x in before)
+
+
+class CudaShardBoundedIndex(CudaShardIndex):
+    """One rank's side of ShardedBoundedRMIIndex on librmi_b200.so (rmi_shard_index_create_bounded): the route, search
+    and gather of CudaShardIndex, and the collective predict (predict_route / predict_search, or predict_native)."""
+
+    def __init__(self, eng: CudaShardEngine, trained, knots: np.ndarray, halo_before: int, knot_counts: list[int],
+                 line_size: int, ends_all: np.ndarray, world: int, rank: int):
+        L = self._bind(eng, trained, world)
+        L.rmi_shard_index_create_bounded.argtypes = [C.POINTER(api._Result), C.c_void_p, C.c_uint64, C.c_uint64,
+                                                     C.c_void_p, C.c_uint64, C.c_void_p, C.POINTER(_Ends), C.c_int,
+                                                     C.c_int, C.POINTER(C.c_void_p)]
+        L.rmi_shard_index_predict_route.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,
+                                                    C.c_void_p, C.c_void_p]
+        L.rmi_shard_index_predict_search.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]
+        L.rmi_shard_index_predict_collective.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p,
+                                                         C.c_void_p, C.c_void_p]
+        self.line_size = int(line_size)
+        k = np.ascontiguousarray(knots, dtype=np.uint64).reshape(-1, 2)
+        kc = np.ascontiguousarray(knot_counts, dtype=np.uint64)
+        api._check(L.rmi_shard_index_create_bounded(
+            api._result_ptr(trained), k.ctypes.data_as(C.c_void_p), k.shape[0], int(halo_before),
+            kc.ctypes.data_as(C.c_void_p), self.line_size, eng.ds._h, _ends_array(ends_all), world, rank,
+            C.byref(self._h)))
+
+    def predict_route(self, q: torch.Tensor):
+        send, slot, counts = torch.empty_like(q), self._u64(q.numel()), self._u64(self.world)
+        api._check(self.lib.rmi_shard_index_predict_route(self._h, q.data_ptr(), q.numel(), send.data_ptr(),
+                                                          slot.data_ptr(), counts.data_ptr(), self._stream()))
+        return send, slot, counts
+
+    def predict_search(self, recv: torch.Tensor):
+        pos = self._u64(recv.numel())
+        api._check(self.lib.rmi_shard_index_predict_search(self._h, recv.data_ptr(), recv.numel(), pos.data_ptr(),
+                                                           self._stream()))
+        return pos, 0
+
+    def predict_native(self, comm, q: torch.Tensor):
+        pos, err = self._u64(q.numel()), self._u64(q.numel())
+        api._check(self.lib.rmi_shard_index_predict_collective(self._h, comm, q.data_ptr(), q.numel(), pos.data_ptr(),
+                                                               err.data_ptr(), self._stream()))
+        return pos, err
+
+
+class ShardedBoundedRMIIndex(ShardedRMIIndex):
+    """A `--bounded` RMI served over range-partitioned uint64 keys (DESIGN.md section 17).  `trained` is the RMI over
+    the cache-fix spline's knots (from train_bounded_sharded, api.train_bounded of the whole keys, or an artefact:
+    ShardedBoundedRMIIndex.load); `data` a ShardedTrainingData of uint64 slabs; `knots` the whole (K, 2) knot array
+    (the same on every rank), or None to take each rank's knots from data.cache_fix_knots, which cache_fix_sharded
+    leaves on its device.  No rank holds every knot: rank r keeps the knots whose key routes to it and a halo of
+    h = 2 e_max + 2 knots on each side (knot_halo_width), assembled once here from one small all-gather.
+
+    lower_bound(q): collective, exact (np.searchsorted(all_keys, q, "left")), routed by key as ShardedRMIIndex's.
+    predict(q) -> (pos, err): collective (unlike ShardedRMIIndex.predict), routed by knot index; bit for bit the
+    one-GPU BoundedRMIIndex(trained, all_knots, line_size, all_keys).predict, err = line_size.  return_fallbacks and
+    native= behave as on ShardedRMIIndex.  Constructing it is collective."""
+
+    def __init__(self, trained, knots, line_size: int, data, group=None, engine=None):
+        eng = engine if engine is not None else data.engine
+        self.group = group if group is not None else getattr(data, "group", None)
+        self.rank, self.world = _world(self.group)
+        self.device = eng.device
+        self.key_type = data.key_type
+        self.line_size = int(line_size)
+        if data.key_type != api.KEY_U64:
+            raise api.RMIError("Can only construct a bounded RMI on u64 data")
+        h = knot_halo_width(trained)
+        ends_all = self.ends_all = gather_ends(data, eng, self.group)
+        if knots is not None:
+            k = np.ascontiguousarray(knots, dtype=np.uint64).reshape(-1, 2)
+            counts = np.bincount(knot_owners(k[:, 0], ends_all), minlength=self.world).tolist()
+            a0 = sum(counts[: self.rank])
+            a1 = a0 + counts[self.rank]
+            lo = max(a0 - h, 0)
+            ext, halo_before = k[lo: min(a1 + h, k.shape[0])], a0 - lo
+        else:
+            line, local = getattr(data, "cache_fix_knots", (None, None))
+            if local is None:
+                raise api.RMIError("knots=None needs the knot slabs cache_fix_sharded leaves on the data")
+            if int(line) != self.line_size:
+                raise api.RMIError(f"the knot slabs on the data are for line size {line}, not {self.line_size}")
+            stage = self.world > 1 and self.device.type == "cuda" and dist.get_backend(self.group) == "gloo"
+            local = local.cpu().numpy().view(np.uint64).reshape(-1, 2)
+            slab, counts = _route_local_knots(local, ends_all, self.world, self.rank, self.group, self.device, stage)
+            ext, halo_before = _assemble_halo(slab, counts, h, self.world, self.rank, self.group, self.device, stage)
+        self.knot_counts = [int(c) for c in counts]
+        self.index = eng.bounded_lookup_index(trained, ext, int(halo_before), self.knot_counts, self.line_size,
+                                              ends_all, self.world, self.rank)
+
+    @classmethod
+    def load(cls, namespace: str, data, out_dir: str = ".", data_dir: str = "rmi_data",
+             group=None) -> "ShardedBoundedRMIIndex":
+        """load_rmi of a generated `--bounded` artefact, served over the slabs with its whole knot array."""
+        trained, cf = api.load_rmi(namespace, out_dir, data_dir)
+        if cf is None:
+            raise api.RMIError("not a --bounded artefact: serve it with ShardedRMIIndex.load")
+        if trained.last_layer_max_l1s is None:
+            raise api.RMIError("a --bounded artefact without errors cannot be served")
+        if data.key_type != api.KEY_U64:
+            raise api.RMIError(f"the artefact's lookup takes uint64_t keys, the data holds "
+                               f"{np.dtype(_NP_OF_KEY[data.key_type])}")
+        return cls(trained, cf[1], cf[0], data, group)
+
+    def predict(self, q: torch.Tensor, native: bool | None = None):
+        """(pos, err) per query: the one-GPU bounded index's, bit for bit; collective (every rank calls it)."""
+        q = self._queries(q)
+        comm = None
+        if native is not False and isinstance(self.index, CudaShardBoundedIndex):
+            comm = native_comm(self.group, self.device, single_rank_ok=native is True)
+            if native is True and comm is None:
+                raise api.RMIError("native=True needs an NCCL process group (or a single rank) and a loadable libnccl.so.2")
+        if comm is not None:
+            return self.index.predict_native(comm, q)
+        pos, _ = self._phases(q, self.index.predict_route, self.index.predict_search)
+        return pos, torch.full_like(pos, self.line_size)
