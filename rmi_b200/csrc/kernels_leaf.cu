@@ -24,6 +24,7 @@
 // bit-identical; parallelism comes from the N independent leaves.
 #include "device_util.cuh"
 #include "kernels.h"
+#include "leaf_resid.cuh"
 #include <mutex>
 #include <type_traits>
 #include <vector>
@@ -39,6 +40,15 @@ constexpr int LEAF_THREADS = 128;
 // per SM, the more of the second read L2 still holds (DESIGN §4).  Measured on an H100 SXM (400 W limit) on the
 // headline build, k_leaf takes 1.46 ms at 5 blocks, 1.39 ms at 4, 1.26 ms at 3, 1.18 ms at 2 and 1.52 ms at 1.
 constexpr int LEAF_MIN_BLOCKS = 2;
+// Linear leaves over distinct integer keys take their forward pass from the fit's residual records (ResidRec) and
+// re-read about one chunk per leaf, so L2 reuse no longer sets their residency: on the headline build (H100 SXM, 700 W
+// limit) k_leaf takes 0.99 ms at 2 blocks and 0.86 ms at 3.  Four blocks leave room for 8 record chunks per lane, too
+// few for the headline build's 190-key leaves.
+constexpr int LEAF_MIN_BLOCKS_RESID = 3;
+template <class T, int LEAF, bool DUPS> __host__ __device__ constexpr bool leaf_resid() { return LEAF == M_LINEAR && !DUPS && !Key<T>::is_float; }
+template <class T, int LEAF, bool DUPS> __host__ __device__ constexpr int leaf_min_blocks() {
+  return leaf_resid<T, LEAF, DUPS>() ? LEAF_MIN_BLOCKS_RESID : LEAF_MIN_BLOCKS;
+}
 constexpr int RCP_TABLE = 512;   // reciprocals of the counts below this live in shared memory
 
 __device__ __forceinline__ void set_status(BuildAux* aux, unsigned bit) { atomicOr(&aux->status, bit); }
@@ -792,6 +802,60 @@ template <class T, bool CHECKED> struct RingStepND {
   __device__ __forceinline__ void step(Prepared x) { w.push_rc_nd(x, w.ring_rc()); }
   template <class I> __device__ __forceinline__ void operator()(T k, I) { step(prep(k)); }
 };
+// Residuals of a linear leaf's vector against a provisional line (leaf_resid.cuh), kept beside the fit: per item one
+// subtraction, one fused multiply-add and a min and a max, none of them on the Welford chain, and per copy-ring chunk
+// three floats in the warp's record area.  After the fit they bound every chunk's forward-pass error, and the lane
+// re-reads only the chunks that can hold the maximum (resid_max_error).
+constexpr int RESID_CAP = 16;                                // chunks per lane: 256 uint64 / 512 uint32 keys
+constexpr int RESID_WARP_BYTES = RESID_CAP * 3 * 32 * 4;    // [RESID_CAP][rmin, rmax, last t][32 lanes] floats
+struct ResidRec {
+  float* area;       // this warp's records
+  double x0, bt;     // the provisional line: vector offset j ~ bt * (x - x0)
+  double rmin, rmax, t;
+  unsigned ci;       // chunks of this lane begun
+  bool on;           // the line exists and every chunk of the lane's vector was recorded
+  __device__ __forceinline__ void key(double x, double j) {
+    t = __dadd_rn(x, -x0);
+    const double r = __fma_rn(-bt, t, j);
+    rmin = fmin(rmin, r);
+    rmax = fmax(rmax, r);
+  }
+  __device__ __forceinline__ void flush() {   // the record of the chunk begun last
+    if (ci > 0 && ci <= (unsigned)RESID_CAP) {
+      float* rec = area + (ci - 1) * 96 + (threadIdx.x & 31);
+      rec[0] = resid_f32_down(rmin);
+      rec[32] = resid_f32_up(rmax);
+      rec[64] = resid_f32_down(t);
+    }
+  }
+  __device__ __forceinline__ void chunk(bool active) {   // a lane's chunks are a prefix of the warp's
+    if (!active) return;
+    flush();
+    rmin = INFINITY; rmax = -INFINITY;
+    ++ci;
+  }
+};
+// FitStepND / RingStepND with the residual upkeep; the item's vector offset is the count before its push.
+template <class T, bool CHECKED> struct FitStepNDResid {
+  LeafWelford<CHECKED>& w;
+  ResidRec& rr;
+  typedef double Prepared;
+  typedef void ChunkHook;
+  __device__ __forceinline__ void chunk_begin(bool active) { rr.chunk(active); }
+  __device__ __forceinline__ Prepared prep(T k) const { return Key<T>::as_float(k); }
+  __device__ __forceinline__ void step(Prepared x) { const double j = w.nf; w.push_t_nd(x); rr.key(x, j); }
+  template <class I> __device__ __forceinline__ void operator()(T k, I) { step(prep(k)); }
+};
+template <class T, bool CHECKED> struct RingStepNDResid {
+  LeafWelford<CHECKED>& w;
+  ResidRec& rr;
+  typedef double Prepared;
+  typedef void ChunkHook;
+  __device__ __forceinline__ void chunk_begin(bool active) { w.ring_chunk(active); rr.chunk(active); }
+  __device__ __forceinline__ Prepared prep(T k) const { return Key<T>::as_float(k); }
+  __device__ __forceinline__ void step(Prepared x) { const double j = w.nf; w.push_rc_nd(x, w.ring_rc()); rr.key(x, j); }
+  template <class I> __device__ __forceinline__ void operator()(T k, I) { step(prep(k)); }
+};
 template <class T, bool CHECKED, bool DUPS> struct RingStepDups {
   LeafWelford<CHECKED>& w;
   ItemTracker<T, DUPS>& it;
@@ -808,10 +872,25 @@ template <class T, bool CHECKED, bool DUPS> struct RingStepDups {
 template <class T, class I, int LEAF, bool DUPS>
 __device__ __forceinline__ void fit_leaf(const T* __restrict__ keys, const Shard<T>& sh, unsigned char* wsm,
                                          const LeafRange<T, I>& r, const double* rcp, double* f, unsigned& bad,
-                                         u64 l2_policy, unsigned rcp_ring) {
+                                         u64 l2_policy, unsigned rcp_ring, ResidRec& rr) {
   const u64 n_keys = l2_policy;   // handed to every stream_pass below
   const I L = (I)(r.ve - r.vs) + (r.p_remote ? (I)1 : (I)0);
   const T kfirst = r.p_remote ? r.pkey : (L ? keys[r.vs] : T());
+  // linear leaves over distinct integer keys record residuals against the line through the vector's first and last
+  // items (ResidRec); the slope is at most L - 1, as the two doubles differ by at least 1
+  constexpr bool RESID = leaf_resid<T, LEAF, DUPS>();
+  rr.on = false;
+  if constexpr (RESID) {
+    rr.ci = 0; rr.rmin = INFINITY; rr.rmax = -INFINITY; rr.t = 0.0;
+    rr.x0 = Key<T>::as_float(kfirst);
+    const double xb = r.ve > r.vs ? Key<T>::as_float(keys[r.ve - 1]) : rr.x0;
+    rr.bt = xb > rr.x0 ? __ddiv_rn(__ull2double_rn((u64)L - 1), __dadd_rn(xb, -rr.x0)) : 0.0;
+    constexpr int KPP = 16 / (int)sizeof(T), SW = 8 * KPP;
+    const u64 rlen = r.ve > r.vs ? (u64)(r.ve - (r.vs & ~(I)(KPP - 1))) : 0;
+    rr.on = xb > rr.x0 && rlen > (u64)SW && rlen <= (u64)RESID_CAP * SW;   // 2 .. RESID_CAP chunks
+  }
+  // warps without a lane that can use the records (long or tiny leaves) skip their upkeep
+  const bool track = RESID && __any_sync(0xffffffffu, rr.on);
   const double vsd = __ull2double_rn(r.vs_global), f0d = __ull2double_rn(r.F0);
   // one pass over the vector: the remote first item (if any), then the local stream
   auto vector_pass = [&](auto&& fn) {
@@ -853,7 +932,13 @@ __device__ __forceinline__ void fit_leaf(const T* __restrict__ keys, const Shard
     };
     if (ND) w.nd_init();
     if (LEAF == M_LINEAR && all_short) {
-      if (ND) {
+      if (RESID && track) {
+        FitStepNDResid<T, CHECKED> item_nd{w, rr};
+        if (r.p_remote) item_nd(r.pkey, (I)0);   // before the first chunk: its residual is not recorded
+        stream_pass<T, I>(keys, n_keys, wsm, r.vs, r.ve, item_nd);
+        rr.flush();
+        nd_materialise(r.ve);
+      } else if (ND) {
         FitStepND<T, CHECKED> item_nd{w};
         if (r.p_remote) item_nd(r.pkey, (I)0);
         stream_pass<T, I>(keys, n_keys, wsm, r.vs, r.ve, item_nd);
@@ -872,7 +957,16 @@ __device__ __forceinline__ void fit_leaf(const T* __restrict__ keys, const Shard
     const bool ring_ok = LEAF == M_LINEAR && !__any_sync(0xffffffffu, (u64)L >= (1ull << 28));
     if (ring_ok) {
       w.ring_begin(rcp_ring);
-      if (ND) {
+      if (RESID && track) {
+        RingStepNDResid<T, CHECKED> item_r{w, rr};
+        if (r.p_remote) item_r(r.pkey, (I)0);
+        stream_pass<T, I, RingStepNDResid<T, CHECKED>&, true>(keys, n_keys, wsm, r.vs, r.ve, item_r, &solo_lane, &solo_at);
+        w.ring_end();
+        rr.flush();
+        const bool solo = solo_lane == (int)(threadIdx.x & 31);
+        rr.on = rr.on && !solo;   // the solo chain finishes this lane's vector without records
+        nd_materialise(solo ? solo_at : r.ve);
+      } else if (ND) {
         RingStepND<T, CHECKED> item_r{w};
         if (r.p_remote) item_r(r.pkey, (I)0);
         stream_pass<T, I, RingStepND<T, CHECKED>&, true>(keys, n_keys, wsm, r.vs, r.ve, item_r, &solo_lane, &solo_at);
@@ -885,6 +979,7 @@ __device__ __forceinline__ void fit_leaf(const T* __restrict__ keys, const Shard
         w.ring_end();
       }
     } else if (ND) {
+      rr.on = false;   // vectors of 2^28 items and more: no records
       auto item_nd = [&](T k, I) { w.push_nd(Key<T>::as_float(k)); };
       if (r.p_remote) item_nd(r.pkey, (I)0);
       stream_pass<T, I, decltype(item_nd)&, true>(keys, n_keys, wsm, r.vs, r.ve, item_nd, &solo_lane, &solo_at);
@@ -1075,6 +1170,64 @@ __device__ __forceinline__ I leaf_predict_clamped(const double* f, double x, I n
   if (sizeof(I) == 4) v = (I)__double2uint_rd(p); else v = (I)__double2ull_rd(p);
   if (NANCHECK) v = p != p ? (I)0 : v;
   return v < n ? v : n;
+}
+
+// Forward pass of one lane's linear leaf from its fit's chunk records (ResidRec): max |pred - offset| over the keys
+// [lo, hi), which the lane's vector chunks (from the 16-byte aligned index a, SW keys each) cover.  Every chunk gets an
+// upper bound on its error (resid_chunk_bound_f); the lane then evaluates, exactly as the full forward pass does, the
+// chunk with the largest bound and then only chunks whose bound exceeds the maximum found so far.  A chunk is skipped
+// only when a key actually evaluated attains an error at least as large as any the chunk can hold, so the result is
+// the full pass's.  Per lane, no warp synchronisation.
+template <class T, class I>
+__device__ __forceinline__ I resid_max_error(const T* __restrict__ keys, float* area, u32 nch, I a, I lo, I hi,
+                                             const double* f, const ResidRec& rr, double F0, I nI, I baseI) {
+  constexpr int KPP = 16 / (int)sizeof(T), SW = 8 * KPP;
+  float* rec = area + (threadIdx.x & 31);
+  const ResidLeaf lf = resid_leaf(f[0], f[1], rr.x0, rr.bt, F0);
+  float tl_prev = 0.0f;
+  for (u32 c = 0; c < nch; ++c) {   // each chunk's bound replaces its rmin
+    const float tl = rec[c * 96 + 64];
+    rec[c * 96] = resid_f32_up(resid_chunk_bound_f(lf, tl_prev, tl, rec[c * 96], rec[c * 96 + 32]));
+    tl_prev = tl;
+  }
+  I max_err = 0;
+  for (;;) {
+    float best = -1.0f;
+    u32 bc = 0;
+    for (u32 c = 0; c < nch; ++c) {
+      const float u = rec[c * 96];
+      if (u > best) { best = u; bc = c; }
+    }
+    if (!((double)best > __ull2double_rd((u64)max_err))) break;
+    rec[bc * 96] = -1.0f;
+    const I s0 = a + (I)bc * (I)SW;
+    const I s = s0 > lo ? s0 : lo, e = (I)(s0 + (I)SW) < hi ? (I)(s0 + (I)SW) : hi;
+    uint4 v[8];
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {   // the chunk's pieces that hold keys of [s, e), all loads in flight at once
+      const I p = s0 + (I)(q * KPP);
+      if (p + (I)KPP > s && p < e) v[q] = __ldg(reinterpret_cast<const uint4*>(keys + p));
+    }
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      const I p = s0 + (I)(q * KPP);
+      if (!(p + (I)KPP > s && p < e)) continue;
+      const unsigned w[4] = {v[q].x, v[q].y, v[q].z, v[q].w};
+#pragma unroll
+      for (int t = 0; t < KPP; ++t) {
+        const I i = p + (I)t;
+        if (i < s || i >= e) continue;
+        T k;
+        if constexpr (sizeof(T) == 8) k = (T)(((u64)w[2 * t + 1] << 32) | w[2 * t]);
+        else k = (T)w[t];
+        const I Fi = (I)(i + baseI);
+        const I pred = leaf_predict_clamped<M_LINEAR, I, false>(f, Key<T>::as_float(k), nI);
+        const I err = pred > Fi ? pred - Fi : Fi - pred;
+        max_err = err > max_err ? err : max_err;
+      }
+    }
+  }
+  return max_err;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1300,17 +1453,21 @@ k_find_long(const Shard<T> sh, u64 N, const u64* __restrict__ S, u32* __restrict
 
 constexpr int RCP_RING_BYTES = 64 * 8;   // per warp (LeafWelford::ring), 512-byte aligned: one extra ring of slack per block
 constexpr size_t SM_SMEM_BYTES = 228 * 1024;   // an H100 SM's shared memory; the runtime reserves 1 KB of it per block
-// What a block uses, raised so that LEAF_MIN_BLOCKS + 1 blocks do not fit on an SM.
-constexpr size_t leaf_smem_bytes() {
+// What a block uses, raised so that blocks + 1 of them do not fit on an SM.
+constexpr size_t leaf_smem_bytes(int blocks) {
   constexpr size_t used = (size_t)RCP_TABLE * sizeof(double) + (size_t)(LEAF_THREADS / 32) * WARP_STREAM_BYTES +
-                          (size_t)(LEAF_THREADS / 32 + 1) * RCP_RING_BYTES;
-  constexpr size_t cap = SM_SMEM_BYTES / (LEAF_MIN_BLOCKS + 1) - 1024 + 16;
+                          (size_t)(LEAF_THREADS / 32 + 1) * RCP_RING_BYTES + (size_t)(LEAF_THREADS / 32) * RESID_WARP_BYTES;
+  const size_t cap = SM_SMEM_BYTES / (blocks + 1) - 1024 + 16;
   return used > cap ? used : cap;
 }
-static_assert(LEAF_MIN_BLOCKS * (leaf_smem_bytes() + 1024) <= SM_SMEM_BYTES, "LEAF_MIN_BLOCKS blocks must fit an SM");
+static_assert(LEAF_MIN_BLOCKS * (leaf_smem_bytes(LEAF_MIN_BLOCKS) + 1024) <= SM_SMEM_BYTES, "LEAF_MIN_BLOCKS blocks must fit an SM");
+static_assert(LEAF_MIN_BLOCKS_RESID * (leaf_smem_bytes(LEAF_MIN_BLOCKS_RESID) + 1024) <= SM_SMEM_BYTES,
+              "LEAF_MIN_BLOCKS_RESID blocks must fit an SM");
+static_assert((LEAF_MIN_BLOCKS_RESID + 1) * (leaf_smem_bytes(LEAF_MIN_BLOCKS_RESID) + 1024) > SM_SMEM_BYTES,
+              "one block more than LEAF_MIN_BLOCKS_RESID must not fit an SM");
 
 template <class T, class I, int LEAF, bool DUPS>
-__global__ void __launch_bounds__(LEAF_THREADS, LEAF_MIN_BLOCKS)
+__global__ void __launch_bounds__(LEAF_THREADS, (leaf_min_blocks<T, LEAF, DUPS>()))
 k_leaf(const T* __restrict__ keys, const Shard<T> sh, u64 N, const u64* __restrict__ S, BuildAux* aux,
        double* __restrict__ params, u64* __restrict__ errors, u64* __restrict__ counts,
        const u32* __restrict__ long_list, int mode_word, u32 block_offset, u32 total_blocks, u32 group_base) {
@@ -1404,7 +1561,11 @@ k_leaf(const T* __restrict__ keys, const Shard<T> sh, u64 N, const u64* __restri
   const unsigned rings0 = (unsigned)__cvta_generic_to_shared(smem_raw + (size_t)RCP_TABLE * sizeof(double) +
                                                              (size_t)(blockDim.x >> 5) * WARP_STREAM_BYTES);
   const unsigned rcp_ring = ((rings0 + (unsigned)RCP_RING_BYTES - 1u) & ~((unsigned)RCP_RING_BYTES - 1u)) + (threadIdx.x >> 5) * (unsigned)RCP_RING_BYTES;
-  fit_leaf<T, I, LEAF, DUPS>(keys, sh, wsm, r, s_rcp, f, bad, l2_policy_of((mode_word >> 4) & 3), rcp_ring);
+  // the warp's residual records: behind the reciprocal rings (and their one ring of slack)
+  ResidRec rr;
+  rr.area = reinterpret_cast<float*>(smem_raw + (size_t)RCP_TABLE * sizeof(double) + (size_t)(blockDim.x >> 5) * WARP_STREAM_BYTES +
+                                     (size_t)((blockDim.x >> 5) + 1) * RCP_RING_BYTES + (size_t)(threadIdx.x >> 5) * RESID_WARP_BYTES);
+  fit_leaf<T, I, LEAF, DUPS>(keys, sh, wsm, r, s_rcp, f, bad, l2_policy_of((mode_word >> 4) & 3), rcp_ring, rr);
 
   // two_layer.rs:186-197: empty leaves (lower-bound-correction sense) except the last
   const u64 next_idx = g_hi;                                        // lb.next_index(j) = S[j+1]
@@ -1441,9 +1602,22 @@ k_leaf(const T* __restrict__ keys, const Shard<T> sh, u64 N, const u64* __restri
   // With ~1500-key vectors this wins for cubic leaves and loses slightly for linear ones — so only where the
   // evaluation is the longer part of a step.
   const bool long_fwd = is_long && (__popc(long_mask) <= 4 || (LEAF == M_CUBIC && __popc(long_mask) >= 28));
+  // Linear leaves over distinct integer keys whose fit recorded every chunk of a vector that covers the leaf's keys
+  // (at least two chunks, at most RESID_CAP) take their maximum from the records and the few chunks they point at
+  // (resid_max_error) instead of walking the leaf again.  The other lanes keep the full pass below.
+  bool resid_on = false;
+  if constexpr (leaf_resid<T, LEAF, DUPS>()) {
+    constexpr int KPP = 16 / (int)sizeof(T), SW = 8 * KPP;
+    const I ra = r.vs & ~(I)(KPP - 1);
+    const u64 nch = r.ve > r.vs ? ((u64)(r.ve - ra) + SW - 1) / SW : 0;
+    resid_on = rr.on && live && !long_fwd && r.hi > r.lo && r.vs <= r.lo && r.hi <= r.ve && nch >= 2 &&
+               nch <= (u64)RESID_CAP;
+    if (resid_on)
+      max_err = resid_max_error<T, I>(keys, rr.area, (u32)nch, ra, r.lo, r.hi, f, rr, __ull2double_rn(r.vs_global), nI, baseI);
+  }
   {
     const u64 pol_fwd = l2_policy_of((mode_word >> 6) & 3);
-    const I fwd_hi = long_fwd ? r.lo : r.hi;
+    const I fwd_hi = (long_fwd || resid_on) ? r.lo : r.hi;
     T pk = (live && g_lo == 0 && g_hi > 0) ? keys[0] : prev_key;
     I F = (I)g_lo, run = 0;
     if (DUPS) {
@@ -1747,7 +1921,12 @@ void launch_leaf_inst(const Launch& L, const T* keys, const Shard<T>& sh, u64 N,
   const u64 G0 = win_lo / LEAF_THREADS, G1 = win_hi > win_lo ? (win_hi + LEAF_THREADS - 1) / LEAF_THREADS : G0;
   const u64 blocks = G1 - G0;
   const u32 gbase = (u32)G0;
-  const size_t smem = leaf_smem_bytes();
+  // The record-keeping instantiations run at LEAF_MIN_BLOCKS_RESID blocks per SM when the mean leaf fits the records
+  // (from 2 to RESID_CAP - 2 chunks); where most lanes take the full forward pass, the re-read wants LEAF_MIN_BLOCKS.
+  constexpr u64 SW = 8 * (16 / sizeof(T));
+  const u64 mean_keys = N ? sh.n_global / N : 0;
+  const bool resid_blocks = leaf_resid<T, LEAF, DUPS>() && mean_keys >= 2 * SW && mean_keys <= (u64)(RESID_CAP - 2) * SW;
+  const size_t smem = leaf_smem_bytes(resid_blocks ? LEAF_MIN_BLOCKS_RESID : LEAF_MIN_BLOCKS);
   // L2 eviction priority of the key copies: fit pass (bits 4-5), forward pass (bits 6-7);
   // 0 normal, 1 evict_first, 2 evict_last.  Keep what the fit pass read, release it after the re-read.
   constexpr int L2_MODE = (2 << 4) | (1 << 6);
