@@ -244,8 +244,9 @@ int rmi_index_lookup_host(const rmi_index* idx, const void* host_queries, uint64
  *     RMI_PHASE_STATS, rmi_shard_finish()
  * All phases are enqueued on the caller's CUDA stream and do not synchronise.  The result is
  * identical on every rank and equal to a single-GPU build of the concatenated array (same
- * tolerance rules).  Offered for the top models linear, robust_linear, linear_spline, cubic,
- * normal, lognormal, radix, radix8..28 and histogram (bradix and loglinear are single-GPU only). */
+ * tolerance rules).  Offered for every top model: linear, robust_linear, linear_spline, cubic,
+ * loglinear, normal, lognormal, radix, radix8..28, bradix and histogram (RMI_FLAG_TOP_FIT_EXACT, a
+ * serial chain, is single-GPU only). */
 typedef struct {          /* what a rank publishes about its slab (host struct) */
   uint64_t first_key_bits, last_key_bits;  /* raw key bits (u32 zero-extended, f64 bit pattern) */
   uint64_t last_run_start;                 /* local index of the first key equal to the last key */
@@ -267,19 +268,18 @@ enum { RMI_PHASE_TOP_LOCAL = 0, RMI_PHASE_TOP_FINISH = 1, RMI_PHASE_BOUNDS = 2, 
        RMI_PHASE_LEAF = 4, RMI_PHASE_STATS = 5, RMI_PHASE_TOP_MID = 6, RMI_NUM_PHASES = 7 };
 
 /* Which collectives the top-model fit of a range-partitioned build needs (the host issues them):
- *   -1  this top model is not offered for range-partitioned builds
+ *   -1  this top model is not offered for range-partitioned builds (no model name gives -1 today but unknown ones)
  *    0  none:  TOP_LOCAL, TOP_FINISH                                   (linear_spline, radix:
  *       O(1) functions of the global end keys, cubic_spline.rs / radix.rs need no pass)
- *    1  TOP_LOCAL -> all-reduce SUM of sums[0,8) as f64 -> TOP_FINISH  (linear, robust_linear)
+ *    1  TOP_LOCAL -> all-reduce SUM of sums[0,8) as f64 -> TOP_FINISH  (linear, robust_linear, loglinear)
  *    2  TOP_LOCAL -> SUM f64 sums[0,8) -> TOP_MID -> SUM f64 sums[0,8) -> TOP_FINISH
  *                                                                       (normal, lognormal)
  *    3  TOP_LOCAL -> all-reduce MIN of sums[8,12) as SIGNED 64-bit integers -> TOP_MID
  *                 -> SUM f64 sums[0,8) -> TOP_FINISH                    (cubic)
- *    4  TOP_LOCAL -> all-reduce MAX of the top model's table (2^bits u32 hints of a radix table, or the u64 pivots
- *                 of a histogram; every entry has one writer, the others hold 0) -> TOP_FINISH
- *                                                                       (radix8..28, histogram)
- *       rmi_shard_train merges the table itself; the host has no handle on it, so the host-driven phases cannot run
- *       these tops over more than one rank. */
+ *    4  TOP_LOCAL -> all-reduce of the top model's table, as rmi_shard_top_table describes it -> TOP_FINISH
+ *                 radix8..28: MAX of the 2^bits u32 hints; histogram: MAX of the u64 pivots (every entry has one
+ *                 writer, the others hold 0); bradix: SUM, wrapping mod 2^32, of the 4 x N u32 per-bin key counts
+ *                 of its four candidates (every rank counts its own keys) */
 int rmi_shard_top_rounds(const char* top_model_name);
 
 /* rmi_shard_build_create: one rank's build object.  ends_all holds every rank's rmi_shard_ends (rmi_shard_ends_get,
@@ -297,6 +297,20 @@ int rmi_shard_build_create(const rmi_dataset* local, const rmi_shard_ends* ends_
                            const rmi_shard_buffers* buffers, void* cuda_stream, rmi_shard_build** out);
 int rmi_shard_phase(rmi_shard_build* b, int phase);
 int rmi_shard_set_halo(rmi_shard_build* b, uint64_t halo_keys);
+
+/* The table a code-4 top model (rmi_shard_top_rounds) merges between RMI_PHASE_TOP_LOCAL and RMI_PHASE_TOP_FINISH:
+ * `entries` entries of `entry_bytes` bytes (4: u32, 8: u64) at the device pointer `table`, which the host-driven flow
+ * all-reduces in place with `op` over the ranks.  The entries are unsigned: a host that reduces them as signed
+ * integers must keep the unsigned order (MAX) and the wrap-around mod 2^32 (SUM).  entries == 0 for the top models
+ * without a table.  The pointer stays valid for the build object's life. */
+enum { RMI_TABLE_REDUCE_MAX = 0, RMI_TABLE_REDUCE_SUM = 1 };
+typedef struct {
+  void* table;
+  uint64_t entries;
+  uint32_t entry_bytes;
+  uint32_t op;            /* RMI_TABLE_REDUCE_* */
+} rmi_shard_top_table_info;
+int rmi_shard_top_table(const rmi_shard_build* b, rmi_shard_top_table_info* out);
 int rmi_shard_finish(rmi_shard_build* b, uint32_t flags, rmi_result** out);
 void rmi_shard_build_destroy(rmi_shard_build* b);
 uint32_t rmi_params_per_model(const char* leaf_model_name);

@@ -80,11 +80,11 @@ struct ModelName { const char* name; int kind; int table_bits; int fparams, ipar
 const ModelName kModels[] = {   // reference train/mod.rs:37-54
     {"linear", M_LINEAR, 0, 2, 0, false, 1},          {"robust_linear", M_ROBUST_LINEAR, 0, 2, 0, false, 1},
     {"linear_spline", M_LINEAR_SPLINE, 0, 2, 0, false, 0}, {"cubic", M_CUBIC, 0, 4, 0, false, 3},
-    {"loglinear", M_LOGLINEAR, 0, 2, 0, false, -1},   {"normal", M_NORMAL, 0, 3, 0, false, 2},
+    {"loglinear", M_LOGLINEAR, 0, 2, 0, false, 1},   {"normal", M_NORMAL, 0, 3, 0, false, 2},
     {"lognormal", M_LOGNORMAL, 0, 3, 0, false, 2},    {"radix", M_RADIX, 0, 0, 2, true, 0},
     {"radix8", M_RADIX_TABLE, 8, 0, 1, false, 4},     {"radix18", M_RADIX_TABLE, 18, 0, 1, false, 4},
     {"radix22", M_RADIX_TABLE, 22, 0, 1, false, 4},   {"radix26", M_RADIX_TABLE, 26, 0, 1, false, 4},
-    {"radix28", M_RADIX_TABLE, 28, 0, 1, false, 4},   {"bradix", M_BRADIX, 0, 0, 3, true, -1},
+    {"radix28", M_RADIX_TABLE, 28, 0, 1, false, 4},   {"bradix", M_BRADIX, 0, 0, 3, true, 4},
     {"histogram", M_HISTOGRAM, 0, 0, 1, true, 4}};
 
 const ModelName* find_model(const std::string& s) {
@@ -328,13 +328,16 @@ void* device_alloc(size_t bytes) {
   return cudaMalloc(&p, bytes) == cudaSuccess ? p : nullptr;
 }
 
-// The device tables of a table top: radix8..28's hint table, the histogram's pivots and, in a build, its radix index.
+// The device tables of a table top: radix8..28's hint table, the histogram's pivots and, in a build, its radix index;
+// in a range-partitioned build, bradix's per-bin counts (not part of any result).
 struct TopTables {
   u32* t32 = nullptr;
   u64* pivots = nullptr;        // hist_bins (+ 1 in a build)
   u64* radix_index = nullptr;   // ri_len; a build's output only: no kernel reads it through TopModel
+  u32* bradix_counts = nullptr; // bradix_len = 4 x N: every candidate's count of keys per bin (shard_bradix_count)
   u64 t32_len = 0, ri_len = 0;
   u64 hist_bins = 0, hist_ipb = 0;
+  u64 bradix_len = 0;
 
   // alloc(bytes) returns device memory or null; false if an allocation failed
   template <class Alloc> bool allocate(const ModelName& top, uint64_t n, uint64_t N, Alloc&& alloc) {
@@ -351,6 +354,14 @@ struct TopTables {
       return pivots && radix_index;
     }
     return true;
+  }
+
+  // A range-partitioned build's bradix counts (the single-GPU fit takes bin boundaries from its scratch instead).
+  template <class Alloc> bool allocate_shard_counts(const ModelName& top, uint64_t N, Alloc&& alloc) {
+    if (top.kind != M_BRADIX) return true;
+    bradix_len = 4 * (u64)N;
+    bradix_counts = (u32*)alloc(sizeof(u32) * bradix_len);
+    return bradix_counts != nullptr;
   }
 
   // The tables of a given result's top model (check_result passed), allocated with alloc and copied on st: the first
@@ -392,6 +403,7 @@ struct TopTables {
     cudaFree(t32);
     cudaFree(pivots);
     cudaFree(radix_index);
+    cudaFree(bradix_counts);
   }
 
   // The TopModel a build starts from; f: nf injected top parameters, or null.
@@ -1803,7 +1815,8 @@ template <class T> int shard_phase_typed(rmi_shard_build* b, int phase) {
       }
       if (b->top->kind == M_HISTOGRAM && (tt.hist_bins == 0 || tt.hist_ipb < 1)) b->host_status |= ST_HIST_BINS;   // histogram.rs:25-27
       b->host_status |= shard_top_local<T>(L, keys, sh, b->top->kind, b->N, b->lay.pivot_x, b->lay.pivot_y, first_key,
-                                           last_key, b->d_scratch, (double*)b->buf.sums);
+                                           last_key, b->lay.last_F, b->d_scratch, (double*)b->buf.sums, b->d_top,
+                                           b->d_aux, tt.bradix_counts);
       if ((b->top->kind == M_RADIX_TABLE || b->top->kind == M_HISTOGRAM) && b->host_status == 0)
         shard_table_local<T>(L, keys, sh, b->top->kind, b->top->table_bits, b->N, first_key, last_key, b->d_aux, tt.t32,
                              tt.pivots, tt.hist_bins, tt.hist_ipb);
@@ -1813,7 +1826,7 @@ template <class T> int shard_phase_typed(rmi_shard_build* b, int phase) {
       break;
     case RMI_PHASE_TOP_FINISH:
       shard_top_finish<T>(L, sh, b->top->kind, b->N, b->lay.pivot_x, b->lay.pivot_y, (const double*)b->buf.sums,
-                          first_key, last_key, b->lay.last_F, b->d_scratch, b->d_top, b->d_aux);
+                          first_key, last_key, b->lay.last_F, b->d_scratch, tt.bradix_counts, b->d_top, b->d_aux);
       if (b->top->kind == M_RADIX_TABLE && b->host_status == 0) shard_table_decode(L, b->top->table_bits, tt.t32);
       if (b->top->kind == M_HISTOGRAM && b->host_status == 0) hist_radix_index(L, tt.pivots, tt.hist_bins, tt.radix_index);
       break;
@@ -1910,9 +1923,8 @@ int rmi_shard_build_create(const rmi_dataset* local, const rmi_shard_ends* ends_
   if (!local || !ends_all || !model_spec || !buffers || !out) return fail(RMI_ERR_INVALID, fn + ": null argument");
   const ModelName *top = nullptr, *leaf = nullptr;
   if (int rc = parse_two_layer(model_spec, &top, &leaf)) return rc;
-  if (top->shard_rounds < 0)
-    return fail(RMI_ERR_UNSUPPORTED, "range-partitioned builds offer the top models linear, robust_linear, linear_spline, "
-                                     "cubic, normal, lognormal, radix, radix8..28, histogram");
+  if (top->shard_rounds < 0)   // every top model of the table is offered now; the check stays for the table's contract
+    return fail(RMI_ERR_UNSUPPORTED, "range-partitioned builds do not offer the top model " + std::string(top->name));
   uint64_t total = 0, base = 0;
   if (int rc = check_slabs(fn, local, ends_all, world, rank, &base, &total)) return rc;
   if (int rc = check_build(total, branch_factor, local->sorted)) return rc;
@@ -1944,7 +1956,8 @@ int rmi_shard_build_create(const rmi_dataset* local, const rmi_shard_ends* ends_
          cudaEventCreateWithFlags(&b->ev_join, cudaEventDisableTiming) == cudaSuccess &&
          cudaMalloc((void**)&b->d_long, sizeof(u32) * (LONG_LEAF_CAP + 1)) == cudaSuccess;
   }
-  ok = ok && b->tables.allocate(*top, total, branch_factor, device_alloc);
+  ok = ok && b->tables.allocate(*top, total, branch_factor, device_alloc) &&
+       b->tables.allocate_shard_counts(*top, branch_factor, device_alloc);
   // rmi_shard_train's exchange: leaf ownership, statistics partials and status words of every rank
   ok = ok && cudaMalloc((void**)&b->d_bases, sizeof(u64) * (world + 1)) == cudaSuccess &&
        cudaMalloc((void**)&b->d_off, sizeof(u64) * (world + 1)) == cudaSuccess &&
@@ -1958,6 +1971,20 @@ int rmi_shard_build_create(const rmi_dataset* local, const rmi_shard_ends* ends_
        cudaMemcpy(b->d_bases, bases.data(), sizeof(u64) * (world + 1), cudaMemcpyHostToDevice) == cudaSuccess;
   if (!ok) { rmi_shard_build_destroy(b); return fail(RMI_ERR_CUDA, fn + ": device allocation failed"); }
   *out = b;
+  return RMI_OK;
+}
+
+int rmi_shard_top_table(const rmi_shard_build* b, rmi_shard_top_table_info* out) {
+  if (!b || !out) return fail(RMI_ERR_INVALID, "rmi_shard_top_table: null argument");
+  const TopTables& tt = b->tables;
+  *out = rmi_shard_top_table_info{};
+  if (b->top->kind == M_RADIX_TABLE) {
+    *out = {tt.t32, tt.t32_len, (uint32_t)sizeof(u32), RMI_TABLE_REDUCE_MAX};
+  } else if (b->top->kind == M_HISTOGRAM) {
+    *out = {tt.pivots, tt.hist_bins, (uint32_t)sizeof(u64), RMI_TABLE_REDUCE_MAX};
+  } else if (b->top->kind == M_BRADIX) {
+    *out = {tt.bradix_counts, tt.bradix_len, (uint32_t)sizeof(u32), RMI_TABLE_REDUCE_SUM};
+  }
   return RMI_OK;
 }
 
@@ -2213,10 +2240,13 @@ static int shard_train_typed(rmi_shard_build* b, rmi_shard_comm* c, uint32_t fla
   if (W > 1 && rc == RMI_OK) {
     if (rounds == 1 || rounds == 2) nccl(nc.AllReduce(sums, sums, 8, ncclFloat64, ncclSum, comm, st), "ncclAllReduce(top sums)");
     if (rounds == 3) nccl(nc.AllReduce(sums + 8, sums + 8, 4, ncclInt64, ncclMin, comm, st), "ncclAllReduce(cubic interior points)");
-    if (rounds == 4 && b->host_status == 0) {   // table tops: merge the ranks' partial tables (one writer per entry, zero elsewhere)
+    if (rounds == 4 && b->host_status == 0) {   // table tops: merge the ranks' partial tables (rmi_shard_top_table)
       const TopTables& tt = b->tables;
       if (b->top->kind == M_RADIX_TABLE)
         nccl(nc.AllReduce(tt.t32, tt.t32, tt.t32_len, ncclUint32, ncclMax, comm, st), "ncclAllReduce(radix table)");
+      else if (b->top->kind == M_BRADIX)
+        nccl(nc.AllReduce(tt.bradix_counts, tt.bradix_counts, tt.bradix_len, ncclUint32, ncclSum, comm, st),
+             "ncclAllReduce(bradix counts)");
       else
         nccl(nc.AllReduce(tt.pivots, tt.pivots, tt.hist_bins, ncclUint64, ncclMax, comm, st), "ncclAllReduce(histogram pivots)");
     }

@@ -310,15 +310,29 @@ void shard_cache_fix_emit(const Launch& L, const CacheFixSlab& S, u64 line, u64 
 
 // ---- range-partitioned build phases (kernels_shard.cu) ---------------------------------------
 size_t shard_scratch_bytes();
+// d_bradix_counts: bradix's 4 x N u32 per-bin counts (null for the other tops), merged by an all-reduce SUM between
+// shard_top_local and shard_top_finish.
 template <class T>
 unsigned shard_top_local(const Launch& L, const T* keys, const Shard<T>& sh, int kind, u64 N, double px, double py,
-                         T first_key, T last_key, void* scratch, double* d_sums);
+                         T first_key, T last_key, u64 last_F, void* scratch, double* d_sums, TopModel* d_top,
+                         BuildAux* d_aux, u32* d_bradix_counts);
 template <class T>
 void shard_top_mid(const Launch& L, const T* keys, const Shard<T>& sh, int kind, u64 N, T first_key, T last_key,
                    void* scratch, double* d_sums, BuildAux* d_aux);
 template <class T>
 void shard_top_finish(const Launch& L, const Shard<T>& sh, int kind, u64 N, double px, double py, const double* d_sums,
-                      T first_key, T last_key, u64 last_F, const void* scratch, TopModel* d_top, BuildAux* d_aux);
+                      T first_key, T last_key, u64 last_F, const void* scratch, const u32* d_bradix_counts,
+                      TopModel* d_top, BuildAux* d_aux);
+// bradix over a range-partitioned array (kernels_top.cu).  shard_bradix_count: zero d_counts (4 x N u32), then count
+// this rank's keys per bin for all four candidates in one pass (the scalars in d_top / d_aux already set).
+// shard_bradix_decide: chi2 of every candidate over the merged counts, the strict minimum in candidate order, commit
+// (k_bradix_pick / k_bradix_commit); scratch holds shard_bradix_scratch_bytes().
+template <class T>
+void shard_bradix_count(const Launch& L, const T* keys, const Shard<T>& sh, u64 N, const TopModel* d_top, BuildAux* d_aux,
+                        u32* d_counts);
+void shard_bradix_decide(const Launch& L, u64 n, u64 N, const u32* d_counts, void* scratch, TopModel* d_top,
+                         BuildAux* d_aux);
+size_t shard_bradix_scratch_bytes();
 template <class T>
 void shard_bounds(const Launch& L, const T* keys, const Shard<T>& sh, int kind, const TopModel* d_top, u64 N, u64* d_S,
                   BuildAux* d_aux);

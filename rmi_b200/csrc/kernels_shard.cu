@@ -4,7 +4,10 @@
 // collectives issued by the host between these phases (rmi_b200/sharded.py):
 //
 //   phase TOP_LOCAL   k_shard_slr_partial / k_shard_slr_reduce   -> 5 partial sums per rank
-//        [all-reduce SUM of 5 doubles]                             (linear, robust_linear)
+//        [all-reduce SUM of 5 doubles]                             (linear, robust_linear, loglinear)
+//                     bradix: the scalars, then shard_bradix_count (kernels_top.cu): per-bin key counts of all
+//                     four candidates in one pass
+//        [all-reduce SUM of 4 x N u32]                             (bradix)
 //                     k_shard_cubic_local: this rank's candidates for the two interior points
 //        [all-reduce MIN of 4 order-encoded u64]                   (cubic)
 //                     k_shard_normal_partial<pass 0>: sum(x - pivot)
@@ -14,9 +17,9 @@
 //        [all-reduce SUM]
 //   phase TOP_FINISH  k_shard_slr_solve, k_shard_top_from_ends (linear_spline, radix: O(1)
 //                     functions of the global first / last key), k_shard_cubic_pick,
-//                     k_shard_normal_solve
+//                     k_shard_normal_solve, shard_bradix_decide (kernels_top.cu)
 //   phase BOUNDS      k_shard_bounds_search (monotone-by-construction tops) or the streaming
-//                     k_shard_bounds_stream (cubic, normal: also verifies monotonicity)
+//                     k_shard_bounds_stream (cubic, loglinear, normal: also verifies monotonicity)
 //                     -> S_local (global indices, n_global where none)
 //        [all-reduce MIN of (N+1) u64]
 //   phase SPLIT       k_split_from_S
@@ -41,8 +44,9 @@ constexpr int SH_MAX_BLOCKS = 132 * 8;   // 8 blocks per SM of an H100 (sh_grid:
 __device__ __forceinline__ void set_status(BuildAux* aux, unsigned bit) { atomicOr(&aux->status, bit); }
 
 // Partial sums of the top-level simple linear regression over the global item range
-// [g0, g1) restricted to this rank's slab, about the common pivot (px, py).
-template <class T>
+// [g0, g1) restricted to this rank's slab, about the common pivot (px, py).  MODE 0: y;  MODE 1: ln(y), items whose
+// ln(y) is not finite dropped (loglinear, as k_slr_partial<T, 1>; the pivot is then (px, 0)).
+template <class T, int MODE>
 __global__ void __launch_bounds__(SH_THREADS)
 k_shard_slr_partial(const T* __restrict__ keys, const Shard<T> sh, u64 g0, u64 g1, double sf, int use_sf, double px,
                     double py, double* __restrict__ partials) {
@@ -58,7 +62,7 @@ k_shard_slr_partial(const T* __restrict__ keys, const Shard<T> sh, u64 g0, u64 g
   for (u64 b = (lo & ~3ull) + ((u64)blockIdx.x * blockDim.x + threadIdx.x) * 4; b < hi; b += stride) {
     T k[4];
     int c = load_keys4(keys, b, sh.n_local, aligned, k);
-    if (c == 4 && b >= lo && b + 4 <= hi) {
+    if (MODE == 0 && c == 4 && b >= lo && b + 4 <= hi) {
       const T before = b > 0 ? keys[b - 1] : sh.prev_key;
       const bool dup = ((b > 0 || sh.has_prev) && before == k[0]) || k[1] == k[0] || k[2] == k[1] || k[3] == k[2];
       if (!dup) {
@@ -85,6 +89,7 @@ k_shard_slr_partial(const T* __restrict__ keys, const Shard<T> sh, u64 g0, u64 g
       if (i < lo || i >= hi) continue;
       double x = Key<T>::as_float(k[e]);
       double y = __ull2double_rn(scale_offset(F, sf, use_sf));
+      if (MODE == 1) { y = log(y); if (!isfinite(y)) continue; }
       double dx = x - px, dy = y - py;
       sx += dx; sy += dy; sxx = fma(dx, dx, sxx); sxy = fma(dx, dy, sxy);
       icnt += 1;
@@ -99,8 +104,9 @@ k_shard_slr_partial(const T* __restrict__ keys, const Shard<T> sh, u64 g0, u64 g
 }
 
 // Block partials -> sums[0..5); the rank holding the global last key adds the drained
-// iterator's repeated final item (models/mod.rs:180) when the fit drains the iterator.
-template <class T>
+// iterator's repeated final item (models/mod.rs:180) when the fit drains the iterator (MODE 1: only if its ln(y) is
+// finite, as k_slr_finish<T, 1>).
+template <class T, int MODE>
 __global__ void __launch_bounds__(SH_THREADS)
 k_shard_slr_reduce(const T* __restrict__ keys, const Shard<T> sh, int repeat, double sf, int use_sf, double px, double py,
                    const double* __restrict__ partials, int nblocks, double* __restrict__ sums) {
@@ -116,13 +122,17 @@ k_shard_slr_reduce(const T* __restrict__ keys, const Shard<T> sh, int repeat, do
     double x = Key<T>::as_float(keys[i]);
     u64 F = global_run_start(keys, i, sh.base, sh.has_prev, sh.prev_key, sh.prev_F);
     double y = __ull2double_rn(scale_offset(F, sf, use_sf));
-    double dx = x - px, dy = y - py;
-    r[0] += dx; r[1] += dy; r[2] += dx * dx; r[3] += dx * dy; r[4] += 1.0;
+    if (MODE == 1) y = log(y);
+    if (MODE == 0 || isfinite(y)) {
+      double dx = x - px, dy = y - py;
+      r[0] += dx; r[1] += dy; r[2] += dx * dx; r[3] += dx * dy; r[4] += 1.0;
+    }
   }
   for (int q = 0; q < 5; ++q) sums[q] = r[q];
 }
 
-// slr()'s closing formulas (linear.rs:36-58) on the globally reduced sums.
+// slr()'s closing formulas (linear.rs:36-58) on the globally reduced sums (loglinear: the same on the ln(y) sums,
+// k_slr_finish<T, 1>).
 __global__ void k_shard_slr_solve(const double* __restrict__ sums, double px, double py, TopModel* top, BuildAux* aux) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
   double sx = sums[0], sy = sums[1], sxx = sums[2], sxy = sums[3], cnt = sums[4];
@@ -148,7 +158,8 @@ __global__ void k_shard_slr_solve(const double* __restrict__ sums, double px, do
 }
 
 // Top models that are O(1) functions of the global first / last item:
-// linear_spline (linear_spline.rs:13-35) and radix (radix.rs:18-40, utils.rs:13-36).
+// linear_spline (linear_spline.rs:13-35) and radix (radix.rs:18-40, utils.rs:13-36); bradix's prefix, bits and
+// max_output (balanced_radix.rs:20-27).
 template <class T>
 __global__ void k_shard_top_from_ends(int kind, T first_key, T last_key, u64 last_F, u64 n, double sf, int use_sf,
                                       TopModel* top, BuildAux* aux) {
@@ -166,7 +177,7 @@ __global__ void k_shard_top_from_ends(int kind, T first_key, T last_key, u64 las
       beta = slope;
     }
     top->f[0] = alpha; top->f[1] = beta;
-  } else if (kind == M_RADIX) {
+  } else if (kind == M_RADIX || kind == M_BRADIX) {   // bradix: the scalars its candidates start from (k_radix_scalars)
     int prefix = common_prefix_sorted(Key<T>::as_int(first_key), Key<T>::as_int(last_key));
     u64 largest = scale_offset(last_F, sf, use_sf);
     aux->max_scaled_y = largest;
@@ -536,12 +547,16 @@ int sh_grid(u64 n, int num_sms) {
 
 // block partials (5 doubles per block) followed by 8 doubles of per-build state:
 // cand[0..6) (cubic / linear-spline candidates) and state[0] (normal: the mean)
-size_t shard_scratch_bytes() { return ((size_t)SH_MAX_BLOCKS * 5 + 8) * sizeof(double); }
+// (bradix's TOP_FINISH takes the block partials' room for its chi2 partials and best candidate)
+size_t shard_scratch_bytes() {
+  return std::max(((size_t)SH_MAX_BLOCKS * 5 + 8) * sizeof(double), shard_bradix_scratch_bytes());
+}
 static inline double* shard_cand(void* scratch) { return (double*)scratch + (size_t)SH_MAX_BLOCKS * 5; }
 
 template <class T>
 unsigned shard_top_local(const Launch& L, const T* keys, const Shard<T>& sh, int kind, u64 N, double px, double py,
-                         T first_key, T last_key, void* scratch, double* d_sums) {
+                         T first_key, T last_key, u64 last_F, void* scratch, double* d_sums, TopModel* d_top,
+                         BuildAux* d_aux, u32* d_bradix_counts) {
   double sf = (double)N / (double)sh.n_global;
   int use_sf = std::fabs(sf - 1.0) > DBL_EPSILON ? 1 : 0;
   double* partials = (double*)scratch;
@@ -559,10 +574,21 @@ unsigned shard_top_local(const Launch& L, const T* keys, const Shard<T>& sh, int
       }
     }
     int g = sh_grid((sh.n_local + 3) / 4 + 1, L.num_sms);
-    k_shard_slr_partial<T><<<g, SH_THREADS, 0, L.stream>>>(keys, sh, g0, g1, sf, use_sf, px, py, partials);
+    k_shard_slr_partial<T, 0><<<g, SH_THREADS, 0, L.stream>>>(keys, sh, g0, g1, sf, use_sf, px, py, partials);
     count_launch();
-    k_shard_slr_reduce<T><<<1, SH_THREADS, 0, L.stream>>>(keys, sh, repeat, sf, use_sf, px, py, partials, g, d_sums);
+    k_shard_slr_reduce<T, 0><<<1, SH_THREADS, 0, L.stream>>>(keys, sh, repeat, sf, use_sf, px, py, partials, g, d_sums);
     count_launch();
+  } else if (kind == M_LOGLINEAR) {   // linear.rs:61-72: the whole stream, ln(y) about the pivot (px, 0)
+    int g = sh_grid((sh.n_local + 3) / 4 + 1, L.num_sms);
+    k_shard_slr_partial<T, 1><<<g, SH_THREADS, 0, L.stream>>>(keys, sh, 0, sh.n_global, sf, use_sf, px, 0.0, partials);
+    count_launch();
+    k_shard_slr_reduce<T, 1><<<1, SH_THREADS, 0, L.stream>>>(keys, sh, 1, sf, use_sf, px, 0.0, partials, g, d_sums);
+    count_launch();
+  } else if (kind == M_BRADIX) {      // the scalars from the global ends, then this rank's per-bin counts
+    cudaMemsetAsync(d_sums, 0, 8 * sizeof(double), L.stream);
+    k_shard_top_from_ends<T><<<1, 32, 0, L.stream>>>(kind, first_key, last_key, last_F, sh.n_global, sf, use_sf, d_top, d_aux);
+    count_launch();
+    shard_bradix_count<T>(L, keys, sh, N, d_top, d_aux, d_bradix_counts);
   } else if (kind == M_CUBIC) {
     cudaMemsetAsync(d_sums, 0, 8 * sizeof(double), L.stream);
     k_shard_cubic_local<T><<<1, 32, 0, L.stream>>>(keys, sh, first_key, last_key, (u64*)d_sums + 8);
@@ -612,11 +638,17 @@ void shard_top_mid(const Launch& L, const T* keys, const Shard<T>& sh, int kind,
 
 template <class T>
 void shard_top_finish(const Launch& L, const Shard<T>& sh, int kind, u64 N, double px, double py, const double* d_sums,
-                      T first_key, T last_key, u64 last_F, const void* scratch, TopModel* d_top, BuildAux* d_aux) {
+                      T first_key, T last_key, u64 last_F, const void* scratch, const u32* d_bradix_counts,
+                      TopModel* d_top, BuildAux* d_aux) {
   double sf = (double)N / (double)sh.n_global;
   int use_sf = std::fabs(sf - 1.0) > DBL_EPSILON ? 1 : 0;
   if (kind == M_LINEAR || kind == M_ROBUST_LINEAR) {
     k_shard_slr_solve<<<1, 32, 0, L.stream>>>(d_sums, px, py, d_top, d_aux);
+  } else if (kind == M_LOGLINEAR) {
+    k_shard_slr_solve<<<1, 32, 0, L.stream>>>(d_sums, px, 0.0, d_top, d_aux);
+  } else if (kind == M_BRADIX) {   // chi2 over the merged counts, the strict minimum in candidate order, commit
+    shard_bradix_decide(L, sh.n_global, N, d_bradix_counts, const_cast<void*>(scratch), d_top, d_aux);
+    return;
   } else if (kind == M_CUBIC) {
     k_shard_cubic_pick<<<1, 32, 0, L.stream>>>(d_sums, shard_cand(const_cast<void*>(scratch)), d_top);
   } else if (kind == M_NORMAL || kind == M_LOGNORMAL) {
@@ -645,7 +677,9 @@ void shard_bounds(const Launch& L, const T* keys, const Shard<T>& sh, int kind, 
     case M_RADIX: k_shard_bounds_search<T, M_RADIX><<<blocks, SH_THREADS, 0, L.stream>>>(keys, sh, d_top, N, d_S); count_launch(); break;
     case M_RADIX_TABLE: k_shard_bounds_search<T, M_RADIX_TABLE><<<blocks, SH_THREADS, 0, L.stream>>>(keys, sh, d_top, N, d_S); count_launch(); break;
     case M_HISTOGRAM: k_shard_bounds_search<T, M_HISTOGRAM><<<blocks, SH_THREADS, 0, L.stream>>>(keys, sh, d_top, N, d_S); count_launch(); break;
+    case M_BRADIX: k_shard_bounds_search<T, M_BRADIX><<<blocks, SH_THREADS, 0, L.stream>>>(keys, sh, d_top, N, d_S); count_launch(); break;
     case M_CUBIC: shard_bounds_stream<T, M_CUBIC>(L, keys, sh, d_top, N, d_S, d_aux); break;
+    case M_LOGLINEAR: shard_bounds_stream<T, M_LOGLINEAR>(L, keys, sh, d_top, N, d_S, d_aux); break;
     case M_NORMAL: shard_bounds_stream<T, M_NORMAL>(L, keys, sh, d_top, N, d_S, d_aux); break;
     case M_LOGNORMAL: shard_bounds_stream<T, M_LOGNORMAL>(L, keys, sh, d_top, N, d_S, d_aux); break;
     default: k_shard_bounds_search<T, M_LINEAR><<<blocks, SH_THREADS, 0, L.stream>>>(keys, sh, d_top, N, d_S); count_launch(); break;
@@ -677,6 +711,8 @@ void shard_split(const Launch& L, const T* keys, const Shard<T>& sh, int kind, c
     case M_RADIX: k_split_from_S<T, M_RADIX><<<1, 32, 0, L.stream>>>(keys, sh, d_top, N, d_S, d_aux); break;
     case M_RADIX_TABLE: k_split_from_S<T, M_RADIX_TABLE><<<1, 32, 0, L.stream>>>(keys, sh, d_top, N, d_S, d_aux); break;
     case M_HISTOGRAM: k_split_from_S<T, M_HISTOGRAM><<<1, 32, 0, L.stream>>>(keys, sh, d_top, N, d_S, d_aux); break;
+    case M_BRADIX: k_split_from_S<T, M_BRADIX><<<1, 32, 0, L.stream>>>(keys, sh, d_top, N, d_S, d_aux); break;
+    case M_LOGLINEAR: k_split_from_S<T, M_LOGLINEAR><<<1, 32, 0, L.stream>>>(keys, sh, d_top, N, d_S, d_aux); break;
     case M_CUBIC: k_split_from_S<T, M_CUBIC><<<1, 32, 0, L.stream>>>(keys, sh, d_top, N, d_S, d_aux); break;
     case M_NORMAL: k_split_from_S<T, M_NORMAL><<<1, 32, 0, L.stream>>>(keys, sh, d_top, N, d_S, d_aux); break;
     case M_LOGNORMAL: k_split_from_S<T, M_LOGNORMAL><<<1, 32, 0, L.stream>>>(keys, sh, d_top, N, d_S, d_aux); break;
@@ -721,10 +757,11 @@ void shard_copy_flags(const Launch& L, const BuildAux* d_aux, unsigned* d_out2) 
 }
 
 #define INST(T)                                                                                                     \
-  template unsigned shard_top_local<T>(const Launch&, const T*, const Shard<T>&, int, u64, double, double, T, T, void*, double*); \
+  template unsigned shard_top_local<T>(const Launch&, const T*, const Shard<T>&, int, u64, double, double, T, T, u64, \
+                                       void*, double*, TopModel*, BuildAux*, u32*);                                 \
   template void shard_top_mid<T>(const Launch&, const T*, const Shard<T>&, int, u64, T, T, void*, double*, BuildAux*); \
   template void shard_top_finish<T>(const Launch&, const Shard<T>&, int, u64, double, double, const double*, T, T, u64,   \
-                                    const void*, TopModel*, BuildAux*);                                             \
+                                    const void*, const u32*, TopModel*, BuildAux*);                                 \
   template void shard_bounds<T>(const Launch&, const T*, const Shard<T>&, int, const TopModel*, u64, u64*, BuildAux*); \
   template void shard_bounds_given<T>(const Launch&, const T*, const Shard<T>&, int, const TopModel*, u64, u64*, BuildAux*); \
   template void shard_split<T>(const Launch&, const T*, const Shard<T>&, int, const TopModel*, u64, const u64*, BuildAux*); \

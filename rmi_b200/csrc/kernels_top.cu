@@ -545,17 +545,40 @@ k_bradix_bounds(const T* __restrict__ keys, u64 n, const TopModel* __restrict__ 
     }
   }
 }
+// The count of bin b (< max_output) of one candidate, as chi2() sees it (the drained stream's extra item included):
+// from the boundaries B of the whole array (single GPU) ...
+struct BradixBoundsCounts {
+  const u64* B;
+  u64 n;
+  __device__ __forceinline__ u64 operator()(u64 b, u64 max_output) const {
+    u64 lo = B[b], hi = (b + 1 < max_output) ? B[b + 1] : n;
+    u64 cnt = hi - lo;
+    if (hi == n && lo < n) cnt += 1;                  // repeated final item
+    return cnt;
+  }
+};
+// ... or from the merged per-bin counts of a range-partitioned build (the sum over ranks mod 2^32)
+struct BradixTableCounts {
+  const u32* c;
+  __device__ __forceinline__ u64 operator()(u64 b, u64) const { return c[b]; }
+};
+// The grid of the chi2 reduction: a function of N alone, so that every rank of a range-partitioned build sums the
+// same terms in the same tree whatever its GPU, and takes the decision rmi_train takes.
+int bradix_chi2_grid(u64 N) {
+  u64 blocks = (N + TOP_THREADS - 1) / TOP_THREADS;
+  if (blocks > (u64)MAX_PARTIAL_BLOCKS) blocks = MAX_PARTIAL_BLOCKS;
+  return blocks < 1 ? 1 : (int)blocks;
+}
+template <class Counts>
 __global__ void __launch_bounds__(TOP_THREADS)
-k_bradix_chi2(u64 n, const BuildAux* __restrict__ aux, const u64* __restrict__ B, double* __restrict__ partials) {
+k_bradix_chi2(u64 n, const BuildAux* __restrict__ aux, Counts count_of, double* __restrict__ partials) {
   __shared__ double sm[32];
   u64 max_output = aux->max_scaled_y;
   double expected = __ddiv_rn(__ull2double_rn(n), __ull2double_rn(max_output));
   double s = 0;
   u64 stride = (u64)gridDim.x * blockDim.x;
   for (u64 b = (u64)blockIdx.x * blockDim.x + threadIdx.x; b < max_output; b += stride) {
-    u64 lo = B[b], hi = (b + 1 < max_output) ? B[b + 1] : n;
-    u64 cnt = hi - lo;
-    if (hi == n && lo < n) cnt += 1;                  // repeated final item
+    u64 cnt = count_of(b, max_output);
     double cf = (double)(int)(unsigned)cnt;           // counts are i32 in the reference
     double dl = __dadd_rn(cf, -expected);
     s += __ddiv_rn(__dmul_rn(dl, dl), expected);
@@ -580,6 +603,51 @@ __global__ void k_bradix_commit(TopModel* top, BuildAux* aux, const BradixCand* 
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
   if (!aux->best_valid) { set_status(aux, ST_NUM_BITS); return; }
   top->ip[0] = best->prefix; top->ip[1] = best->bits; top->ip[2] = best->clamp; top->high = best->high;
+}
+
+// bradix over a range-partitioned array: this rank's keys counted per bin, for all four candidates in ONE pass over
+// the slab, into counts[which * N + bin] (zero-initialised u32, N > max_output).  Predictions are monotone in the key,
+// so a bin's keys form one run; the lane that sees a run start subtracts its local index, the lane that sees it end
+// adds the index one past it, and the wrapping u32 sum is the run's length — two atomics per run and candidate,
+// whichever thread sees which end.  The rank holding the global last key counts the drained stream's extra item in
+// that key's bin.  Summed over the ranks (mod 2^32) these are the counts k_bradix_chi2 takes from B on one GPU.
+template <class T>
+__global__ void __launch_bounds__(TOP_THREADS)
+k_bradix_count(const T* __restrict__ keys, const Shard<T> sh, u64 N, const TopModel* __restrict__ top, BuildAux* aux,
+               u32* __restrict__ counts) {
+  const u64 max_output = aux->max_scaled_y;
+  BradixCand c[4];
+#pragma unroll
+  for (int w = 0; w < 4; ++w) c[w] = bradix_candidate(top, aux, w);
+  const bool aligned = is_aligned16(keys);
+  const u64 n = sh.n_local;
+  unsigned bad = 0;
+  u64 stride = (u64)gridDim.x * blockDim.x * 4;
+  for (u64 b = ((u64)blockIdx.x * blockDim.x + threadIdx.x) * 4; b < n; b += stride) {
+    T k[4];
+    const int cnt = load_keys4(keys, b, n, aligned, k);
+    const T kp = b > 0 ? keys[b - 1] : k[0];
+#pragma unroll
+    for (int w = 0; w < 4; ++w) {
+      if (c[w].bits >= 64) continue;               // `for test_bits in bits..min(bits+2, 64)`
+      u32* cw = counts + (u64)w * N;
+      u64 pp = bradix_pred(c[w], kp);
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        if (e >= cnt) break;
+        const u64 i = b + e;
+        const u64 p = bradix_pred(c[w], k[e]);
+        if (p >= max_output) bad = ST_BRADIX_OOB;
+        if (i == 0 || p != pp) {
+          if (i > 0 && pp < max_output) atomicAdd(cw + pp, (u32)i);
+          if (p < max_output) atomicAdd(cw + p, 0u - (u32)i);
+        }
+        if (i + 1 == n && p < max_output) atomicAdd(cw + p, (u32)n + (sh.is_last ? 1u : 0u));
+        pp = p;
+      }
+    }
+  }
+  if (bad) set_status(aux, bad);
 }
 
 // histogram (histogram.rs:20-54, utils.rs:55-102): equi-depth pivots + 20-bit radix index.
@@ -623,6 +691,31 @@ void hist_radix_index(const Launch& L, const u64* d_pivots, u64 num_bins, u64* d
   k_hist_radix_index<<<grid_for((1ull << 20) + 1, L.num_sms), TOP_THREADS, 0, L.stream>>>(d_pivots, num_bins, d_radix_index);
   count_launch();
 }
+
+template <class T>
+void shard_bradix_count(const Launch& L, const T* keys, const Shard<T>& sh, u64 N, const TopModel* d_top, BuildAux* d_aux,
+                        u32* d_counts) {
+  cudaMemsetAsync(d_counts, 0, sizeof(u32) * 4 * N, L.stream);
+  if (sh.n_local == 0) return;
+  k_bradix_count<T><<<grid_for((sh.n_local + 3) / 4, L.num_sms), TOP_THREADS, 0, L.stream>>>(keys, sh, N, d_top, d_aux, d_counts);
+  count_launch();
+}
+
+void shard_bradix_decide(const Launch& L, u64 n, u64 N, const u32* d_counts, void* scratch, TopModel* d_top,
+                         BuildAux* d_aux) {
+  double* partials = (double*)scratch;
+  BradixCand* best = (BradixCand*)(partials + MAX_PARTIAL_BLOCKS);
+  const int gb = bradix_chi2_grid(N);
+  for (int which = 0; which < 4; ++which) {
+    k_bradix_chi2<<<gb, TOP_THREADS, 0, L.stream>>>(n, d_aux, BradixTableCounts{d_counts + (u64)which * N}, partials);
+    count_launch();
+    k_bradix_pick<<<1, TOP_THREADS, 0, L.stream>>>(partials, gb, which, d_top, d_aux, best);
+    count_launch();
+  }
+  k_bradix_commit<<<1, 32, 0, L.stream>>>(d_top, d_aux, best);
+  count_launch();
+}
+size_t shard_bradix_scratch_bytes() { return (size_t)MAX_PARTIAL_BLOCKS * sizeof(double) + sizeof(BradixCand); }
 
 size_t top_scratch_bytes(u64 num_leaves) {
   // partials (5 doubles per block) + candidates + state + bradix boundaries (N+2 u64) + best cand
@@ -738,8 +831,8 @@ unsigned fit_top_model(const Launch& L, const T* keys, u64 n, int kind, int tabl
       for (int which = 0; which < 4; ++which) {
         k_fill_u64<<<grid_for(num_leaves + 2, L.num_sms), TOP_THREADS, 0, st>>>(B, num_leaves + 2, n); count_launch();
         k_bradix_bounds<T><<<g, TOP_THREADS, 0, st>>>(keys, n, d_top, d_aux, which, B); count_launch();
-        int gb = grid_for(num_leaves, L.num_sms);
-        k_bradix_chi2<<<gb, TOP_THREADS, 0, st>>>(n, d_aux, B, partials); count_launch();
+        int gb = bradix_chi2_grid(num_leaves);
+        k_bradix_chi2<<<gb, TOP_THREADS, 0, st>>>(n, d_aux, BradixBoundsCounts{B, n}, partials); count_launch();
         k_bradix_pick<<<1, TOP_THREADS, 0, st>>>(partials, gb, which, d_top, d_aux, best); count_launch();
       }
       k_bradix_commit<<<1, 32, 0, st>>>(d_top, d_aux, best);
@@ -763,6 +856,9 @@ unsigned fit_top_model(const Launch& L, const T* keys, u64 n, int kind, int tabl
   return 0;
 }
 
+template void shard_bradix_count<u64>(const Launch&, const u64*, const Shard<u64>&, u64, const TopModel*, BuildAux*, u32*);
+template void shard_bradix_count<u32>(const Launch&, const u32*, const Shard<u32>&, u64, const TopModel*, BuildAux*, u32*);
+template void shard_bradix_count<double>(const Launch&, const double*, const Shard<double>&, u64, const TopModel*, BuildAux*, u32*);
 template unsigned fit_top_model<u64>(const Launch&, const u64*, u64, int, int, u64, bool, TopModel*, BuildAux*, void*, u32*, u64*, u64*, u64*);
 template unsigned fit_top_model<u32>(const Launch&, const u32*, u64, int, int, u64, bool, TopModel*, BuildAux*, void*, u32*, u64*, u64*, u32*);
 template unsigned fit_top_model<double>(const Launch&, const double*, u64, int, int, u64, bool, TopModel*, BuildAux*, void*, u32*, u64*, u64*, double*);

@@ -9,8 +9,10 @@ concatenated key array (reference semantics: rmi_lib::train on the whole data se
 
 Data path per build (SURVEY.md section 8(e)):
     top model        0, 1 or 2 tiny all-reduces (TOP_ROUNDS): SUM of 8 doubles (linear /
-                     robust_linear sums; normal / lognormal mean, then variance; cubic L1
-                     comparison), MIN of 4 x i64 (cubic: the two interior points of the spline)
+                     robust_linear / loglinear sums; normal / lognormal mean, then variance; cubic L1
+                     comparison), MIN of 4 x i64 (cubic: the two interior points of the spline);
+                     or one all-reduce of the top model's table (NATIVE_ONLY_TOPS): MAX of a radix table's
+                     hints or a histogram's pivots, SUM of bradix's 4 x N per-bin key counts
     all-reduce MIN   (N+1) x u64        leaf boundaries S
     (halo keys — the tail of a rank's last leaf that lives on the next rank(s) — are fetched once
      per data set, not per build: the keys are immutable)
@@ -42,12 +44,14 @@ PHASE_TOP_LOCAL, PHASE_TOP_FINISH, PHASE_BOUNDS, PHASE_SPLIT, PHASE_LEAF, PHASE_
 # Collectives of the top-model fit (include/rmi_b200.h rmi_shard_top_rounds): the first one follows
 # TOP_LOCAL, the second one (two-round tops) follows TOP_MID.  "sum": all-reduce SUM of sums[0:8]
 # as f64; "min": all-reduce MIN of sums[8:12] as signed 64-bit integers.
-TOP_ROUNDS = {"linear_spline": (), "radix": (), "linear": ("sum",), "robust_linear": ("sum",),
+TOP_ROUNDS = {"linear_spline": (), "radix": (), "linear": ("sum",), "robust_linear": ("sum",), "loglinear": ("sum",),
               "normal": ("sum", "sum"), "lognormal": ("sum", "sum"), "cubic": ("min", "sum")}
-# Table tops (rmi_shard_top_rounds == 4: one all-reduce MAX of the hint table / the pivots): offered by the one-call path
-# (rmi_shard_train, NCCL) only — this host-driven orchestrator has no view of the library-owned table.
-NATIVE_ONLY_TOPS = ("radix8", "radix18", "radix22", "radix26", "radix28", "histogram")
+# Table tops (rmi_shard_top_rounds == 4): one all-reduce of the library-owned table that rmi_shard_top_table describes
+# (MAX of the hint table / the pivots, SUM of bradix's counts), between TOP_LOCAL and TOP_FINISH.  The name is older
+# than the host-driven path's handle on that table; it stays bound to the code-4 tops.
+NATIVE_ONLY_TOPS = ("radix8", "radix18", "radix22", "radix26", "radix28", "histogram", "bradix")
 SHARDED_TOPS = tuple(TOP_ROUNDS) + NATIVE_ONLY_TOPS
+TABLE_REDUCE_MAX, TABLE_REDUCE_SUM = 0, 1      # rmi_shard_top_table_info.op
 _PPM = {"linear": 2, "robust_linear": 2, "linear_spline": 2, "loglinear": 2, "cubic": 4, "normal": 3, "lognormal": 3}
 _TORCH_OF_KEY = {api.KEY_U64: torch.int64, api.KEY_U32: torch.int32, api.KEY_F64: torch.float64}
 
@@ -55,6 +59,17 @@ _TORCH_OF_KEY = {api.KEY_U64: torch.int64, api.KEY_U32: torch.int32, api.KEY_F64
 class _Ends(C.Structure):
     _fields_ = [("first_key_bits", C.c_uint64), ("last_key_bits", C.c_uint64), ("last_run_start", C.c_uint64),
                 ("n_local", C.c_uint64), ("no_dups", C.c_uint64)]
+
+
+class _TopTable(C.Structure):
+    _fields_ = [("table", C.c_void_p), ("entries", C.c_uint64), ("entry_bytes", C.c_uint32), ("op", C.c_uint32)]
+
+
+class _DeviceArray:
+    """A 1-D view of library-owned device memory that torch.as_tensor takes without a copy."""
+
+    def __init__(self, ptr: int, n: int, typestr: str):
+        self.__cuda_array_interface__ = {"shape": (n,), "typestr": typestr, "data": (ptr, False), "version": 2}
 
 
 class _Buffers(C.Structure):
@@ -183,6 +198,7 @@ class CudaShardEngine:
                                              C.c_uint64, C.POINTER(_Buffers), C.c_void_p, C.POINTER(C.c_void_p)]
         L.rmi_shard_phase.argtypes = [C.c_void_p, C.c_int]
         L.rmi_shard_set_halo.argtypes = [C.c_void_p, C.c_uint64]
+        L.rmi_shard_top_table.argtypes = [C.c_void_p, C.POINTER(_TopTable)]
         L.rmi_shard_finish.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.POINTER(api._Result))]
         L.rmi_shard_build_destroy.argtypes = [C.c_void_p]
         L.rmi_shard_comm_unique_id.argtypes = [C.c_void_p]
@@ -219,6 +235,16 @@ class CudaShardEngine:
 
     def set_halo(self, count: int):
         api._check(self.lib.rmi_shard_set_halo(self._build, count))
+
+    def top_table(self):
+        """(table, op) of a code-4 top model (rmi_shard_top_table): an int32 / int64 device view of the u32 / u64
+        entries and TABLE_REDUCE_MAX / _SUM; None for the other tops."""
+        t = _TopTable()
+        api._check(self.lib.rmi_shard_top_table(self._build, C.byref(t)))
+        if t.entries == 0:
+            return None
+        typestr = "<i4" if t.entry_bytes == 4 else "<i8"
+        return torch.as_tensor(_DeviceArray(int(t.table), int(t.entries), typestr), device=self.device), int(t.op)
 
     def halo_view(self, offset: int, count: int) -> torch.Tensor:
         n = self.data.n_local
@@ -387,9 +413,6 @@ def train_sharded(data, model_spec: str, num_leaves: int, flags: int = 0, group=
                 raise
         return _retry_with_larger_halo(data, bufs, bases, n_global, N, model_spec, num_leaves, flags, group, world, dev, counts, native)
 
-    if parts[0] in NATIVE_ONLY_TOPS:
-        raise api.RMIError(f"a range-partitioned build with the top model {parts[0]} needs the one-call path "
-                           "(rmi_shard_train over an NCCL process group, or native=True with a single rank)")
     # 2. top model: local part -> tiny all-reduce(s) -> closed form (identical on every rank)
     def top_collective(kind):
         if world <= 1:
@@ -399,8 +422,13 @@ def train_sharded(data, model_spec: str, num_leaves: int, flags: int = 0, group=
         else:
             dist.all_reduce(bufs["sums"].view(torch.int64)[8:12], op=dist.ReduceOp.MIN, group=group)
 
-    rounds = TOP_ROUNDS[parts[0]]
+    rounds = TOP_ROUNDS.get(parts[0], ())
     eng.phase(PHASE_TOP_LOCAL)
+    if parts[0] in NATIVE_ONLY_TOPS and world > 1:
+        table = eng.top_table()
+        if table is not None:
+            # gloo cannot reduce device memory (one-GPU test boxes): stage through the host there
+            _merge_top_table(*table, group, dev.type == "cuda" and dist.get_backend(group) == "gloo")
     if rounds:
         top_collective(rounds[0])
     if len(rounds) > 1:
@@ -441,6 +469,25 @@ def train_sharded(data, model_spec: str, num_leaves: int, flags: int = 0, group=
         if world <= 1 or "halo" not in str(e):
             raise
     return _retry_with_larger_halo(data, bufs, bases, n_global, N, model_spec, num_leaves, flags, group, world, dev, counts, native)
+
+
+def _merge_top_table(table: torch.Tensor, op: int, group, stage: bool):
+    """All-reduce, in place, of a code-4 top model's table: `table` is the signed torch view (int32 / int64) of its
+    unsigned entries.  torch reduces signed integers, so MAX runs on the entries with their sign bit flipped (signed
+    order == unsigned order), and the u32 counts of a SUM are added as int64 and wrapped back to 32 bits."""
+    if op == TABLE_REDUCE_SUM:
+        assert table.dtype == torch.int32
+        h = table.to(torch.int64) & 0xFFFFFFFF
+        h = h.cpu() if stage else h
+        dist.all_reduce(h, op=dist.ReduceOp.SUM, group=group)
+        h = h & 0xFFFFFFFF
+        table.copy_(torch.where(h >= 1 << 31, h - (1 << 32), h).to(torch.int32))
+    else:
+        sign = -(1 << (8 * table.element_size() - 1))
+        h = table ^ sign
+        h = h.cpu() if stage else h
+        dist.all_reduce(h, op=dist.ReduceOp.MAX, group=group)
+        table.copy_(h ^ sign)
 
 
 def evaluate_sharded(trained, data, flags: int = 0, group=None, engine=None, counts: bool = True,
