@@ -336,6 +336,44 @@ int rmi_shard_comm_create(const void* id128, int world, int rank, int device, rm
 void rmi_shard_comm_destroy(rmi_shard_comm* c);
 int rmi_shard_train(rmi_shard_build* b, rmi_shard_comm* c, uint32_t flags, rmi_result** out);
 
+/* ---- The configuration search's unit of work over a range-partitioned data set (DESIGN.md section 9) ------------
+ * rmi_train_stats_batch over the slabs: the configurations "top,leaf_k" (k < num_leaf_models) of ONE top model and
+ * branching factor, statistics only.  The top model is fitted once and the leaf boundaries derived once, with the
+ * collectives of rmi_shard_train; then, for every leaf type, the fused leaf kernel runs over the leaves this rank owns
+ * and reduces them to one statistics partial.  One all-gather carries every rank's K RECORDS
+ * (RMI_SHARD_STATS_RECORD_BYTES each: the 40-byte partial, then the u32 status word and the u32 "could not replace"
+ * flag) and every rank merges them in rank order: the results are identical on every rank, and no leaf record leaves
+ * the rank that owns it.  out[k] follows the statistics of rmi_train_stats_batch on the concatenated keys (avg_l2 and
+ * avg_log2 are summed over a different tree); it holds no leaf tables.  Release each with rmi_result_free.
+ *
+ * rmi_shard_stats_batch_create refuses, before any device work, in this order: a null argument or num_leaf_models < 1
+ * (RMI_ERR_INVALID); an unknown top or leaf model (RMI_ERR_PANIC); a radix-table leaf (RMI_ERR_UNSUPPORTED); then
+ * whatever rmi_shard_build_create refuses (the ends-table checks, the keys).  It returns a build object whose phases
+ * RMI_PHASE_TOP_LOCAL .. RMI_PHASE_SPLIT, rmi_shard_top_table and rmi_shard_set_halo work as for a build;
+ * RMI_PHASE_LEAF / RMI_PHASE_STATS are refused (RMI_ERR_INVALID).  Of `buffers` it reads sums, S, errors, counts and
+ * status (N entries each, whatever the leaf types); params is not used: the leaf parameters go to the batch's own
+ * scratch.  Release with rmi_shard_build_destroy.
+ *
+ * Host-driven form (rmi_b200/sharded.py drives it over gloo): the phases and collectives of a build up to and including
+ * RMI_PHASE_SPLIT and the halo, then for k = 0 .. K-1 rmi_shard_stats_leaf, which writes this rank's record of leaf
+ * type k at d_record (device memory), then an all-gather of the K records of every rank (world x K records, rank by
+ * rank) and rmi_shard_stats_finish over them.  The leaf calls are enqueued on the build's stream without a host
+ * synchronisation.
+ * One-call form: rmi_shard_train_stats_batch runs all of it on the build's stream over c (NCCL), with no host
+ * synchronisation but the final one.
+ * A status bit on any rank fails the call on EVERY rank with the same message, prefixed "top,leaf: " of the first leaf
+ * type that has one; a leaf that reaches past the halo is reported as by rmi_shard_train ("... past the halo ..."), and
+ * the caller may grow the halo and measure again.  flags: none is read (the batch is statistics only).  device_time_ns: the batch's device time shared out evenly
+ * (one call: the whole stream, collectives included; host-driven: the sum of the phases). */
+#define RMI_SHARD_STATS_RECORD_BYTES 48
+int rmi_shard_stats_batch_create(const rmi_dataset* local, const rmi_shard_ends* ends_all, int world, int rank,
+                                 const char* top_model, const char* const* leaf_models, int num_leaf_models,
+                                 uint64_t branch_factor, uint64_t halo_capacity, const rmi_shard_buffers* buffers,
+                                 void* cuda_stream, rmi_shard_build** out);
+int rmi_shard_stats_leaf(rmi_shard_build* b, int k, void* d_record);
+int rmi_shard_stats_finish(rmi_shard_build* b, const void* d_records, uint32_t flags, rmi_result** out);
+int rmi_shard_train_stats_batch(rmi_shard_build* b, rmi_shard_comm* c, uint32_t flags, rmi_result** out);
+
 /* ---- Lookups over a range-partitioned data set (DESIGN.md section 14) ------------------------------------------
  * Every rank holds the whole model and its own slab of the keys; together the slabs are the key set the model was
  * trained on (or evaluated on).  Query q is answered by the last non-empty rank whose first key is < q (the first
@@ -607,6 +645,16 @@ typedef struct {
 } rmi_config_stats;
 int rmi_find_pareto_efficient_configs(const rmi_dataset* const* replicas, int num_replicas, uint64_t restrict_to,
                                       uint32_t flags, rmi_config_stats* out, uint64_t capacity, uint64_t* out_count);
+/* The same search with the caller's measuring step: measure(ctx, top, bf, leaves, K, flags, out) fills out[k]'s
+ * average_log2_error, max_log2_error and size (rmi_model_size(r, 1, 0) of a result) for the configurations
+ * "top,leaves[k]" at branching factor bf, and returns 0; any other value stops the search, which then fails with
+ * RMI_ERR_PANIC and the message the callback left in rmi_last_error() (if any).  The callback runs on the calling thread,
+ * once per (top, branching factor) group of each phase, every group whole, smallest branching factor first (the order of
+ * the replicas' sweep).  rmi_b200/sharded.py measures range-partitioned slabs with it. */
+typedef int (*rmi_measure_group_fn)(void* ctx, const char* top_model, uint64_t branch_factor, const char* const* leaf_models,
+                                    int num_leaf_models, uint32_t flags, rmi_config_stats* out);
+int rmi_find_pareto_efficient_configs_with(rmi_measure_group_fn measure, void* ctx, uint64_t restrict_to, uint32_t flags,
+                                           rmi_config_stats* out, uint64_t capacity, uint64_t* out_count);
 
 /* rmi_train keeps one CUDA stream set and one device scratch buffer per host thread and device (created on first use,
  * grown to the largest build and reused by later builds; results never live in it).  A worker thread that will not

@@ -722,6 +722,48 @@ int rmi_find_pareto_efficient_configs(const rmi_dataset* const* replicas, int nu
   }
 }
 
+int rmi_find_pareto_efficient_configs_with(rmi_measure_group_fn measure, void* ctx, uint64_t restrict_to, uint32_t flags,
+                                           rmi_config_stats* out, uint64_t capacity, uint64_t* out_count) {
+  g_last_error.clear();
+  if (!measure || !out_count || (capacity && !out))
+    return fail(RMI_ERR_INVALID, "rmi_find_pareto_efficient_configs_with: bad argument");
+  try {
+    rmihost::MeasureStep step;   // one thread, and every (top, branching factor) group whole
+    step.measure = [&](size_t, const rmihost::MeasureGroup& g) {
+      std::vector<const char*> names;
+      for (auto& l : g.leaves) names.push_back(l.c_str());
+      std::vector<rmi_config_stats> res(g.leaves.size());
+      memset(res.data(), 0, sizeof(rmi_config_stats) * res.size());
+      g_last_error.clear();
+      const int rc = measure(ctx, g.top.c_str(), g.bf, names.data(), (int)names.size(), flags, res.data());
+      if (rc != 0) {
+        std::string msg = rmi_last_error();
+        throw std::runtime_error(msg.empty() ? "the measuring callback returned " + std::to_string(rc) : msg);
+      }
+      std::vector<rmihost::RMIStatistics> v(res.size());
+      for (size_t k = 0; k < res.size(); ++k) {
+        v[k].average_log2_error = res[k].average_log2_error;
+        v[k].max_log2_error = res[k].max_log2_error;
+        v[k].size = res[k].size;
+      }
+      return v;
+    };
+    std::vector<rmihost::RMIStatistics> front = rmihost::find_pareto_efficient_configs(step, (size_t)restrict_to);
+    g_last_error.clear();
+    *out_count = front.size();
+    for (size_t i = 0; i < front.size() && i < capacity; ++i) {
+      std::snprintf(out[i].models, sizeof out[i].models, "%s", front[i].models.c_str());
+      out[i].branching_factor = front[i].branching_factor;
+      out[i].average_log2_error = front[i].average_log2_error;
+      out[i].max_log2_error = front[i].max_log2_error;
+      out[i].size = front[i].size;
+    }
+    return RMI_OK;
+  } catch (const std::exception& e) {
+    return fail(RMI_ERR_PANIC, e.what());
+  }
+}
+
 int rmi_dataset_replicate(const rmi_dataset* src, int device, rmi_dataset** out) {
   g_last_error.clear();
   if (!src || !out) return fail(RMI_ERR_INVALID, "rmi_dataset_replicate: null argument");
@@ -1733,6 +1775,13 @@ struct rmi_shard_build {
   // table tops (radix8..28, histogram): the table every rank fills its part of, merged by an all-reduce MAX
   TopTables tables;
   cudaEvent_t ev_off = nullptr, ev_t0 = nullptr, ev_t1 = nullptr;
+  // statistics-only batches (rmi_shard_stats_batch_create): the K leaf types and scratch of the batch's own
+  std::vector<const ModelName*> batch;       // empty: an ordinary build object
+  double* d_batch_params = nullptr;          // N x the largest params-per-model of the batch
+  BuildAux* d_batch_aux = nullptr;           // K: every leaf type's status, replacement flag and statistics
+  char* d_batch_recs = nullptr;              // world x K records (rmi_shard_train_stats_batch gathers into it)
+  char* d_batch_parts = nullptr;             // K x world statistics partials, leaf type by leaf type
+  unsigned char* h_batch_recs = nullptr;     // pinned: world x K records
 };
 
 struct rmi_shard_comm {
@@ -1990,6 +2039,8 @@ int rmi_shard_top_table(const rmi_shard_build* b, rmi_shard_top_table_info* out)
 
 int rmi_shard_phase(rmi_shard_build* b, int phase) {
   if (!b) return fail(RMI_ERR_INVALID, "rmi_shard_phase: null build");
+  if (!b->batch.empty() && (phase == RMI_PHASE_LEAF || phase == RMI_PHASE_STATS))
+    return fail(RMI_ERR_INVALID, "rmi_shard_phase: a statistics batch runs its leaves with rmi_shard_stats_leaf");
   b->gather_mode = false;   // host-driven flow: the caller combines the leaf records with an all-reduce SUM of zero-filled arrays
   CUDA_TRY(cudaSetDevice(b->ds->device));
   return with_key_type(b->ds->key_type, [&](auto k) { return shard_phase_typed<decltype(k)>(b, phase); });
@@ -2007,7 +2058,7 @@ int rmi_shard_set_halo(rmi_shard_build* b, uint64_t halo_keys) {
 // The public result from what copy_result_to_host brought back (after the stream has been synchronised).
 // st_all: OR of every rank's status word; cnr: some rank could not replace an empty leaf.
 static int shard_result(rmi_shard_build* b, ResultBox* box, unsigned st_all, bool cnr, const uint64_t* total_device_ns,
-                        rmi_result** out) {
+                        rmi_result** out, const ModelName* leaf = nullptr) {
   if (st_all) {
     std::string msg = status_text((b->host_status | result_aux(box).status | st_all) & ~ST_HALO_TOO_SMALL);
     if (st_all & ST_HALO_TOO_SMALL) msg += (msg.empty() ? "" : "; ") + std::string("a leaf reaches past the halo copied from the next rank");
@@ -2015,7 +2066,7 @@ static int shard_result(rmi_shard_build* b, ResultBox* box, unsigned st_all, boo
     delete box;
     return fail(RMI_ERR_PANIC, msg);
   }
-  fill_result(box, *b->top, *b->leaf, b->tables, b->lay.n_global, b->N);
+  fill_result(box, *b->top, leaf ? *leaf : *b->leaf, b->tables, b->lay.n_global, b->N);
   rmi_result& R = box->pub;
   {   // device time of this rank's phases (collectives between them are not included)
     const int map[RMI_NUM_PHASES] = {0, 0, 1, 1, 2, 3, 0};
@@ -2186,53 +2237,22 @@ void rmi_shard_comm_destroy(rmi_shard_comm* c) {
 
 }  // extern "C"
 
-template <class T>
-static int shard_train_typed(rmi_shard_build* b, rmi_shard_comm* c, uint32_t flags, rmi_result** out) {
+// The top model and the leaf boundaries of a one-call build (rmi_shard_train, rmi_shard_train_stats_batch): phases
+// RMI_PHASE_TOP_LOCAL to RMI_PHASE_SPLIT and their collectives, enqueued on the build's stream.  mark(what): a trace
+// point after each step.
+template <class T, class Mark>
+static int shard_top_and_bounds(rmi_shard_build* b, rmi_shard_comm* c, Mark&& mark) {
   const NcclApi& nc = nccl_api();
   const uint64_t N = b->N;
-  const int ppm = leaf_params_per_model(b->leaf->kind);
-  const int W = b->world, rank = b->rank;
-  const bool stats_only = (flags & RMI_FLAG_STATS_ONLY) != 0;
-  const bool want_counts = !stats_only && (flags & RMI_FLAG_LEAF_COUNTS) != 0;
+  const int W = b->world;
   cudaStream_t st = b->st;
   ncclComm_t comm = c->comm;
-  // RMI_FLAG_SHARD_ROOT_ONLY on one node: every rank copies the records of the leaves it owns into a host region all
-  // ranks share (comm_ensure_shared) — rank 0's result points into it — instead of rank 0 copying all N records itself
-  bool shared = !stats_only && (flags & RMI_FLAG_SHARD_ROOT_ONLY) != 0 && W > 1 && c->single_node;
-  const size_t shared_bytes = sizeof(double) * N * ppm + sizeof(u64) * N * (want_counts ? 2 : 1);
-  if (shared) {
-    if (int rcs = comm_ensure_shared(c, shared_bytes, st)) return rcs;
-    shared = c->single_node && c->shm != nullptr;
-  }
-  unsigned char* const region = shared ? c->shm + (size_t)c->parity * c->shm_half : nullptr;
-  double* const sh_params = (double*)region;
-  u64* const sh_errors = shared ? (u64*)(region + sizeof(double) * N * ppm) : nullptr;
-  u64* const sh_counts = (shared && want_counts) ? sh_errors + N : nullptr;
-  const bool leaves_to_host = !shared && !stats_only && (rank == 0 || (flags & RMI_FLAG_SHARD_ROOT_ONLY) == 0);
-  Launch L{st, b->num_sms};
   double* sums = (double*)b->buf.sums;
-  // pinned host memory for the results first (nothing below waits for the host except the owner offsets)
-  auto box = new ResultBox();
-  if (!reserve_result(box, &b->tables, N, ppm, leaves_to_host, want_counts)) { delete box; return fail(RMI_ERR_CUDA, kPinnedFailed); }
-  b->gather_mode = true;
   int rc = RMI_OK;
   auto phase = [&](int ph) { if (rc == RMI_OK) rc = shard_phase_typed<T>(b, ph); };
   auto nccl = [&](ncclResult_t r, const char* what) {
     if (rc == RMI_OK && r != ncclSuccess) rc = fail(RMI_ERR_CUDA, std::string(what) + ": " + nc.GetErrorString(r));
   };
-  // RMI_DEV_SHARD_TRACE=1: device time between the marks below, printed per build by every rank (developer probe)
-  static const bool trace = [] { const char* e = getenv("RMI_DEV_SHARD_TRACE"); return e && e[0] == '1'; }();
-  struct Mark { const char* what; cudaEvent_t ev; };
-  static thread_local std::vector<Mark> marks;
-  size_t n_marks = 0;
-  auto mark = [&](const char* what) {
-    if (!trace) return;
-    if (n_marks == marks.size()) { Mark m{what, nullptr}; cudaEventCreate(&m.ev); marks.push_back(m); }
-    marks[n_marks].what = what;
-    cudaEventRecord(marks[n_marks++].ev, st);
-  };
-  cudaEventRecord(b->ev_t0, st);
-  mark("start");
   // ---- top model: local part, 0-2 tiny all-reduces, closed form (identical on every rank) -----------------
   phase(RMI_PHASE_TOP_LOCAL);
   mark("top local");
@@ -2264,6 +2284,56 @@ static int shard_train_typed(rmi_shard_build* b, rmi_shard_comm* c, uint32_t fla
   if (W > 1 && rc == RMI_OK) nccl(nc.AllReduce(b->buf.S, b->buf.S, N + 1, ncclUint64, ncclMin, comm, st), "ncclAllReduce(leaf boundaries)");
   mark("bounds all-reduce");
   phase(RMI_PHASE_SPLIT);
+  return rc;
+}
+
+template <class T>
+static int shard_train_typed(rmi_shard_build* b, rmi_shard_comm* c, uint32_t flags, rmi_result** out) {
+  const NcclApi& nc = nccl_api();
+  const uint64_t N = b->N;
+  const int ppm = leaf_params_per_model(b->leaf->kind);
+  const int W = b->world, rank = b->rank;
+  const bool stats_only = (flags & RMI_FLAG_STATS_ONLY) != 0;
+  const bool want_counts = !stats_only && (flags & RMI_FLAG_LEAF_COUNTS) != 0;
+  cudaStream_t st = b->st;
+  ncclComm_t comm = c->comm;
+  // RMI_FLAG_SHARD_ROOT_ONLY on one node: every rank copies the records of the leaves it owns into a host region all
+  // ranks share (comm_ensure_shared) — rank 0's result points into it — instead of rank 0 copying all N records itself
+  bool shared = !stats_only && (flags & RMI_FLAG_SHARD_ROOT_ONLY) != 0 && W > 1 && c->single_node;
+  const size_t shared_bytes = sizeof(double) * N * ppm + sizeof(u64) * N * (want_counts ? 2 : 1);
+  if (shared) {
+    if (int rcs = comm_ensure_shared(c, shared_bytes, st)) return rcs;
+    shared = c->single_node && c->shm != nullptr;
+  }
+  unsigned char* const region = shared ? c->shm + (size_t)c->parity * c->shm_half : nullptr;
+  double* const sh_params = (double*)region;
+  u64* const sh_errors = shared ? (u64*)(region + sizeof(double) * N * ppm) : nullptr;
+  u64* const sh_counts = (shared && want_counts) ? sh_errors + N : nullptr;
+  const bool leaves_to_host = !shared && !stats_only && (rank == 0 || (flags & RMI_FLAG_SHARD_ROOT_ONLY) == 0);
+  Launch L{st, b->num_sms};
+  // pinned host memory for the results first (nothing below waits for the host except the owner offsets)
+  auto box = new ResultBox();
+  if (!reserve_result(box, &b->tables, N, ppm, leaves_to_host, want_counts)) { delete box; return fail(RMI_ERR_CUDA, kPinnedFailed); }
+  b->gather_mode = true;
+  int rc = RMI_OK;
+  auto phase = [&](int ph) { if (rc == RMI_OK) rc = shard_phase_typed<T>(b, ph); };
+  auto nccl = [&](ncclResult_t r, const char* what) {
+    if (rc == RMI_OK && r != ncclSuccess) rc = fail(RMI_ERR_CUDA, std::string(what) + ": " + nc.GetErrorString(r));
+  };
+  // RMI_DEV_SHARD_TRACE=1: device time between the marks below, printed per build by every rank (developer probe)
+  static const bool trace = [] { const char* e = getenv("RMI_DEV_SHARD_TRACE"); return e && e[0] == '1'; }();
+  struct Mark { const char* what; cudaEvent_t ev; };
+  static thread_local std::vector<Mark> marks;
+  size_t n_marks = 0;
+  auto mark = [&](const char* what) {
+    if (!trace) return;
+    if (n_marks == marks.size()) { Mark m{what, nullptr}; cudaEventCreate(&m.ev); marks.push_back(m); }
+    marks[n_marks].what = what;
+    cudaEventRecord(marks[n_marks++].ev, st);
+  };
+  cudaEventRecord(b->ev_t0, st);
+  mark("start");
+  rc = shard_top_and_bounds<T>(b, c, mark);
   if (rc == RMI_OK) {
     shard_owner_offsets(L, (const u64*)b->buf.S, N, b->d_bases, W, b->r_last, b->d_off);
     cudaMemcpyAsync(b->h_off, b->d_off, sizeof(u64) * (W + 1), cudaMemcpyDeviceToHost, st);
@@ -2390,6 +2460,112 @@ static int shard_train_typed(rmi_shard_build* b, rmi_shard_comm* c, uint32_t fla
   return rcf;
 }
 
+// ---- statistics-only batches over the slabs (rmi_shard_stats_batch_create) ---------------------------------------
+// A record: this rank's statistics partial of the leaves it owns, then {status word, could_not_replace != 0}.
+static size_t stats_record_bytes() { return stats_partial_bytes() + 2 * sizeof(unsigned); }
+
+// Leaf type k of the batch over the leaves this rank owns, after RMI_PHASE_SPLIT: the fused leaf kernel into the
+// batch's own parameter scratch, then this rank's record at d_rec.  The owner offsets are derived again here (one
+// tiny kernel) so that the host-driven flow needs no extra call.
+template <class T> static int shard_stats_leaf_typed(rmi_shard_build* b, int k, char* d_rec) {
+  const T* keys = (const T*)b->ds->d_keys;
+  Shard<T> sh = shard_of<T>(b->lay, b->ds->n, b->ds->n + b->halo);
+  Launch L{b->st, b->num_sms};
+  L.side = b->side; L.ev_fork = b->ev_fork; L.ev_join = b->ev_join; L.d_long = b->d_long;
+  if (k == 0) {
+    cudaEventRecord(b->ev_begin[RMI_PHASE_LEAF], b->st);
+    b->ran[RMI_PHASE_LEAF] = true;
+    shard_owner_offsets(L, (const u64*)b->buf.S, b->N, b->d_bases, b->world, b->r_last, b->d_off);
+  }
+  BuildAux* a = b->d_batch_aux + k;   // starts from the state the top model and the boundaries left
+  cudaMemcpyAsync(a, b->d_aux, sizeof(BuildAux), cudaMemcpyDeviceToDevice, b->st);
+  fit_leaves<T>(L, keys, sh, b->batch[k]->kind, b->N, (const u64*)b->buf.S, a, b->d_batch_params, (u64*)b->buf.errors,
+                (u64*)b->buf.counts);
+  leaf_statistics_owned(L, b->lay.n_global, b->N, (const u64*)b->buf.errors, (const u64*)b->buf.counts, b->d_off, b->rank,
+                        b->world, d_rec, b->d_stats);
+  shard_copy_flags(L, a, (unsigned*)(d_rec + stats_partial_bytes()));
+  cudaEventRecord(b->ev_end[RMI_PHASE_LEAF], b->st);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(RMI_ERR_CUDA, std::string("rmi_shard_stats_leaf: ") + cudaGetErrorString(e));
+  return RMI_OK;
+}
+
+// The K results from every rank's records (d_recs: world x K records in device memory, rank by rank): the partials of
+// each leaf type are merged in rank order into its BuildAux, the status words and replacement flags OR-ed over the
+// ranks.  The batch's device time is shared out evenly: with one_call, the whole stream from the first phase to the
+// merge (collectives included), otherwise the sum of the phases.
+static int shard_stats_results(rmi_shard_build* b, const char* d_recs, bool one_call, rmi_result** out) {
+  const int K = (int)b->batch.size(), W = b->world;
+  const size_t rec = stats_record_bytes(), part = stats_partial_bytes();
+  cudaStream_t st = b->st;
+  Launch L{st, b->num_sms};
+  std::vector<ResultBox*> boxes(K, nullptr);
+  bool ok = true;
+  for (int k = 0; k < K; ++k) {
+    boxes[k] = new ResultBox();
+    ok = ok && reserve_result(boxes[k], &b->tables, b->N, 0, false, false);
+  }
+  if (!ok) { for (auto* x : boxes) delete x; return fail(RMI_ERR_CUDA, kPinnedFailed); }
+  if (!b->ran[RMI_PHASE_STATS]) { cudaEventRecord(b->ev_begin[RMI_PHASE_STATS], st); b->ran[RMI_PHASE_STATS] = true; }
+  for (int k = 0; k < K; ++k) {
+    char* parts = b->d_batch_parts + part * W * k;   // leaf type k's partials of ranks 0..W-1, contiguous
+    cudaMemcpy2DAsync(parts, part, d_recs + rec * k, rec * K, part, W, cudaMemcpyDeviceToDevice, st);
+    leaf_statistics_merge(L, parts, W, b->d_batch_aux + k);
+    copy_result_to_host(boxes[k], &b->tables, b->d_batch_aux + k, b->d_top, nullptr, nullptr, nullptr, st);
+  }
+  cudaEventRecord(b->ev_end[RMI_PHASE_STATS], st);
+  cudaMemcpyAsync(b->h_batch_recs, d_recs, rec * K * W, cudaMemcpyDeviceToHost, st);
+  cudaError_t e = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) { for (auto* x : boxes) delete x; return fail(RMI_ERR_CUDA, std::string("rmi_shard_stats_finish: ") + cudaGetErrorString(e)); }
+  uint64_t device_ns = 0;
+  if (one_call) device_ns = elapsed_ns(b->ev_t0, b->ev_end[RMI_PHASE_STATS]);
+  else for (int q = 0; q < RMI_NUM_PHASES; ++q) if (b->ran[q]) device_ns += elapsed_ns(b->ev_begin[q], b->ev_end[q]);
+  int rc = RMI_OK;
+  for (int k = 0; k < K; ++k) {
+    unsigned st_all = b->host_status;
+    bool cnr = false;
+    for (int r = 0; r < W; ++r) {
+      const unsigned* f = (const unsigned*)(b->h_batch_recs + rec * ((size_t)r * K + k) + part);
+      st_all |= f[0];
+      cnr = cnr || f[1] != 0;
+    }
+    const uint64_t share = device_ns / (uint64_t)K;
+    if (rc == RMI_OK) {
+      rc = shard_result(b, boxes[k], st_all, cnr, &share, &out[k], b->batch[k]);   // deletes the box on failure
+      if (rc != RMI_OK) {
+        const std::string msg = std::string(b->top->name) + "," + b->batch[k]->name + ": " + rmi_last_error();
+        for (int q = 0; q < k; ++q) rmi_result_free(out[q]);
+        rc = fail(rc, msg);
+      }
+    } else {
+      delete boxes[k];
+    }
+  }
+  if (rc != RMI_OK) return rc;
+  for (int k = 0; k < K; ++k) out[k]->build_time_ns /= (uint64_t)K;   // the batch's wall time, shared out evenly
+  return RMI_OK;
+}
+
+template <class T>
+static int shard_stats_batch_typed(rmi_shard_build* b, rmi_shard_comm* c, rmi_result** out) {
+  const int K = (int)b->batch.size(), W = b->world;
+  const size_t rec = stats_record_bytes();
+  cudaStream_t st = b->st;
+  b->gather_mode = true;
+  cudaEventRecord(b->ev_t0, st);
+  int rc = shard_top_and_bounds<T>(b, c, [](const char*) {});
+  char* mine = b->d_batch_recs + rec * K * b->rank;
+  for (int k = 0; k < K && rc == RMI_OK; ++k) rc = shard_stats_leaf_typed<T>(b, k, mine + rec * k);
+  // one all-gather carries every leaf type's partial and status words: K records per rank
+  if (rc == RMI_OK && W > 1) {
+    ncclResult_t r = nccl_api().AllGather(mine, b->d_batch_recs, rec * K, ncclChar, c->comm, st);
+    if (r != ncclSuccess) rc = fail(RMI_ERR_CUDA, std::string("ncclAllGather(statistics records): ") + nccl_api().GetErrorString(r));
+  }
+  if (rc != RMI_OK) { cudaStreamSynchronize(st); return rc; }
+  // the records are merged on the stream behind the gather
+  return shard_stats_results(b, b->d_batch_recs, true, out);
+}
+
 extern "C" {
 
 int rmi_shard_train(rmi_shard_build* b, rmi_shard_comm* c, uint32_t flags, rmi_result** out) {
@@ -2402,6 +2578,76 @@ int rmi_shard_train(rmi_shard_build* b, rmi_shard_comm* c, uint32_t flags, rmi_r
   if (!nccl_api().ok) return fail(RMI_ERR_UNSUPPORTED, nccl_api().error);
   CUDA_TRY(cudaSetDevice(b->ds->device));
   return with_key_type(b->ds->key_type, [&](auto k) { return shard_train_typed<decltype(k)>(b, c, flags, out); });
+}
+
+int rmi_shard_stats_batch_create(const rmi_dataset* local, const rmi_shard_ends* ends_all, int world, int rank,
+                                 const char* top_model, const char* const* leaf_models, int num_leaf_models,
+                                 uint64_t branch_factor, uint64_t halo_capacity, const rmi_shard_buffers* buffers,
+                                 void* cuda_stream, rmi_shard_build** out) {
+  const std::string fn = "rmi_shard_stats_batch_create";
+  g_last_error.clear();
+  if (!local || !ends_all || !top_model || !leaf_models || num_leaf_models < 1 || !buffers || !out)
+    return fail(RMI_ERR_INVALID, fn + ": bad argument");
+  // rmi_train_stats_batch's checks of the model names first, then rmi_shard_build_create's (the ends table and the keys)
+  const ModelName* top = nullptr;
+  if (int rc = find_layer(top_model, true, &top)) return rc;
+  std::vector<const ModelName*> leaves(num_leaf_models);
+  for (int k = 0; k < num_leaf_models; ++k) {
+    if (int rc = find_layer(leaf_models[k] ? leaf_models[k] : "(null)", false, &leaves[k])) return rc;
+    if (int rc = check_leaf(leaves[k])) return rc;
+  }
+  const std::string spec = std::string(top->name) + "," + leaves[0]->name;
+  rmi_shard_build* b = nullptr;
+  if (int rc = rmi_shard_build_create(local, ends_all, world, rank, spec.c_str(), branch_factor, halo_capacity, buffers,
+                                      cuda_stream, &b)) {
+    std::string msg = rmi_last_error();
+    if (msg.rfind("rmi_shard_build_create", 0) == 0) msg = fn + msg.substr(strlen("rmi_shard_build_create"));
+    return fail(rc, msg);
+  }
+  b->batch = leaves;
+  int max_ppm = 2;
+  for (auto* lf : leaves) max_ppm = std::max(max_ppm, leaf_params_per_model(lf->kind));
+  const size_t rec = stats_record_bytes(), K = leaves.size();
+  bool ok = rec == RMI_SHARD_STATS_RECORD_BYTES &&
+            cudaMalloc((void**)&b->d_batch_params, sizeof(double) * branch_factor * max_ppm) == cudaSuccess &&
+            cudaMalloc((void**)&b->d_batch_aux, sizeof(BuildAux) * K) == cudaSuccess &&
+            cudaMalloc((void**)&b->d_batch_recs, rec * K * world) == cudaSuccess &&
+            cudaMalloc((void**)&b->d_batch_parts, stats_partial_bytes() * K * world) == cudaSuccess &&
+            cudaMallocHost((void**)&b->h_batch_recs, rec * K * world) == cudaSuccess;
+  if (!ok) { rmi_shard_build_destroy(b); return fail(RMI_ERR_CUDA, fn + ": device allocation failed"); }
+  *out = b;
+  return RMI_OK;
+}
+
+int rmi_shard_stats_leaf(rmi_shard_build* b, int k, void* d_record) {
+  if (!b || !d_record) return fail(RMI_ERR_INVALID, "rmi_shard_stats_leaf: null argument");
+  if (b->batch.empty() || k < 0 || k >= (int)b->batch.size())
+    return fail(RMI_ERR_INVALID, "rmi_shard_stats_leaf: not a leaf type of this statistics batch");
+  b->gather_mode = false;
+  CUDA_TRY(cudaSetDevice(b->ds->device));
+  return with_key_type(b->ds->key_type, [&](auto t) { return shard_stats_leaf_typed<decltype(t)>(b, k, (char*)d_record); });
+}
+
+int rmi_shard_stats_finish(rmi_shard_build* b, const void* d_records, uint32_t flags, rmi_result** out) {
+  (void)flags;
+  if (!b || !d_records || !out) return fail(RMI_ERR_INVALID, "rmi_shard_stats_finish: null argument");
+  if (b->batch.empty()) return fail(RMI_ERR_INVALID, "rmi_shard_stats_finish: not a statistics batch");
+  CUDA_TRY(cudaSetDevice(b->ds->device));
+  return shard_stats_results(b, (const char*)d_records, false, out);
+}
+
+int rmi_shard_train_stats_batch(rmi_shard_build* b, rmi_shard_comm* c, uint32_t flags, rmi_result** out) {
+  (void)flags;
+  g_last_error.clear();
+  if (!b || !c || !out) return fail(RMI_ERR_INVALID, "rmi_shard_train_stats_batch: null argument");
+  if (b->batch.empty()) return fail(RMI_ERR_INVALID, "rmi_shard_train_stats_batch: not a statistics batch");
+  if (c->world != b->world || c->rank != b->rank)
+    return fail(RMI_ERR_INVALID, "rmi_shard_train_stats_batch: the communicator is rank " + std::to_string(c->rank) + " of " +
+                                     std::to_string(c->world) + ", the build rank " + std::to_string(b->rank) + " of " +
+                                     std::to_string(b->world));
+  if (!nccl_api().ok) return fail(RMI_ERR_UNSUPPORTED, nccl_api().error);
+  CUDA_TRY(cudaSetDevice(b->ds->device));
+  return with_key_type(b->ds->key_type, [&](auto t) { return shard_stats_batch_typed<decltype(t)>(b, c, out); });
 }
 
 void rmi_shard_build_destroy(rmi_shard_build* b) {
@@ -2417,6 +2663,8 @@ void rmi_shard_build_destroy(rmi_shard_build* b) {
   if (b->h_off) cudaFreeHost(b->h_off);
   if (b->h_flags_all) cudaFreeHost(b->h_flags_all);
   for (cudaEvent_t e : {b->ev_off, b->ev_t0, b->ev_t1}) if (e) cudaEventDestroy(e);
+  cudaFree(b->d_batch_params); cudaFree(b->d_batch_aux); cudaFree(b->d_batch_recs); cudaFree(b->d_batch_parts);
+  if (b->h_batch_recs) cudaFreeHost(b->h_batch_recs);
   delete b;
 }
 

@@ -1652,8 +1652,13 @@ k_leaf(const T* __restrict__ keys, const Shard<T> sh, u64 N, const u64* __restri
   u64 cnt = g_hi - g_lo;
   if (g_hi == n && g_lo < g_hi) cnt += 1;   // the drained iterator's repeated final item
 
-  // two_layer.rs:226-259 widening
-  T next_key = next_idx < n ? keys[next_idx - sh.base] : Key<T>::max_value();
+  // two_layer.rs:226-259 widening.  The key after the leaf may live on a later rank: it is read from the halo, and a
+  // halo that does not reach it fails the build like a leaf that reaches past it (never a read past the keys held here)
+  T next_key = Key<T>::max_value();
+  if (next_idx < n) {
+    if (next_idx < sh.base + sh.n_avail) next_key = keys[next_idx - sh.base];
+    else set_status(aux, ST_HALO_TOO_SMALL);
+  }
   if (!have_prev) prev_key = Key<T>::zero_value();
   u64 first_idx = j == 0 ? S[1] : g_lo;                            // lb.next_index(max(j-1, 0))
   u64 up = leaf_predict64<LEAF>(f, Key<T>::as_float(Key<T>::minus_epsilon(next_key)));

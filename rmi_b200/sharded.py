@@ -29,6 +29,10 @@ only its own keys, and one all-reduce MAX of per-leaf maxima combines them.
 
 cache_fix_sharded fits the `--bounded` cache-fix spline over the same slabs (DESIGN.md section 16), knot for knot the
 single-GPU scan's, and train_bounded_sharded builds the bounded RMI over the knots without gathering them on one GPU.
+
+find_pareto_efficient_configs_sharded runs the configuration search over the same slabs (DESIGN.md section 9.1): the
+library's search loop, every (top, branching factor) group measured by train_stats_batch_sharded; train_for_size_sharded
+is built on it.
 """
 from __future__ import annotations
 
@@ -205,6 +209,12 @@ class CudaShardEngine:
         L.rmi_shard_comm_create.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p)]
         L.rmi_shard_comm_destroy.argtypes = [C.c_void_p]
         L.rmi_shard_train.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(C.POINTER(api._Result))]
+        L.rmi_shard_stats_batch_create.argtypes = [C.c_void_p, C.POINTER(_Ends), C.c_int, C.c_int, C.c_char_p,
+                                                   C.POINTER(C.c_char_p), C.c_int, C.c_uint64, C.c_uint64, C.POINTER(_Buffers),
+                                                   C.c_void_p, C.POINTER(C.c_void_p)]
+        L.rmi_shard_stats_leaf.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
+        L.rmi_shard_stats_finish.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(C.POINTER(api._Result))]
+        L.rmi_shard_train_stats_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(C.POINTER(api._Result))]
         self.device = data.buf.device
         self.ds = api.RMITrainingData.from_device(data.buf.data_ptr(), data.n_local, data.key_type,
                                                   self.device.index or 0, keep_alive=data.buf)
@@ -229,6 +239,39 @@ class CudaShardEngine:
                                                    C.byref(h)))
         self._build = h
         self._spec = spec
+
+    def begin_batch(self, ends_all: np.ndarray, world: int, rank: int, top: str, leaves: list[str], num_leaves: int, bufs: dict):
+        """A statistics-only batch of the leaf types `leaves` under one top model (rmi_shard_stats_batch_create)."""
+        key = ("batch", top, tuple(leaves), num_leaves, tuple(bufs[k].data_ptr() for k in sorted(bufs)))
+        if self._build is not None and getattr(self, "_build_key", None) == key:
+            return
+        self.end()
+        self._build_key = key
+        cb = _Buffers(*(bufs[k].data_ptr() for k in ("sums", "S", "params", "errors", "counts", "status")))
+        names = (C.c_char_p * len(leaves))(*[m.encode() for m in leaves])
+        h = C.c_void_p()
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        api._check(self.lib.rmi_shard_stats_batch_create(self.ds._h, _ends_array(ends_all), world, rank, top.encode(), names,
+                                                         len(leaves), num_leaves, self.data.halo_capacity, C.byref(cb),
+                                                         C.c_void_p(stream), C.byref(h)))
+        self._build = h
+        self._batch = [f"{top},{m}" for m in leaves]
+
+    def stats_leaf(self, k: int, record: torch.Tensor):
+        """Leaf type k of the batch over the leaves this rank owns: its record (STATS_RECORD_WORDS int64) into `record`."""
+        api._check(self.lib.rmi_shard_stats_leaf(self._build, int(k), C.c_void_p(record.data_ptr())))
+
+    def stats_finish(self, records: torch.Tensor, flags: int = 0):
+        """The batch's results from every rank's records (world x K records, rank by rank, on this device)."""
+        out = (C.POINTER(api._Result) * len(self._batch))()
+        api._check(self.lib.rmi_shard_stats_finish(self._build, C.c_void_p(records.data_ptr()), int(flags), out))
+        return [api.result_from_pointer(out[k], spec) for k, spec in enumerate(self._batch)]
+
+    def train_stats_batch(self, comm, flags: int = 0):
+        """The whole batch in one library call (rmi_shard_train_stats_batch)."""
+        out = (C.POINTER(api._Result) * len(self._batch))()
+        api._check(self.lib.rmi_shard_train_stats_batch(self._build, comm, int(flags), out))
+        return [api.result_from_pointer(out[k], spec) for k, spec in enumerate(self._batch)]
 
     def phase(self, k: int):
         api._check(self.lib.rmi_shard_phase(self._build, k))
@@ -378,6 +421,49 @@ def train_sharded(data, model_spec: str, num_leaves: int, flags: int = 0, group=
         bases.append(bases[-1] + int(n_local))
     n_global = bases[-1]
 
+    bufs = _buffers(data, N, ppm, dev)
+    eng.begin(ends_all, world, rank, model_spec, N, bufs)
+
+    comm = None
+    if native is not False and isinstance(eng, CudaShardEngine):
+        comm = native_comm(group, dev, single_rank_ok=native is True)
+        if native is True and comm is None:
+            raise api.RMIError("native=True needs an NCCL process group (or a single rank) and a loadable libnccl.so.2")
+    if comm is not None:
+        # halo keys are fetched once per data set (see step 4 below), then the whole build is one call
+        _fetch_halo_once(data, eng, bases, n_global, group, world, rank, dev)
+        try:
+            return eng.train(comm, int(flags) | (api.FLAG_LEAF_COUNTS if counts else 0))
+        except api.RMIPanic as e:
+            if "halo" not in str(e):
+                raise
+        return _retry_with_larger_halo(data, bufs, bases, n_global, N, model_spec, num_leaves, flags, group, world, dev, counts, native)
+
+    _host_top_and_bounds(data, eng, bufs, parts[0], bases, n_global, group, world, rank, dev)
+    # 5. leaves owned by this rank, then everyone gets everything
+    eng.phase(PHASE_LEAF)
+    if world > 1:
+        rec = bufs["records"]
+        dist.all_reduce(rec if counts else rec[: N * (ppm + 1)], op=dist.ReduceOp.SUM, group=group)
+        # the status word is a BIT MASK (kernels.h StatusBit): combine by OR, not MAX, so that every rank sees every
+        # rank's bits and all of them take the same decision below (retry with a larger halo / raise)
+        st_all = [torch.empty_like(bufs["status"]) for _ in range(world)]
+        dist.all_gather(st_all, bufs["status"], group=group)
+        acc = st_all[0].clone()
+        for t in st_all[1:]:
+            acc |= t
+        bufs["status"].copy_(acc)
+    eng.phase(PHASE_STATS)
+    try:
+        return eng.finish(int(flags) | (api.FLAG_LEAF_COUNTS if counts else 0))
+    except api.RMIPanic as e:
+        if world <= 1 or "halo" not in str(e):
+            raise
+    return _retry_with_larger_halo(data, bufs, bases, n_global, N, model_spec, num_leaves, flags, group, world, dev, counts, native)
+
+
+def _buffers(data, N: int, ppm: int, dev) -> dict:
+    """The device buffers of a build of N leaves with ppm parameters per leaf (cached on `data`)."""
     bufs = getattr(data, "_bufs", None)
     if bufs is None or bufs["S"].numel() != N + 1 or bufs["params"].numel() != N * ppm:
         # params | errors | counts live in ONE allocation so that a single all-reduce combines them
@@ -389,30 +475,24 @@ def train_sharded(data, model_spec: str, num_leaves: int, flags: int = 0, group=
                     counts=rec[N * (ppm + 1):],
                     status=torch.zeros(1, dtype=torch.int32, device=dev), records=rec)
         data._bufs = bufs
-    eng.begin(ends_all, world, rank, model_spec, N, bufs)
+    return bufs
 
-    comm = None
-    if native is not False and isinstance(eng, CudaShardEngine):
-        comm = native_comm(group, dev, single_rank_ok=native is True)
-        if native is True and comm is None:
-            raise api.RMIError("native=True needs an NCCL process group (or a single rank) and a loadable libnccl.so.2")
-    if comm is not None:
-        # halo keys are fetched once per data set (see step 4 below), then the whole build is one call
-        if getattr(data, "_halo_have", None) is None:
-            if world > 1:
-                cap = _min_halo_capacity(data, group, world, dev)
-                moves = plan_halo(bases, [bases[g + 1] + cap - 1 for g in range(world)], n_global)
-                data._halo_have = _exchange_halo(eng, moves, rank, group, dev)
-            else:
-                data._halo_have = 0
-        eng.set_halo(data._halo_have or 0)
-        try:
-            return eng.train(comm, int(flags) | (api.FLAG_LEAF_COUNTS if counts else 0))
-        except api.RMIPanic as e:
-            if "halo" not in str(e):
-                raise
-        return _retry_with_larger_halo(data, bufs, bases, n_global, N, model_spec, num_leaves, flags, group, world, dev, counts, native)
 
+def _fetch_halo_once(data, eng, bases, n_global, group, world, rank, dev):
+    """The first halo_capacity keys behind every slab, fetched once per data set (the keys are immutable)."""
+    if getattr(data, "_halo_have", None) is None:
+        if world > 1:
+            cap = _min_halo_capacity(data, group, world, dev)
+            moves = plan_halo(bases, [bases[g + 1] + cap - 1 for g in range(world)], n_global)
+            data._halo_have = _exchange_halo(eng, moves, rank, group, dev)
+        else:
+            data._halo_have = 0
+    eng.set_halo(data._halo_have or 0)
+
+
+def _host_top_and_bounds(data, eng, bufs, top, bases, n_global, group, world, rank, dev):
+    """Host-sequenced phases of a build up to the leaves: the top model with its collectives, the leaf boundaries
+    with their all-reduce MIN, the split, and the halo."""
     # 2. top model: local part -> tiny all-reduce(s) -> closed form (identical on every rank)
     def top_collective(kind):
         if world <= 1:
@@ -422,9 +502,9 @@ def train_sharded(data, model_spec: str, num_leaves: int, flags: int = 0, group=
         else:
             dist.all_reduce(bufs["sums"].view(torch.int64)[8:12], op=dist.ReduceOp.MIN, group=group)
 
-    rounds = TOP_ROUNDS.get(parts[0], ())
+    rounds = TOP_ROUNDS.get(top, ())
     eng.phase(PHASE_TOP_LOCAL)
-    if parts[0] in NATIVE_ONLY_TOPS and world > 1:
+    if top in NATIVE_ONLY_TOPS and world > 1:
         table = eng.top_table()
         if table is not None:
             # gloo cannot reduce device memory (one-GPU test boxes): stage through the host there
@@ -449,26 +529,6 @@ def train_sharded(data, model_spec: str, num_leaves: int, flags: int = 0, group=
         moves = plan_halo(bases, [bases[g + 1] + cap - 1 for g in range(world)], n_global)
         data._halo_have = _exchange_halo(eng, moves, rank, group, dev)
     eng.set_halo(getattr(data, "_halo_have", 0) or 0)
-    # 5. leaves owned by this rank, then everyone gets everything
-    eng.phase(PHASE_LEAF)
-    if world > 1:
-        rec = bufs["records"]
-        dist.all_reduce(rec if counts else rec[: N * (ppm + 1)], op=dist.ReduceOp.SUM, group=group)
-        # the status word is a BIT MASK (kernels.h StatusBit): combine by OR, not MAX, so that every rank sees every
-        # rank's bits and all of them take the same decision below (retry with a larger halo / raise)
-        st_all = [torch.empty_like(bufs["status"]) for _ in range(world)]
-        dist.all_gather(st_all, bufs["status"], group=group)
-        acc = st_all[0].clone()
-        for t in st_all[1:]:
-            acc |= t
-        bufs["status"].copy_(acc)
-    eng.phase(PHASE_STATS)
-    try:
-        return eng.finish(int(flags) | (api.FLAG_LEAF_COUNTS if counts else 0))
-    except api.RMIPanic as e:
-        if world <= 1 or "halo" not in str(e):
-            raise
-    return _retry_with_larger_halo(data, bufs, bases, n_global, N, model_spec, num_leaves, flags, group, world, dev, counts, native)
 
 
 def _merge_top_table(table: torch.Tensor, op: int, group, stage: bool):
@@ -547,6 +607,12 @@ def evaluate_sharded(trained, data, flags: int = 0, group=None, engine=None, cou
 def _retry_with_larger_halo(data, bufs, bases, n_global, N, model_spec, num_leaves, flags, group, world, dev, counts, native):
     # A leaf reaches past the prefetched halo (heavy skew).  The status word is the OR over ranks, so
     # every rank arrives here together: size the halo from the global boundaries S and build again.
+    _grow_halo(data, bufs, bases, n_global, N, group, world, dev)
+    return train_sharded(data, model_spec, num_leaves, flags, group, counts=counts, native=native)
+
+
+def _grow_halo(data, bufs, bases, n_global, N, group, world, dev):
+    """Re-home every slab behind a halo that holds the keys the boundaries S of the last build need (collective)."""
     S = bufs["S"]
     cuts = torch.tensor(bases[1:], dtype=torch.int64, device=dev)
     pos = torch.searchsorted(S, cuts).clamp_(max=N)
@@ -558,7 +624,123 @@ def _retry_with_larger_halo(data, bufs, bases, n_global, N, model_spec, num_leav
     if most <= _min_halo_capacity(data, group, world, dev) or not hasattr(data, "grow_halo"):
         raise api.RMIError(f"a leaf reaches further into the next rank than the halo capacity ({most} keys needed)")
     data.grow_halo(int(most * 1.25) + 1024)
-    return train_sharded(data, model_spec, num_leaves, flags, group, counts=counts, native=native)
+
+
+STATS_RECORD_WORDS = 6      # RMI_SHARD_STATS_RECORD_BYTES / 8: a rank's statistics partial and status words of one leaf type
+
+
+def train_stats_batch_sharded(data, top_model: str, leaf_models: list[str], num_leaves: int, flags: int = 0, group=None,
+                              engine=None, native: bool | None = None) -> list:
+    """api.train_stats_batch over a range-partitioned key array (DESIGN.md section 9): the statistics-only results of
+    "top_model,leaf" for every leaf of `leaf_models` at `num_leaves` leaves, the same list on every rank.  The top
+    model and the leaf boundaries are derived once; every rank fits only the leaves it owns, for every leaf type, and
+    one all-gather of K x 48 bytes per rank carries the statistics.  No result holds leaf tables.
+
+    native=None (default): with the CUDA engine over an NCCL group the batch is ONE library call
+    (rmi_shard_train_stats_batch); otherwise (gloo, the numpy engine, native=False) the phases are sequenced here.  A leaf
+    that reaches past the halo grows the halo (it never shrinks) and measures the batch again."""
+    eng = engine if engine is not None else data.engine
+    group = group if group is not None else getattr(data, "group", None)
+    rank, world = _world(group)
+    dev = eng.device
+    if top_model not in SHARDED_TOPS:
+        raise api.RMIError(f"range-partitioned builds offer the top models {SHARDED_TOPS}")
+    leaves = list(leaf_models)
+    if not leaves:
+        raise api.RMIError("train_stats_batch_sharded: no leaf models")
+    N = int(num_leaves)
+    ends_all = gather_ends(data, eng, group)
+    bases = [0]
+    for n_local in ends_all[:, 3]:
+        bases.append(bases[-1] + int(n_local))
+    n_global = bases[-1]
+    # the batch reads S, the sums, the error bounds, the counts and the status word; its leaf parameters go to its own
+    # scratch, so the buffers of a two-parameter leaf do for every leaf type
+    bufs = _buffers(data, N, _PPM.get(leaves[0], 2), dev)
+    eng.begin_batch(ends_all, world, rank, top_model, leaves, N, bufs)
+    comm = None
+    if native is not False and isinstance(eng, CudaShardEngine):
+        comm = native_comm(group, dev, single_rank_ok=native is True)
+        if native is True and comm is None:
+            raise api.RMIError("native=True needs an NCCL process group (or a single rank) and a loadable libnccl.so.2")
+    try:
+        if comm is not None:
+            _fetch_halo_once(data, eng, bases, n_global, group, world, rank, dev)
+            return eng.train_stats_batch(comm, int(flags))
+        _host_top_and_bounds(data, eng, bufs, top_model, bases, n_global, group, world, rank, dev)
+        K = len(leaves)
+        mine = torch.empty(K * STATS_RECORD_WORDS, dtype=torch.int64, device=dev)
+        for k in range(K):
+            eng.stats_leaf(k, mine[k * STATS_RECORD_WORDS:(k + 1) * STATS_RECORD_WORDS])
+        if world > 1:
+            # gloo cannot gather device memory (one-GPU test boxes): stage through the host there
+            stage = dev.type == "cuda" and dist.get_backend(group) == "gloo"
+            src = mine.cpu() if stage else mine
+            got = [torch.empty_like(src) for _ in range(world)]
+            dist.all_gather(got, src, group=group)
+            records = torch.cat(got).to(dev)
+        else:
+            records = mine
+        return eng.stats_finish(records, int(flags))
+    except api.RMIPanic as e:
+        if world <= 1 or "halo" not in str(e):
+            raise
+    _grow_halo(data, bufs, bases, n_global, N, group, world, dev)
+    return train_stats_batch_sharded(data, top_model, leaves, num_leaves, flags, group, native=native)
+
+
+_MEASURE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_char_p, C.c_uint64, C.POINTER(C.c_char_p), C.c_int, C.c_uint32,
+                          C.POINTER(api._ConfigStats))
+
+
+def find_pareto_efficient_configs_sharded(data, restrict_to: int = 10, flags: int = 0, group=None, native: bool | None = None,
+                                          engine=None) -> list[dict]:
+    """api.find_pareto_efficient_configs over a range-partitioned key array.  Collective: every rank calls it and every
+    rank returns the same list.  The search itself is the library's (host/optimizer.hpp, rmi_find_pareto_efficient_configs_with),
+    run on every rank over bit-identical merged statistics, so no rank coordinates the others; each (top model,
+    branching factor) group is measured by train_stats_batch_sharded.  RMI_OPTIMIZER_PROFILE selects the grid."""
+    L = api.load_library()
+    L.rmi_find_pareto_efficient_configs_with.argtypes = [_MEASURE_FN, C.c_void_p, C.c_uint64, C.c_uint32,
+                                                         C.POINTER(api._ConfigStats), C.c_uint64, C.POINTER(C.c_uint64)]
+    failures = []
+
+    def measure(_ctx, top, bf, leaves, k_count, fl, out):
+        try:
+            names = [leaves[k].decode() for k in range(k_count)]
+            res = train_stats_batch_sharded(data, top.decode(), names, int(bf), int(fl), group=group, engine=engine,
+                                            native=native)
+            for k, r in enumerate(res):
+                out[k].average_log2_error = r.model_avg_log2_error
+                out[k].max_log2_error = r.model_max_log2_error
+                out[k].size = api.rmi_size(r)
+            return 0
+        except BaseException as e:  # noqa: BLE001 - re-raised below, after the library has unwound the search
+            failures.append(e)
+            return 1
+
+    cb = _MEASURE_FN(measure)
+    cap = max(4096, int(restrict_to) if restrict_to < (1 << 20) else 0)
+    out = (api._ConfigStats * cap)()
+    cnt = C.c_uint64(0)
+    rc = L.rmi_find_pareto_efficient_configs_with(cb, None, int(restrict_to), int(flags), out, cap, C.byref(cnt))
+    if failures:
+        raise failures[0]
+    api._check(rc)
+    if int(cnt.value) > cap:
+        raise api.RMIError(f"Pareto front has {int(cnt.value)} entries, more than the {cap} this call can return")
+    return [dict(models=out[i].models.decode(), branching_factor=int(out[i].branching_factor),
+                 average_log2_error=float(out[i].average_log2_error), max_log2_error=float(out[i].max_log2_error),
+                 size=int(out[i].size)) for i in range(int(cnt.value))]
+
+
+def train_for_size_sharded(data, max_size: int, flags: int = 0, group=None, native: bool | None = None):
+    """api.train_for_size over a range-partitioned key array (collective): the first configuration of the un-narrowed
+    Pareto front smaller than max_size bytes, trained with train_sharded."""
+    front = find_pareto_efficient_configs_sharded(data, 1000, flags, group=group, native=native)
+    pick = next((c for c in front if c["size"] < max_size), None)
+    if pick is None:
+        raise api.RMIPanic(f"Could not find any configurations smaller than {max_size}")
+    return train_sharded(data, pick["models"], pick["branching_factor"], flags, group, native=native)
 
 
 def _exchange_halo(eng, moves, rank, group, dev) -> int:
