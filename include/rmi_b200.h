@@ -226,6 +226,26 @@ int rmi_index_lower_bound(const rmi_index* idx, const void* d_queries, uint64_t 
  * may be NULL) or lower_bound (*fallbacks, may be NULL, is SET to the fallback count) and copies the results back. */
 int rmi_index_lookup_host(const rmi_index* idx, const void* host_queries, uint64_t n, int lower_bound,
                           uint64_t* host_out, uint64_t* host_err, uint64_t* fallbacks);
+/* Upper bounds and equal ranges (DESIGN.md section 18), on either kind of index:
+ *   upper_bound  the number of keys k with k <= q (std::upper_bound for every non-NaN q; n for q >= the last key).  A
+ *                NaN query gives 0, so that equal_range(NaN) is the empty range [0, 0), as lower_bound(NaN) = 0.  Keys
+ *                compare by value: -0.0 <= 0.0.  The search runs in the same window as lower_bound's: the model's
+ *                error bounds cover the runs of equal keys (the reference widens each leaf's bound by its longest
+ *                run), so for a key of the data set the window holds both ends of its run; a query >= the last key
+ *                gets n without a search, because the data set's final run is the one no bound records.
+ *   equal_range  (lower_bound(q), upper_bound(q)), half-open, in two arrays, from one model evaluation and one window;
+ *                d_first is bit-equal to what rmi_index_lower_bound returns.
+ * Always exact: a window that misses takes the galloping fallback.  *d_fallbacks (may be NULL) is incremented by the
+ * number of queries whose window missed (for equal_range, a query counts once if either end missed); never, for a key
+ * of the data set on a plain index.  One kernel launch per call (n == 0: none), enqueued on cuda_stream. */
+int rmi_index_upper_bound(const rmi_index* idx, const void* d_queries, uint64_t n, uint64_t* d_out,
+                          uint64_t* d_fallbacks, void* cuda_stream);
+int rmi_index_equal_range(const rmi_index* idx, const void* d_queries, uint64_t n, uint64_t* d_first,
+                          uint64_t* d_last, uint64_t* d_fallbacks, void* cuda_stream);
+/* The same on host arrays, synchronously: upper bounds into host_last, and with host_first non-NULL the equal range
+ * (lower bounds into host_first).  *fallbacks (may be NULL) is SET to the fallback count. */
+int rmi_index_range_host(const rmi_index* idx, const void* host_queries, uint64_t n, uint64_t* host_first,
+                         uint64_t* host_last, uint64_t* fallbacks);
 
 /* ---- Range-partitioned (multi-GPU) build ----------------------------------------------------
  * One process per GPU; rank r holds the r-th contiguous slab of the globally sorted key array
@@ -419,7 +439,24 @@ int rmi_shard_index_gather(const rmi_shard_index* idx, const uint64_t* d_slot, c
  * Returns after the exchanges are enqueued; the answers are in d_out when cuda_stream reaches them. */
 int rmi_shard_index_lower_bound(rmi_shard_index* idx, rmi_shard_comm* c, const void* d_queries, uint64_t n,
                                 uint64_t* d_out, uint64_t* d_fallbacks, void* cuda_stream);
-/* What the last rmi_shard_index_lower_bound on this index did (waits for it to finish).  phase_ms: CUDA-event times of
+/* Upper bounds over the slabs (DESIGN.md section 18), as the lower bound above but routed by <=: query q goes to the last
+ * non-empty rank whose first key is <= q (the first non-empty rank if none is, a NaN query included).  Every key
+ * before that rank's slab is <= q and every key after it is > q, so the global upper bound (the number of keys <= q;
+ * 0 for NaN) is the slab's base + the upper bound inside the slab; the routing differs from the lower bound's only
+ * for a query equal to some slab's first key.  route_upper and search_upper are the phases (launches as for route and
+ * search; rmi_shard_index_gather completes them), and on a bounded index search_upper searches the key line as
+ * lower_bound does (section 18 shows the halo of section 17 still covers its reads).  A query >= the last key of the
+ * slab it reaches gets base + n_local without a search, and is not counted.  rmi_shard_index_upper_bound is the
+ * one-call form over c, with the exchange code of rmi_shard_index_lower_bound.  All take plain and bounded indexes,
+ * with the checks of the lower-bound calls.  An equal range over the slabs is a lower_bound and an upper_bound. */
+int rmi_shard_index_route_upper(const rmi_shard_index* idx, const void* d_queries, uint64_t n, void* d_send,
+                                uint64_t* d_slot, uint64_t* d_send_counts, void* cuda_stream);
+int rmi_shard_index_search_upper(const rmi_shard_index* idx, const void* d_received, uint64_t m, uint64_t* d_answers,
+                                 uint64_t* d_fallbacks, void* cuda_stream);
+int rmi_shard_index_upper_bound(rmi_shard_index* idx, rmi_shard_comm* c, const void* d_queries, uint64_t n,
+                                uint64_t* d_out, uint64_t* d_fallbacks, void* cuda_stream);
+/* What the last one-call lookup on this index (rmi_shard_index_lower_bound, rmi_shard_index_upper_bound or, on a
+ * bounded index, rmi_shard_index_predict_collective) did (waits for it to finish).  phase_ms: CUDA-event times of
  * route, count exchange with the host read, query exchange, search, answer exchange, gather. */
 typedef struct {
   float phase_ms[6];

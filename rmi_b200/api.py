@@ -112,6 +112,10 @@ def load_library():
         L.rmi_index_lower_bound.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]
         L.rmi_index_lookup_host.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_void_p, C.c_void_p,
                                             C.c_void_p]
+        L.rmi_index_upper_bound.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.rmi_index_equal_range.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p]
+        L.rmi_index_range_host.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib = L
     return _lib
 
@@ -473,8 +477,10 @@ class RMIIndex:
     """A trained RMI bound to the device-resident keys it was trained on, for batched lookups on the GPU.
 
     ``predict(q)`` returns the generated code's ``lookup(key, &err)`` for every query as ``(pos, err)``;
-    ``lower_bound(q)`` returns the exact number of keys below each query (``std::lower_bound``).  Both take a
-    numpy array of the dataset's key type and return ``np.uint64`` arrays.  The ``*_device`` forms take raw device
+    ``lower_bound(q)`` returns the exact number of keys below each query (``std::lower_bound``), ``upper_bound(q)``
+    the number of keys <= each query (``std::upper_bound``; 0 for NaN) and ``equal_range(q)`` both, from one window
+    per query (DESIGN §18).  All take a numpy array of the dataset's key type and return ``np.uint64`` arrays.  The
+    ``*_device`` forms take raw device
     pointers and a CUDA stream handle (torch: ``t.data_ptr()``, ``torch.cuda.current_stream().cuda_stream``) and
     enqueue one kernel without synchronising.  ``trained`` must hold its leaf tables (not FLAG_STATS_ONLY) and
     ``data`` must be the key set it was trained on; the index keeps ``data`` alive.
@@ -533,6 +539,28 @@ class RMIIndex:
                                                      out.ctypes.data_as(C.c_void_p), None, C.byref(fb)))
         return (out, int(fb.value)) if return_fallbacks else out
 
+    def upper_bound(self, q: np.ndarray, return_fallbacks: bool = False):
+        """Exact upper bound per query (np.uint64): the number of keys <= q, 0 for NaN; with return_fallbacks also
+        the number of queries whose error window missed the answer."""
+        q = self._queries(q)
+        last = np.empty(q.size, dtype=np.uint64)
+        fb = C.c_uint64(0)
+        _check(load_library().rmi_index_range_host(self._h, q.ctypes.data_as(C.c_void_p), q.size, None,
+                                                    last.ctypes.data_as(C.c_void_p), C.byref(fb)))
+        return (last, int(fb.value)) if return_fallbacks else last
+
+    def equal_range(self, q: np.ndarray, return_fallbacks: bool = False):
+        """(first, last) per query, the half-open range of keys equal to q: first is lower_bound(q), last is
+        upper_bound(q); with return_fallbacks also the number of queries whose window missed either end."""
+        q = self._queries(q)
+        first = np.empty(q.size, dtype=np.uint64)
+        last = np.empty(q.size, dtype=np.uint64)
+        fb = C.c_uint64(0)
+        _check(load_library().rmi_index_range_host(self._h, q.ctypes.data_as(C.c_void_p), q.size,
+                                                    first.ctypes.data_as(C.c_void_p), last.ctypes.data_as(C.c_void_p),
+                                                    C.byref(fb)))
+        return (first, last, int(fb.value)) if return_fallbacks else (first, last)
+
     def predict_device(self, q_ptr: int, n: int, pos_ptr: int, err_ptr: int = 0, stream: int = 0) -> None:
         _check(load_library().rmi_index_predict(self._h, C.c_void_p(q_ptr), int(n), C.c_void_p(pos_ptr),
                                                 C.c_void_p(err_ptr or None), C.c_void_p(stream or None)))
@@ -540,6 +568,16 @@ class RMIIndex:
     def lower_bound_device(self, q_ptr: int, n: int, out_ptr: int, fallbacks_ptr: int = 0, stream: int = 0) -> None:
         _check(load_library().rmi_index_lower_bound(self._h, C.c_void_p(q_ptr), int(n), C.c_void_p(out_ptr),
                                                     C.c_void_p(fallbacks_ptr or None), C.c_void_p(stream or None)))
+
+    def upper_bound_device(self, q_ptr: int, n: int, out_ptr: int, fallbacks_ptr: int = 0, stream: int = 0) -> None:
+        _check(load_library().rmi_index_upper_bound(self._h, C.c_void_p(q_ptr), int(n), C.c_void_p(out_ptr),
+                                                    C.c_void_p(fallbacks_ptr or None), C.c_void_p(stream or None)))
+
+    def equal_range_device(self, q_ptr: int, n: int, first_ptr: int, last_ptr: int, fallbacks_ptr: int = 0,
+                           stream: int = 0) -> None:
+        _check(load_library().rmi_index_equal_range(self._h, C.c_void_p(q_ptr), int(n), C.c_void_p(first_ptr),
+                                                    C.c_void_p(last_ptr), C.c_void_p(fallbacks_ptr or None),
+                                                    C.c_void_p(stream or None)))
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:

@@ -822,6 +822,7 @@ struct rmi_index {
   void* d_knots = nullptr;   // K x rmi_spline_point
   uint64_t K = 0;
   uint64_t line_size = 0;
+  uint64_t last_key_bits = 0;   // ds's last key (raw bits, u32 zero-extended): upper bounds of queries >= it are n
 };
 
 namespace {
@@ -858,6 +859,68 @@ int index_launch(const rmi_index* idx, const void* d_queries, uint64_t n, uint64
   CUDA_TRY(cudaGetLastError());
   return RMI_OK;
 }
+// Upper bounds into d_last, and with d_first non-null the lower bounds too (equal_range): one launch.
+int index_launch_range(const rmi_index* idx, const void* d_queries, uint64_t n, uint64_t* d_first, uint64_t* d_last,
+                       uint64_t* d_fallbacks, void* cuda_stream) {
+  if (n == 0) return RMI_OK;
+  const rmi_dataset* ds = idx->ds;
+  CUDA_TRY(cudaSetDevice(ds->device));
+  Launch L{(cudaStream_t)cuda_stream, idx->num_sms};
+  if (idx->d_knots) {
+    lookup_bounded_range_batch(L, idx->top, idx->leaf_kind, idx->d_records, idx->N, idx->d_knots, idx->K,
+                               idx->line_size, (const u64*)ds->d_keys, idx->n, idx->last_key_bits,
+                               (const u64*)d_queries, n, (u64*)d_first, (u64*)d_last, (u64*)d_fallbacks);
+    CUDA_TRY(cudaGetLastError());
+    return RMI_OK;
+  }
+  with_key_type(ds->key_type, [&](auto k) {
+    using T = decltype(k);
+    lookup_range_batch<T>(L, idx->top, idx->leaf_kind, idx->d_records, idx->N, (const T*)ds->d_keys, idx->n,
+                          rmihost::key_from_bits<T>(idx->last_key_bits), (const T*)d_queries, n, (u64*)d_first,
+                          (u64*)d_last, (u64*)d_fallbacks);
+  });
+  CUDA_TRY(cudaGetLastError());
+  return RMI_OK;
+}
+
+// The host-array form of a lookup, synchronously on a stream of its own: copies the n queries to the device, runs
+// launch(d_q, d_a, d_b, d_fallbacks, stream) (d_b null when host_b is; *d_fallbacks starts at 0) and copies d_a to
+// host_a, d_b to host_b and the fallback count to *fallbacks where those are given.
+template <class Launch_>
+int index_host_call(const rmi_index* idx, const void* host_queries, uint64_t n, uint64_t* host_a, uint64_t* host_b,
+                    uint64_t* fallbacks, const char* fn, Launch_&& launch) {
+  if (n == 0) return RMI_OK;
+  CUDA_TRY(cudaSetDevice(idx->ds->device));
+  const size_t qb = (size_t)n * key_bytes(idx->ds->key_type), ob = (size_t)n * sizeof(uint64_t);
+  cudaStream_t st = nullptr;
+  char* d = nullptr;   // queries | a | b | fallback counter
+  cudaError_t e = cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking);
+  if (e == cudaSuccess) e = cudaMallocAsync((void**)&d, qb + 2 * ob + 8 + 8, st);
+  int rc = RMI_OK;
+  if (e == cudaSuccess) {
+    char* d_q = d;
+    uint64_t* d_a = (uint64_t*)(d + ((qb + 7) & ~(size_t)7));
+    uint64_t* d_b = d_a + n;
+    uint64_t* d_fb = d_b + n;
+    e = cudaMemcpyAsync(d_q, host_queries, qb, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(d_fb, 0, sizeof(u64), st);
+    if (e == cudaSuccess) rc = launch(d_q, d_a, host_b ? d_b : nullptr, d_fb, st);
+    if (e == cudaSuccess && rc == RMI_OK) e = cudaMemcpyAsync(host_a, d_a, ob, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess && rc == RMI_OK && host_b) e = cudaMemcpyAsync(host_b, d_b, ob, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess && rc == RMI_OK && fallbacks)
+      e = cudaMemcpyAsync(fallbacks, d_fb, sizeof(u64), cudaMemcpyDeviceToHost, st);
+    cudaFreeAsync(d, st);
+  }
+  if (st) {
+    cudaError_t es = cudaStreamSynchronize(st);
+    if (e == cudaSuccess) e = es;
+    cudaStreamDestroy(st);
+  }
+  if (rc != RMI_OK) return rc;
+  if (e != cudaSuccess) return fail(RMI_ERR_CUDA, std::string(fn) + ": " + cudaGetErrorString(e));
+  return RMI_OK;
+}
+
 // After check_result, the checks every kind of index shares: r must have been trained on `rows` rows (the dataset's
 // keys, the knots of a bounded index, or the keys of all slabs of a range-partitioned one), which `holder` names in
 // the message; `keys` is the number of keys the index searches (0: an empty index).  Messages name `fn`.
@@ -887,6 +950,10 @@ int index_upload(const rmi_result* r, const rmi_dataset* ds, uint64_t n, const r
   idx->top = idx->tables.given(*r);
   if (e == cudaSuccess) e = cudaMalloc(&idx->d_records, packed.size());
   if (e == cudaSuccess) e = cudaMemcpy(idx->d_records, packed.data(), packed.size(), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess && ds->n > 0) {
+    const size_t kb = key_bytes(ds->key_type);
+    e = cudaMemcpy(&idx->last_key_bits, (const char*)ds->d_keys + (ds->n - 1) * kb, kb, cudaMemcpyDeviceToHost);
+  }
   if (e == cudaSuccess && knots) {
     e = cudaMalloc(&idx->d_knots, sizeof(rmi_spline_point) * K);
     if (e == cudaSuccess) e = cudaMemcpy(idx->d_knots, knots, sizeof(rmi_spline_point) * K, cudaMemcpyHostToDevice);
@@ -956,43 +1023,38 @@ int rmi_index_lower_bound(const rmi_index* idx, const void* d_queries, uint64_t 
   return index_launch(idx, d_queries, n, d_out, nullptr, d_fallbacks, cuda_stream, true);
 }
 
+int rmi_index_upper_bound(const rmi_index* idx, const void* d_queries, uint64_t n, uint64_t* d_out,
+                          uint64_t* d_fallbacks, void* cuda_stream) {
+  if (int rc = index_check_call(idx, d_queries, n, d_out, "rmi_index_upper_bound")) return rc;
+  return index_launch_range(idx, d_queries, n, nullptr, d_out, d_fallbacks, cuda_stream);
+}
+
+int rmi_index_equal_range(const rmi_index* idx, const void* d_queries, uint64_t n, uint64_t* d_first, uint64_t* d_last,
+                          uint64_t* d_fallbacks, void* cuda_stream) {
+  if (int rc = index_check_call(idx, d_queries, n, d_last, "rmi_index_equal_range")) return rc;
+  if (n && !d_first) return fail(RMI_ERR_INVALID, "rmi_index_equal_range: null query or output pointer");
+  return index_launch_range(idx, d_queries, n, d_first, d_last, d_fallbacks, cuda_stream);
+}
+
+int rmi_index_range_host(const rmi_index* idx, const void* host_queries, uint64_t n, uint64_t* host_first,
+                         uint64_t* host_last, uint64_t* fallbacks) {
+  if (int rc = index_check_call(idx, host_queries, n, host_last, "rmi_index_range_host")) return rc;
+  if (fallbacks) *fallbacks = 0;
+  return index_host_call(idx, host_queries, n, host_last, host_first, fallbacks, "rmi_index_range_host",
+                         [&](const void* d_q, uint64_t* d_last, uint64_t* d_first, uint64_t* d_fb, cudaStream_t st) {
+                           return index_launch_range(idx, d_q, n, d_first, d_last, d_fb, st);
+                         });
+}
+
 int rmi_index_lookup_host(const rmi_index* idx, const void* host_queries, uint64_t n, int lower_bound,
                           uint64_t* host_out, uint64_t* host_err, uint64_t* fallbacks) {
   if (int rc = index_check_call(idx, host_queries, n, host_out, "rmi_index_lookup_host")) return rc;
-  if (n == 0) return RMI_OK;
-  CUDA_TRY(cudaSetDevice(idx->ds->device));
-  const size_t qb = (size_t)n * key_bytes(idx->ds->key_type), ob = (size_t)n * sizeof(uint64_t);
-  cudaStream_t st = nullptr;
-  char* d = nullptr;   // queries | out | err | fallback counter
-  cudaError_t e = cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaMallocAsync((void**)&d, qb + 2 * ob + 8 + 8, st);
-  int rc = RMI_OK;
-  if (e == cudaSuccess) {
-    char* d_q = d;
-    uint64_t* d_out = (uint64_t*)(d + ((qb + 7) & ~(size_t)7));
-    uint64_t* d_err = d_out + n;
-    uint64_t* d_fb = d_err + n;
-    e = cudaMemcpyAsync(d_q, host_queries, qb, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_fb, 0, sizeof(u64), st);
-    if (e == cudaSuccess) {
-      rc = lower_bound ? index_launch(idx, d_q, n, d_out, nullptr, d_fb, st, true)
-                       : index_launch(idx, d_q, n, d_out, host_err ? d_err : nullptr, nullptr, st, false);
-    }
-    if (e == cudaSuccess && rc == RMI_OK) e = cudaMemcpyAsync(host_out, d_out, ob, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess && rc == RMI_OK && !lower_bound && host_err)
-      e = cudaMemcpyAsync(host_err, d_err, ob, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess && rc == RMI_OK && lower_bound && fallbacks)
-      e = cudaMemcpyAsync(fallbacks, d_fb, sizeof(u64), cudaMemcpyDeviceToHost, st);
-    cudaFreeAsync(d, st);
-  }
-  if (st) {
-    cudaError_t es = cudaStreamSynchronize(st);
-    if (e == cudaSuccess) e = es;
-    cudaStreamDestroy(st);
-  }
-  if (rc != RMI_OK) return rc;
-  if (e != cudaSuccess) return fail(RMI_ERR_CUDA, std::string("rmi_index_lookup_host: ") + cudaGetErrorString(e));
-  return RMI_OK;
+  return index_host_call(idx, host_queries, n, host_out, lower_bound ? nullptr : host_err,
+                         lower_bound ? fallbacks : nullptr, "rmi_index_lookup_host",
+                         [&](const void* d_q, uint64_t* d_out, uint64_t* d_err, uint64_t* d_fb, cudaStream_t st) {
+                           return lower_bound ? index_launch(idx, d_q, n, d_out, nullptr, d_fb, st, true)
+                                              : index_launch(idx, d_q, n, d_out, d_err, nullptr, st, false);
+                         });
 }
 
 }  // extern "C"
@@ -2717,32 +2779,35 @@ struct PoolScratch {
 
 size_t round8(size_t b) { return (b + 7) & ~(size_t)7; }
 
+// upper: route by <= for upper bounds (DESIGN §18)
 template <class T>
 int shard_lookup_route(const rmi_shard_index* si, const T* d_q, uint64_t n, T* d_send, u64* d_slot, u64* d_counts,
-                       cudaStream_t st) {
+                       cudaStream_t st, bool upper) {
   const u64 nb = shard_route_blocks(n), W = (u64)si->world;
   PoolScratch s{nullptr, st};
   if (n) CUDA_TRY(cudaMallocAsync(&s.p, nb * W * (sizeof(u64) + sizeof(u32)), st));
   Launch L{st, si->idx->num_sms};
   shard_route<T>(L, shard_route_of<T>(si), si->world, d_q, n, (u32*)((u64*)s.p + nb * W), (u64*)s.p, d_send, d_slot,
-                 d_counts);
+                 d_counts, upper);
   CUDA_TRY(cudaGetLastError());
   return RMI_OK;
 }
 
+// upper: upper bounds of queries routed by <=
 template <class T>
 int shard_lookup_search(const rmi_shard_index* si, const T* d_recv, uint64_t m, u64* d_answers, u64* d_fallbacks,
-                        cudaStream_t st) {
+                        cudaStream_t st, bool upper) {
   if (m == 0) return RMI_OK;
   const rmi_index* idx = si->idx;
   const rmi_dataset* ds = idx->ds;
   if (ds->n == 0)
-    return fail(RMI_ERR_INVALID, "rmi_shard_index_search: this rank holds no keys, so no query is routed to it");
+    return fail(RMI_ERR_INVALID, std::string(upper ? "rmi_shard_index_search_upper" : "rmi_shard_index_search") +
+                                     ": this rank holds no keys, so no query is routed to it");
   if constexpr (std::is_same<T, u64>::value) {
     if (si->d_knots) {
       Launch L{st, idx->num_sms};
       shard_bounded_search(L, idx->top, idx->leaf_kind, idx->d_records, idx->N, si->ks, (const u64*)ds->d_keys, ds->n,
-                           si->base, si->n_global, d_recv, m, d_answers, d_fallbacks, true);
+                           si->base, si->n_global, d_recv, m, d_answers, d_fallbacks, true, upper, idx->last_key_bits);
       CUDA_TRY(cudaGetLastError());
       return RMI_OK;
     }
@@ -2753,7 +2818,7 @@ int shard_lookup_search(const rmi_shard_index* si, const T* d_recv, uint64_t m, 
   if (int rc = index_launch(idx, d_recv, m, pos, pos + m, nullptr, st, false)) return rc;
   Launch L{st, idx->num_sms};
   shard_search<T>(L, (const T*)ds->d_keys, ds->n, si->base, si->n_global, d_recv, m, (const u64*)pos,
-                  (const u64*)pos + m, d_answers, d_fallbacks);
+                  (const u64*)pos + m, d_answers, d_fallbacks, upper, rmihost::key_from_bits<T>(idx->last_key_bits));
   CUDA_TRY(cudaGetLastError());
   return RMI_OK;
 }
@@ -2779,7 +2844,7 @@ int shard_predict_route(const rmi_shard_index* si, const u64* d_q, uint64_t n, u
   PoolScratch s2{nullptr, st};
   if (n) CUDA_TRY(cudaMallocAsync(&s2.p, nb * W * (sizeof(u64) + sizeof(u32)), st));
   shard_route<u64>(L, route, si->world, (const u64*)pos, n, (u32*)((u64*)s2.p + nb * W), (u64*)s2.p, d_send, d_slot,
-                   d_counts);
+                   d_counts, false);
   shard_scatter_queries(L, d_q, d_slot, n, d_send);
   CUDA_TRY(cudaGetLastError());
   return RMI_OK;
@@ -2867,11 +2932,15 @@ int shard_one_call(rmi_shard_index* si, rmi_shard_comm* c, uint64_t n, u64* d_ou
 
 template <class T>
 int shard_lookup_one_call(rmi_shard_index* si, rmi_shard_comm* c, const T* d_q, uint64_t n, u64* d_out, u64* d_fallbacks,
-                          cudaStream_t st) {
+                          cudaStream_t st, bool upper) {
   return shard_one_call<T>(
-      si, c, n, d_out, st, "rmi_shard_index_lower_bound",
-      [&](T* d_send, u64* d_slot, u64* d_counts) { return shard_lookup_route<T>(si, d_q, n, d_send, d_slot, d_counts, st); },
-      [&](const T* d_recv, u64 m, u64* d_ans) { return shard_lookup_search<T>(si, d_recv, m, d_ans, d_fallbacks, st); });
+      si, c, n, d_out, st, upper ? "rmi_shard_index_upper_bound" : "rmi_shard_index_lower_bound",
+      [&](T* d_send, u64* d_slot, u64* d_counts) {
+        return shard_lookup_route<T>(si, d_q, n, d_send, d_slot, d_counts, st, upper);
+      },
+      [&](const T* d_recv, u64 m, u64* d_ans) {
+        return shard_lookup_search<T>(si, d_recv, m, d_ans, d_fallbacks, st, upper);
+      });
 }
 
 // The checks of a call that takes a communicator (the one-call forms).
@@ -2949,29 +3018,71 @@ int rmi_shard_index_predict(const rmi_shard_index* si, const void* d_queries, ui
   return index_launch(si->idx, d_queries, n, d_pos, d_err, nullptr, cuda_stream, false);
 }
 
-int rmi_shard_index_route(const rmi_shard_index* si, const void* d_queries, uint64_t n, void* d_send, uint64_t* d_slot,
-                          uint64_t* d_send_counts, void* cuda_stream) {
-  const char* fn = "rmi_shard_index_route";
+}  // extern "C"
+
+namespace {
+int shard_route_call(const rmi_shard_index* si, const void* d_queries, uint64_t n, void* d_send, uint64_t* d_slot,
+                     uint64_t* d_send_counts, void* cuda_stream, bool upper) {
+  const char* fn = upper ? "rmi_shard_index_route_upper" : "rmi_shard_index_route";
   if (!si || !d_send_counts) return fail(RMI_ERR_INVALID, std::string(fn) + ": null index or count pointer");
   if (n && (!d_queries || !d_send || !d_slot)) return fail(RMI_ERR_INVALID, std::string(fn) + ": null query, send or slot pointer");
   CUDA_TRY(cudaSetDevice(si->idx->ds->device));
   return with_key_type(si->idx->ds->key_type, [&](auto k) {
     using T = decltype(k);
     return shard_lookup_route<T>(si, (const T*)d_queries, n, (T*)d_send, (u64*)d_slot, (u64*)d_send_counts,
-                                 (cudaStream_t)cuda_stream);
+                                 (cudaStream_t)cuda_stream, upper);
   });
 }
 
-int rmi_shard_index_search(const rmi_shard_index* si, const void* d_received, uint64_t m, uint64_t* d_answers,
-                           uint64_t* d_fallbacks, void* cuda_stream) {
-  if (!si) return fail(RMI_ERR_INVALID, "rmi_shard_index_search: null index");
-  if (int rc = index_check_call(si->idx, d_received, m, d_answers, "rmi_shard_index_search")) return rc;
+int shard_search_call(const rmi_shard_index* si, const void* d_received, uint64_t m, uint64_t* d_answers,
+                      uint64_t* d_fallbacks, void* cuda_stream, bool upper) {
+  const char* fn = upper ? "rmi_shard_index_search_upper" : "rmi_shard_index_search";
+  if (!si) return fail(RMI_ERR_INVALID, std::string(fn) + ": null index");
+  if (int rc = index_check_call(si->idx, d_received, m, d_answers, fn)) return rc;
   CUDA_TRY(cudaSetDevice(si->idx->ds->device));
   return with_key_type(si->idx->ds->key_type, [&](auto k) {
     using T = decltype(k);
     return shard_lookup_search<T>(si, (const T*)d_received, m, (u64*)d_answers, (u64*)d_fallbacks,
-                                  (cudaStream_t)cuda_stream);
+                                  (cudaStream_t)cuda_stream, upper);
   });
+}
+
+int shard_bound_call(rmi_shard_index* si, rmi_shard_comm* c, const void* d_queries, uint64_t n, uint64_t* d_out,
+                     uint64_t* d_fallbacks, void* cuda_stream, bool upper) {
+  const char* fn = upper ? "rmi_shard_index_upper_bound" : "rmi_shard_index_lower_bound";
+  g_last_error.clear();
+  if (!si || !c) return fail(RMI_ERR_INVALID, std::string(fn) + ": null index or communicator");
+  if (n && (!d_queries || !d_out)) return fail(RMI_ERR_INVALID, std::string(fn) + ": null query or output pointer");
+  if (int rc = shard_check_comm(si, c, fn)) return rc;
+  CUDA_TRY(cudaSetDevice(si->idx->ds->device));
+  return with_key_type(si->idx->ds->key_type, [&](auto k) {
+    using T = decltype(k);
+    return shard_lookup_one_call<T>(si, c, (const T*)d_queries, n, (u64*)d_out, (u64*)d_fallbacks,
+                                    (cudaStream_t)cuda_stream, upper);
+  });
+}
+}  // namespace
+
+extern "C" {
+
+int rmi_shard_index_route(const rmi_shard_index* si, const void* d_queries, uint64_t n, void* d_send, uint64_t* d_slot,
+                          uint64_t* d_send_counts, void* cuda_stream) {
+  return shard_route_call(si, d_queries, n, d_send, d_slot, d_send_counts, cuda_stream, false);
+}
+
+int rmi_shard_index_route_upper(const rmi_shard_index* si, const void* d_queries, uint64_t n, void* d_send,
+                                uint64_t* d_slot, uint64_t* d_send_counts, void* cuda_stream) {
+  return shard_route_call(si, d_queries, n, d_send, d_slot, d_send_counts, cuda_stream, true);
+}
+
+int rmi_shard_index_search(const rmi_shard_index* si, const void* d_received, uint64_t m, uint64_t* d_answers,
+                           uint64_t* d_fallbacks, void* cuda_stream) {
+  return shard_search_call(si, d_received, m, d_answers, d_fallbacks, cuda_stream, false);
+}
+
+int rmi_shard_index_search_upper(const rmi_shard_index* si, const void* d_received, uint64_t m, uint64_t* d_answers,
+                                 uint64_t* d_fallbacks, void* cuda_stream) {
+  return shard_search_call(si, d_received, m, d_answers, d_fallbacks, cuda_stream, true);
 }
 
 int rmi_shard_index_gather(const rmi_shard_index* si, const uint64_t* d_slot, const uint64_t* d_returned, uint64_t n,
@@ -2987,22 +3098,17 @@ int rmi_shard_index_gather(const rmi_shard_index* si, const uint64_t* d_slot, co
 
 int rmi_shard_index_lower_bound(rmi_shard_index* si, rmi_shard_comm* c, const void* d_queries, uint64_t n,
                                 uint64_t* d_out, uint64_t* d_fallbacks, void* cuda_stream) {
-  const char* fn = "rmi_shard_index_lower_bound";
-  g_last_error.clear();
-  if (!si || !c) return fail(RMI_ERR_INVALID, std::string(fn) + ": null index or communicator");
-  if (n && (!d_queries || !d_out)) return fail(RMI_ERR_INVALID, std::string(fn) + ": null query or output pointer");
-  if (int rc = shard_check_comm(si, c, fn)) return rc;
-  CUDA_TRY(cudaSetDevice(si->idx->ds->device));
-  return with_key_type(si->idx->ds->key_type, [&](auto k) {
-    using T = decltype(k);
-    return shard_lookup_one_call<T>(si, c, (const T*)d_queries, n, (u64*)d_out, (u64*)d_fallbacks,
-                                    (cudaStream_t)cuda_stream);
-  });
+  return shard_bound_call(si, c, d_queries, n, d_out, d_fallbacks, cuda_stream, false);
+}
+
+int rmi_shard_index_upper_bound(rmi_shard_index* si, rmi_shard_comm* c, const void* d_queries, uint64_t n,
+                                uint64_t* d_out, uint64_t* d_fallbacks, void* cuda_stream) {
+  return shard_bound_call(si, c, d_queries, n, d_out, d_fallbacks, cuda_stream, true);
 }
 
 int rmi_shard_index_last_stats(const rmi_shard_index* si, rmi_shard_lookup_stats* out) {
   if (!si || !out) return fail(RMI_ERR_INVALID, "rmi_shard_index_last_stats: null argument");
-  if (!si->ran) return fail(RMI_ERR_INVALID, "rmi_shard_index_last_stats: no rmi_shard_index_lower_bound has run");
+  if (!si->ran) return fail(RMI_ERR_INVALID, "rmi_shard_index_last_stats: no one-call lookup has run");
   CUDA_TRY(cudaEventSynchronize(si->ev[SHARD_LOOKUP_EVENTS - 1]));
   *out = si->last;
   for (int q = 0; q + 1 < SHARD_LOOKUP_EVENTS; ++q) CUDA_TRY(cudaEventElapsedTime(&out->phase_ms[q], si->ev[q], si->ev[q + 1]));

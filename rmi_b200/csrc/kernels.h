@@ -201,6 +201,17 @@ void lookup_batch(const Launch& L, const TopModel& top, int leaf_kind, const voi
 void lookup_bounded_batch(const Launch& L, const TopModel& top, int leaf_kind, const void* d_records, u64 N,
                           const void* d_knots, u64 K, u64 line_size, const u64* keys, u64 n, const u64* d_queries,
                           u64 nq, u64* d_out, u64* d_out_err, u64* d_fallbacks, bool lower_bound);
+// Exact upper bounds (the number of keys <= q; 0 for NaN) of nq queries into d_last, and with d_first non-null the
+// lower bounds too (equal_range), from one window per query (kernels_lookup_range.cu).  last = keys[n-1]; queries >= it
+// get n without a search.  One launch (none for nq == 0); *d_fallbacks (may be null) grows by the queries whose window
+// missed either end.
+template <class T>
+void lookup_range_batch(const Launch& L, const TopModel& top, int leaf_kind, const void* d_records, u64 N, const T* keys,
+                        u64 n, T last, const T* d_queries, u64 nq, u64* d_first, u64* d_last, u64* d_fallbacks);
+// The same on a bounded index (lookup_bounded_batch's arguments), searching the key line of lookup_bounded_batch.
+void lookup_bounded_range_batch(const Launch& L, const TopModel& top, int leaf_kind, const void* d_records, u64 N,
+                                const void* d_knots, u64 K, u64 line_size, const u64* keys, u64 n, u64 last,
+                                const u64* d_queries, u64 nq, u64* d_first, u64* d_last, u64* d_fallbacks);
 
 // ---- lookups over a range-partitioned data set (kernels_shard_lookup.cu, DESIGN.md section 14) -------------------
 // A query goes to the last non-empty rank whose first key is < q (the first non-empty rank if none is).
@@ -215,15 +226,17 @@ template <class T> struct ShardRoute {
 u64 shard_route_blocks(u64 n);
 // Three launches (none for n == 0, where d_send_counts is zeroed): d_send receives the n queries in per-rank segments
 // in rank order, d_send_counts[r] the length of rank r's segment, d_slot[i] the position of query i in d_send.
+// upper: route by <= (the last non-empty rank whose first key is <= q), for upper bounds.
 template <class T>
 void shard_route(const Launch& L, const ShardRoute<T>& route, int world, const T* d_q, u64 n, u32* d_block_counts,
-                 u64* d_block_offsets, T* d_send, u64* d_slot, u64* d_send_counts);
+                 u64* d_block_offsets, T* d_send, u64* d_slot, u64* d_send_counts, bool upper = false);
 // Exact global lower bounds of m queries routed to this rank (slab keys[0, n_local) at global index base), from the
 // predictions d_pos / d_err of lookup_batch (predict, n = n_global).  One launch; *d_fallbacks (may be null) grows by
-// the number of windows that missed.  n_local >= 1.
+// the number of windows that missed.  n_local >= 1.  upper: exact global upper bounds of queries routed by <= instead;
+// last = keys[n_local - 1] (queries >= it get base + n_local without a search).
 template <class T>
 void shard_search(const Launch& L, const T* keys, u64 n_local, u64 base, u64 n_global, const T* d_q, u64 m,
-                  const u64* d_pos, const u64* d_err, u64* d_out, u64* d_fallbacks);
+                  const u64* d_pos, const u64* d_err, u64* d_out, u64* d_fallbacks, bool upper = false, T last = T());
 // d_out[i] = d_returned[d_slot[i]].  One launch (none for n == 0).
 void shard_gather(const Launch& L, const u64* d_slot, const u64* d_returned, u64 n, u64* d_out);
 
@@ -238,9 +251,11 @@ struct BoundedKnotSlab {
 // (slab keys[0, n_local) at global index base, n_local >= 1); *d_fallbacks (may be null) grows by the far queries and
 // by the others whose global line missed.  lower_bound = false: the single-GPU bounded pos of m queries routed to this
 // rank by knot index.  The RMI (d_records, N leaves, `top` by value) runs over the K knots.
+// upper (with lower_bound): upper bounds of queries routed to this rank by key with <=; last = keys[n_local - 1].
 void shard_bounded_search(const Launch& L, const TopModel& top, int leaf_kind, const void* d_records, u64 N,
                           const BoundedKnotSlab& ks, const u64* keys, u64 n_local, u64 base, u64 n_global,
-                          const u64* d_queries, u64 m, u64* d_out, u64* d_fallbacks, bool lower_bound);
+                          const u64* d_queries, u64 m, u64* d_out, u64* d_fallbacks, bool lower_bound,
+                          bool upper = false, u64 last = 0);
 // d_out[i] = max(d_pos[i] - d_err[i], 0) + 1 (d_out may be d_pos): the value shard_route<u64> routes by knot index
 // (a route whose "first keys" are the knot bases of the ranks that hold knots).  One launch (none for n == 0).
 void shard_knot_route_keys(const Launch& L, const u64* d_pos, const u64* d_err, u64 n, u64* d_out);

@@ -25,16 +25,6 @@ namespace rmi {
 
 namespace {
 
-// Queries per thread and threads per block, measured on an H100 SXM (DESIGN §11) on the headline index
-// (linear,linear 2^20 over 200M uint64 keys, 2^27 random present keys): lower_bound took 27.4 / 34.2 / 36.6 /
-// 37.0 ms at 1 / 2 / 4 / 8 queries per thread with 128 threads (28.4 / 33.9 / 35.2 / 37.2 ms with 256); predict
-// was 2.65-2.72 ms at 1, 2 and 4 and 2.95 ms at 8.  One query per thread needs 32 registers, so 64 warps fit on
-// an SM, and those warps keep more probes in flight than fewer warps carrying several queries each: the lockstep
-// search waits for the longest window of its queries, and the registers it needs cost warps.
-constexpr int LOOKUP_Q = 1;
-constexpr int LOOKUP_THREADS = 128;
-constexpr int LOOKUP_MAX_BLOCKS_PER_SM = 32;   // grid cap; beyond it the blocks stride over the tiles
-
 template <class T, int TOP, int LEAF>
 __global__ void __launch_bounds__(LOOKUP_THREADS)
 k_lookup(const __grid_constant__ TopModel top, const ulonglong2* __restrict__ recs, const T* __restrict__ keys, u64 n,

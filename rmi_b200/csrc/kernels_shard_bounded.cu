@@ -11,6 +11,11 @@
 //          confirm themselves (§14).  A "far" query, whose window misses [a0, a1], may need knots past the halo: it
 //          searches the whole slab instead, exactly, and is always counted as a fallback.  Any other query is counted
 //          when its global line [pos, pos + line] does not hold its lower bound, as on one GPU.
+// upper    (UPPER) upper bounds of queries routed to r by key with <= (DESIGN §18): the same steps with k <= q.  A query
+//          equal to r's first key F may have its answer knot up to two knots before a0 (the knots with keys F - 1 and F
+//          route to an earlier rank), but a non-far query's reads lie in [lower - 1, upper] wherever that knot is, and
+//          the window meets [a0, a1], so they stay inside the halo of 2 e_max + 2.  A query >= the slab's last key gets
+//          base + n_local without a search, uncounted.
 // predict  pos of queries routed to r BY KNOT INDEX (the rank whose knot slab holds lower = start - e): the window and
 //          the knot before it lie inside the halo, so every pos is the single-GPU one.
 // The route by knot index reuses §14's route over the values lower + 1 (knot_route_keys), then moves the queries
@@ -26,18 +31,22 @@ namespace {
 constexpr int SB_THREADS = 128;
 constexpr int SB_MAX_BLOCKS_PER_SM = 32;
 
-template <int TOP, int LEAF>
+template <int TOP, int LEAF, bool UPPER>
 __global__ void __launch_bounds__(SB_THREADS)
 k_shard_bounded(const __grid_constant__ TopModel top, const ulonglong2* __restrict__ recs, u64 N,
                 const __grid_constant__ BoundedKnotSlab ks, const u64* __restrict__ keys, u64 n_local, u64 base,
                 u64 n_global, const u64* __restrict__ qs, u64 m, u64* __restrict__ out, u64* fallbacks,
-                int lower_bound) {
+                int lower_bound, u64 last) {
   using R = Rec<LEAF>;
   const ulonglong2* __restrict__ kext = (const ulonglong2*)ks.knots;
   const u64 K = ks.K, line = ks.line;
   unsigned misses = 0, local_misses = 0;
   for (u64 i = (u64)blockIdx.x * SB_THREADS + threadIdx.x; i < m; i += (u64)gridDim.x * SB_THREADS) {
     const u64 q = __ldcs(qs + i);
+    if (UPPER && q >= last) {
+      __stcs(out + i, base + n_local);
+      continue;
+    }
     u64 t = top_predict<TOP>(top, q);
     t = t < N - 1 ? t : N - 1;
     ulonglong2 v[R::LOADS];
@@ -53,7 +62,7 @@ k_shard_bounded(const __grid_constant__ TopModel top, const ulonglong2* __restri
     u64 r;
     if (lower_bound && (upper < ks.a0 || lower > ks.a1)) {
       // far: the whole slab, whose edges confirm themselves
-      RMI_LINE_SEARCH(keys, n_local, q, (u64)0, n_local, n_local, local_misses, r);
+      RMI_LINE_SEARCH_AS(keys, n_local, q, (u64)0, n_local, n_local, local_misses, r, UPPER);
       ++misses;
       __stcs(out + i, base + r);
       continue;
@@ -77,7 +86,7 @@ k_shard_bounded(const __grid_constant__ TopModel top, const ulonglong2* __restri
     const u64 ghi = line >= n_global - glo ? n_global : glo + line;
     const u64 lo = glo <= base ? 0 : (glo - base < n_local ? glo - base : n_local);
     const u64 hi = ghi <= base ? 0 : (ghi - base < n_local ? ghi - base : n_local);
-    RMI_LINE_SEARCH(keys, n_local, q, lo, hi, line, local_misses, r);
+    RMI_LINE_SEARCH_AS(keys, n_local, q, lo, hi, line, local_misses, r, UPPER);
     if (base + r < glo || base + r > ghi) ++misses;
     __stcs(out + i, base + r);
   }
@@ -90,20 +99,24 @@ k_shard_bounded(const __grid_constant__ TopModel top, const ulonglong2* __restri
 template <int TOP, int LEAF>
 void launch_shard_bounded(const Launch& L, const TopModel& top, const void* recs, u64 N, const BoundedKnotSlab& ks,
                           const u64* keys, u64 n_local, u64 base, u64 n_global, const u64* q, u64 m, u64* out,
-                          u64* fallbacks, bool lb) {
+                          u64* fallbacks, bool lb, bool upper, u64 last) {
   u64 blocks = (m + SB_THREADS - 1) / SB_THREADS;
   const u64 cap = (u64)L.num_sms * SB_MAX_BLOCKS_PER_SM;
   if (blocks > cap) blocks = cap;
-  k_shard_bounded<TOP, LEAF><<<(unsigned)blocks, SB_THREADS, 0, L.stream>>>(
-      top, (const ulonglong2*)recs, N, ks, keys, n_local, base, n_global, q, m, out, fallbacks, lb ? 1 : 0);
+  if (upper)
+    k_shard_bounded<TOP, LEAF, true><<<(unsigned)blocks, SB_THREADS, 0, L.stream>>>(
+        top, (const ulonglong2*)recs, N, ks, keys, n_local, base, n_global, q, m, out, fallbacks, 1, last);
+  else
+    k_shard_bounded<TOP, LEAF, false><<<(unsigned)blocks, SB_THREADS, 0, L.stream>>>(
+        top, (const ulonglong2*)recs, N, ks, keys, n_local, base, n_global, q, m, out, fallbacks, lb ? 1 : 0, last);
   count_launch();
 }
 
-#define RMI_SB_ARGS recs, N, ks, keys, n_local, base, n_global, q, m, out, fallbacks, lb
+#define RMI_SB_ARGS recs, N, ks, keys, n_local, base, n_global, q, m, out, fallbacks, lb, upper, last
 template <int TOP>
 void shard_bounded_leaf(const Launch& L, const TopModel& top, int leaf_kind, const void* recs, u64 N,
                         const BoundedKnotSlab& ks, const u64* keys, u64 n_local, u64 base, u64 n_global, const u64* q,
-                        u64 m, u64* out, u64* fallbacks, bool lb) {
+                        u64 m, u64* out, u64* fallbacks, bool lb, bool upper, u64 last) {
   switch (lookup_leaf_group(leaf_kind)) {
     case M_LINEAR: launch_shard_bounded<TOP, M_LINEAR>(L, top, RMI_SB_ARGS); break;
     case M_CUBIC: launch_shard_bounded<TOP, M_CUBIC>(L, top, RMI_SB_ARGS); break;
@@ -141,7 +154,7 @@ unsigned elementwise_blocks(const Launch& L, u64 n) {
 
 void shard_bounded_search(const Launch& L, const TopModel& top, int leaf_kind, const void* recs, u64 N,
                           const BoundedKnotSlab& ks, const u64* keys, u64 n_local, u64 base, u64 n_global, const u64* q,
-                          u64 m, u64* out, u64* fallbacks, bool lb) {
+                          u64 m, u64* out, u64* fallbacks, bool lb, bool upper, u64 last) {
   if (m == 0) return;
   switch (lookup_top_group(top.kind)) {
     case M_LINEAR: shard_bounded_leaf<M_LINEAR>(L, top, leaf_kind, RMI_SB_ARGS); break;

@@ -4,6 +4,10 @@
 // < q (the first non-empty rank if none is, which includes a NaN query): every key before that rank's slab is < q and
 // every key after it is not, so the global lower bound is base_r + the lower bound inside the slab.
 //
+// Upper bounds route by <= instead (DESIGN §18): the last non-empty rank whose first key is <= q, or the first non-empty
+// rank.  Every key before that rank's slab is <= q and every key after it is > q, so the global upper bound is base_r +
+// the upper bound inside the slab.  The two rules differ only for a query equal to some slab's first key.
+//
 // route    count / scan / scatter: each block takes a tile of ROUTE_THREADS * ROUTE_Q queries, finds every query's
 //          rank by a binary search over the first keys (in shared memory) and counts queries per rank; one block scans
 //          the (rank, block) counts rank-major; the scatter repeats the search and writes each query into its rank's
@@ -30,13 +34,13 @@ constexpr int SCAN_THREADS = 1024;
 constexpr int SEARCH_THREADS = 128;
 constexpr int SEARCH_MAX_BLOCKS_PER_SM = 32;
 
-// Index into route.rank of the non-empty rank that owns q: the number of first keys < q, less one (0 if none).  The
-// first keys are in order, so the ones < q are a prefix.
-template <class T> __device__ __forceinline__ int route_slot(const T* s_first, int count, T q) {
+// Index into route.rank of the non-empty rank that owns q: the number of first keys < q (<= q for UPPER), less one
+// (0 if none).  The first keys are in order, so the ones < q (<= q) are a prefix.
+template <class T, bool UPPER = false> __device__ __forceinline__ int route_slot(const T* s_first, int count, T q) {
   int lo = 0, len = count;
   while (len > 0) {
     const int h = len >> 1;
-    if (s_first[lo + h] < q) { lo += h + 1; len -= h + 1; } else { len = h; }
+    if (UPPER ? s_first[lo + h] <= q : s_first[lo + h] < q) { lo += h + 1; len -= h + 1; } else { len = h; }
   }
   return lo > 0 ? lo - 1 : 0;
 }
@@ -49,7 +53,7 @@ __device__ __forceinline__ void route_load(const ShardRoute<T>& route, T* s_firs
   }
 }
 
-template <class T>
+template <class T, bool UPPER>
 __global__ void __launch_bounds__(ROUTE_THREADS)
 k_route_count(const __grid_constant__ ShardRoute<T> route, const T* __restrict__ qs, u64 n, int world, u64 nblocks,
               u32* __restrict__ block_counts) {
@@ -66,7 +70,7 @@ k_route_count(const __grid_constant__ ShardRoute<T> route, const T* __restrict__
     const u64 i = tile + (u64)j * ROUTE_THREADS + threadIdx.x;
     const unsigned active = __ballot_sync(0xffffffffu, i < n);
     if (i < n) {
-      const int d = s_rank[route_slot(s_first, route.count, __ldg(qs + i))];
+      const int d = s_rank[route_slot<T, UPPER>(s_first, route.count, __ldg(qs + i))];
       const unsigned peers = __match_any_sync(active, d);
       if (lane == (unsigned)(__ffs(peers) - 1)) atomicAdd(&s_count[d], (u32)__popc(peers));
     }
@@ -118,7 +122,7 @@ k_route_scan(const u32* __restrict__ counts, u64 total, u64 nblocks, int world, 
   }
 }
 
-template <class T>
+template <class T, bool UPPER>
 __global__ void __launch_bounds__(ROUTE_THREADS)
 k_route_scatter(const __grid_constant__ ShardRoute<T> route, const T* __restrict__ qs, u64 n, int world, u64 nblocks,
                 const u64* __restrict__ offsets, T* __restrict__ send, u64* __restrict__ slot) {
@@ -137,7 +141,7 @@ k_route_scatter(const __grid_constant__ ShardRoute<T> route, const T* __restrict
     const unsigned active = __ballot_sync(0xffffffffu, i < n);
     if (i < n) {
       const T q = __ldcs(qs + i);
-      const int d = s_rank[route_slot(s_first, route.count, q)];
+      const int d = s_rank[route_slot<T, UPPER>(s_first, route.count, q)];
       const unsigned peers = __match_any_sync(active, d);
       const int leader = __ffs(peers) - 1;
       unsigned long long p = 0;
@@ -149,13 +153,20 @@ k_route_scatter(const __grid_constant__ ShardRoute<T> route, const T* __restrict
   }
 }
 
-template <class T>
+// UPPER: upper bounds of queries routed by <=; last = keys[n_local - 1], and a query >= it gets base + n_local without
+// a search (the slab's final run is the one a leaf bound may not record).
+template <class T, bool UPPER>
 __global__ void __launch_bounds__(SEARCH_THREADS)
 k_shard_search(const T* __restrict__ keys, u64 n_local, u64 base, u64 n_global, const T* __restrict__ qs, u64 m,
-               const u64* __restrict__ pos, const u64* __restrict__ err, u64* __restrict__ out, u64* fallbacks) {
+               const u64* __restrict__ pos, const u64* __restrict__ err, u64* __restrict__ out, u64* fallbacks,
+               T last) {
   unsigned misses = 0;
   for (u64 i = (u64)blockIdx.x * SEARCH_THREADS + threadIdx.x; i < m; i += (u64)gridDim.x * SEARCH_THREADS) {
     const T q[1] = {__ldcs(qs + i)};
+    if (UPPER && q[0] >= last) {
+      __stcs(out + i, base + n_local);
+      continue;
+    }
     const bool live[1] = {true};
     const u64 p = __ldcs(pos + i), e = __ldcs(err + i);
     // the global window, then its part inside this slab
@@ -164,7 +175,8 @@ k_shard_search(const T* __restrict__ keys, u64 n_local, u64 base, u64 n_global, 
     u64 lo[1], hi[1];
     lo[0] = glo <= base ? 0 : (glo - base < n_local ? glo - base : n_local);
     hi[0] = ghi <= base ? 0 : (ghi - base < n_local ? ghi - base : n_local);
-    window_search<T, 1>(keys, n_local, q, live, lo, hi, misses, [&](int, u64 r) { __stcs(out + i, base + r); });
+    window_search<T, 1, UPPER ? 1u : 0u>(keys, n_local, q, live, lo, hi, misses,
+                                         [&](int, u64 r) { __stcs(out + i, base + r); });
   }
   if (fallbacks) {
     misses = __reduce_add_sync(0xffffffffu, misses);
@@ -184,29 +196,41 @@ u64 shard_route_blocks(u64 n) { return (n + ROUTE_TILE - 1) / ROUTE_TILE; }
 
 template <class T>
 void shard_route(const Launch& L, const ShardRoute<T>& route, int world, const T* q, u64 n, u32* d_block_counts,
-                 u64* d_block_offsets, T* d_send, u64* d_slot, u64* d_send_counts) {
+                 u64* d_block_offsets, T* d_send, u64* d_slot, u64* d_send_counts, bool upper) {
   if (n == 0) {
     cudaMemsetAsync(d_send_counts, 0, sizeof(u64) * world, L.stream);
     return;
   }
   const u64 nb = shard_route_blocks(n);
-  k_route_count<T><<<(unsigned)nb, ROUTE_THREADS, 0, L.stream>>>(route, q, n, world, nb, d_block_counts);
+  if (upper)
+    k_route_count<T, true><<<(unsigned)nb, ROUTE_THREADS, 0, L.stream>>>(route, q, n, world, nb, d_block_counts);
+  else
+    k_route_count<T, false><<<(unsigned)nb, ROUTE_THREADS, 0, L.stream>>>(route, q, n, world, nb, d_block_counts);
   count_launch();
   k_route_scan<<<1, SCAN_THREADS, 0, L.stream>>>(d_block_counts, nb * world, nb, world, d_block_offsets, d_send_counts);
   count_launch();
-  k_route_scatter<T><<<(unsigned)nb, ROUTE_THREADS, 0, L.stream>>>(route, q, n, world, nb, d_block_offsets, d_send, d_slot);
+  if (upper)
+    k_route_scatter<T, true><<<(unsigned)nb, ROUTE_THREADS, 0, L.stream>>>(route, q, n, world, nb, d_block_offsets,
+                                                                            d_send, d_slot);
+  else
+    k_route_scatter<T, false><<<(unsigned)nb, ROUTE_THREADS, 0, L.stream>>>(route, q, n, world, nb, d_block_offsets,
+                                                                             d_send, d_slot);
   count_launch();
 }
 
 template <class T>
 void shard_search(const Launch& L, const T* keys, u64 n_local, u64 base, u64 n_global, const T* q, u64 m,
-                  const u64* d_pos, const u64* d_err, u64* d_out, u64* d_fallbacks) {
+                  const u64* d_pos, const u64* d_err, u64* d_out, u64* d_fallbacks, bool upper, T last) {
   if (m == 0) return;
   u64 blocks = (m + SEARCH_THREADS - 1) / SEARCH_THREADS;
   const u64 cap = (u64)L.num_sms * SEARCH_MAX_BLOCKS_PER_SM;
   if (blocks > cap) blocks = cap;
-  k_shard_search<T><<<(unsigned)blocks, SEARCH_THREADS, 0, L.stream>>>(keys, n_local, base, n_global, q, m, d_pos, d_err,
-                                                                      d_out, d_fallbacks);
+  if (upper)
+    k_shard_search<T, true><<<(unsigned)blocks, SEARCH_THREADS, 0, L.stream>>>(keys, n_local, base, n_global, q, m,
+                                                                              d_pos, d_err, d_out, d_fallbacks, last);
+  else
+    k_shard_search<T, false><<<(unsigned)blocks, SEARCH_THREADS, 0, L.stream>>>(keys, n_local, base, n_global, q, m,
+                                                                               d_pos, d_err, d_out, d_fallbacks, last);
   count_launch();
 }
 
@@ -220,9 +244,10 @@ void shard_gather(const Launch& L, const u64* d_slot, const u64* d_returned, u64
 }
 
 #define RMI_SHARD_LOOKUP_INST(T)                                                                                    \
-  template void shard_route<T>(const Launch&, const ShardRoute<T>&, int, const T*, u64, u32*, u64*, T*, u64*, u64*); \
+  template void shard_route<T>(const Launch&, const ShardRoute<T>&, int, const T*, u64, u32*, u64*, T*, u64*, u64*, \
+                               bool);                                                                              \
   template void shard_search<T>(const Launch&, const T*, u64, u64, u64, const T*, u64, const u64*, const u64*, u64*,  \
-                                u64*);
+                                u64*, bool, T);
 RMI_SHARD_LOOKUP_INST(u64)
 RMI_SHARD_LOOKUP_INST(u32)
 RMI_SHARD_LOOKUP_INST(double)

@@ -1,56 +1,78 @@
 // lookup_search.cuh — the exact search of a lookup's error window, shared by the single-GPU lookup kernels
-// (kernels_lookup.cu) and the searches over a rank's slab of a range-partitioned data set (kernels_shard_lookup.cu,
-// kernels_shard_bounded.cu), with the pieces of a bounded lookup both bounded kernels take: the knot-window search,
-// the key-line step and the packed leaf record.
+// (kernels_lookup.cu, kernels_lookup_range.cu) and the searches over a rank's slab of a range-partitioned data set
+// (kernels_shard_lookup.cu, kernels_shard_bounded.cu), with the pieces of a bounded lookup every bounded kernel takes:
+// the knot-window search, the key-line step and the packed leaf record.
 //
 // For a window [lo, hi] of candidate answers over keys[0, n): a branchless binary search over keys [lo, hi),
 // confirmed by the keys just outside the window (lo == 0 and hi == n need no confirmation), and a galloping search
 // outward from the window's edge when the window does not bracket the answer (counted in `misses`).
+//
+// Every search counts the keys k before q under one predicate: k < q (strict: the lower bound, what the predict /
+// lower_bound kernels run) or k <= q (UPPER: the upper bound, kernels_lookup_range.cu).  Both compare by value, so
+// -0.0 and 0.0 are equal, and a NaN q has no key before it under either.
 #pragma once
+#include <type_traits>
+
 #include "models.cuh"
 
 namespace rmi {
 namespace {
 
-// First index in [lo, hi) whose key is not < q, or hi.
-template <class T> __device__ __forceinline__ u64 search_range(const T* __restrict__ keys, u64 lo, u64 hi, T q) {
+// Queries per thread and threads per block of the lookup kernels, measured on an H100 SXM (DESIGN §11) on the headline
+// index (linear,linear 2^20 over 200M uint64 keys, 2^27 random present keys): lower_bound took 27.4 / 34.2 / 36.6 /
+// 37.0 ms at 1 / 2 / 4 / 8 queries per thread with 128 threads (28.4 / 33.9 / 35.2 / 37.2 ms with 256); predict
+// was 2.65-2.72 ms at 1, 2 and 4 and 2.95 ms at 8.  One query per thread needs 32 registers, so 64 warps fit on
+// an SM, and those warps keep more probes in flight than fewer warps carrying several queries each: the lockstep
+// search waits for the longest window of its queries, and the registers it needs cost warps.
+constexpr int LOOKUP_Q = 1;
+constexpr int LOOKUP_THREADS = 128;
+constexpr int LOOKUP_MAX_BLOCKS_PER_SM = 32;   // grid cap; beyond it the blocks stride over the tiles
+
+// Whether key k counts before q: k < q, or k <= q for UPPER.  search_range and lookup_fallback spell the same
+// conditional out: through this helper the float64 instances of the strict fallback compiled to different SASS.
+template <bool UPPER, class T> __device__ __forceinline__ bool before(T k, T q) { return UPPER ? k <= q : k < q; }
+
+// First index in [lo, hi) whose key does not count before q, or hi.
+template <class T, bool UPPER = false>
+__device__ __forceinline__ u64 search_range(const T* __restrict__ keys, u64 lo, u64 hi, T q) {
   while (lo < hi) {
     u64 mid = lo + ((hi - lo) >> 1);
-    if (keys[mid] < q) lo = mid + 1; else hi = mid;
+    if (UPPER ? keys[mid] <= q : keys[mid] < q) lo = mid + 1; else hi = mid;
   }
   return lo;
 }
 
-// The window [lo, hi] missed: the answer is below lo (!left_ok: keys[lo-1] is not < q) or above hi
-// (keys[hi] < q).  Gallop outward from that edge until the answer is bracketed, then search the bracket.
-template <class T>
+// The window [lo, hi] missed: the answer is below lo (!left_ok: keys[lo-1] does not count before q) or above hi
+// (keys[hi] counts before q).  Gallop outward from that edge until the answer is bracketed, then search the bracket.
+template <class T, bool UPPER = false>
 __device__ __noinline__ u64 lookup_fallback(const T* __restrict__ keys, u64 n, T q, u64 lo, u64 hi, bool left_ok) {
   if (!left_ok) {
     u64 R = lo - 1, step = 1, L = 0;   // answer <= R
     while (true) {
       if (R < step) { L = 0; break; }
       u64 c = R - step;
-      if (keys[c] < q) { L = c + 1; break; }
+      if (UPPER ? keys[c] <= q : keys[c] < q) { L = c + 1; break; }
       R = c;
       step <<= 1;
     }
-    return search_range(keys, L, R, q);
+    return search_range<T, UPPER>(keys, L, R, q);
   }
   u64 L = hi + 1, step = 1, R = n;     // answer >= L
   while (true) {
     if (n - L < step) { R = n; break; }
     u64 c = L + step - 1;
-    if (!(keys[c] < q)) { R = c; break; }
+    if (!(UPPER ? keys[c] <= q : keys[c] < q)) { R = c; break; }
     L = c + 1;
     step <<= 1;
   }
-  return search_range(keys, L, R, q);
+  return search_range<T, UPPER>(keys, L, R, q);
 }
 
 // Q queries in lockstep (keeps Q independent probes in flight per step).  Windows [lo[j], hi[j]] with
 // lo[j] <= hi[j] <= n and n >= 1.  For every live query, emit(j, r) receives r = the exact lower bound of q[j] over
-// keys[0, n).
-template <class T, int Q, class Emit>
+// keys[0, n), or its upper bound where bit j of UPPER is set (lanes over the same window, as equal_range runs them,
+// share the edge loads).
+template <class T, int Q, unsigned UPPER = 0u, class Emit>
 __device__ __forceinline__ void window_search(const T* __restrict__ keys, u64 n, const T (&q)[Q], const bool (&live)[Q],
                                               const u64 (&lo)[Q], const u64 (&hi)[Q], unsigned& misses, Emit&& emit) {
   u64 b[Q], len[Q];
@@ -67,9 +89,11 @@ __device__ __forceinline__ void window_search(const T* __restrict__ keys, u64 n,
     bool more = false;
 #pragma unroll
     for (int j = 0; j < Q; ++j) {
+      const bool up = (UPPER >> j) & 1u;
       if (len[j] > 1) {
         u64 h = len[j] >> 1;
-        b[j] = keys[b[j] + h] < q[j] ? b[j] + h : b[j];
+        const T k = keys[b[j] + h];
+        b[j] = (up ? before<true>(k, q[j]) : before<false>(k, q[j])) ? b[j] + h : b[j];
         len[j] -= h;
         more |= len[j] > 1;
       }
@@ -78,14 +102,16 @@ __device__ __forceinline__ void window_search(const T* __restrict__ keys, u64 n,
   }
 #pragma unroll
   for (int j = 0; j < Q; ++j) {
+    const bool up = (UPPER >> j) & 1u;
     u64 r = b[j];
-    if (len[j] == 1) r += keys[r] < q[j] ? 1 : 0;
-    bool left_ok = lo[j] == 0 || edge_l[j] < q[j];
-    bool right_ok = hi[j] == n || !(edge_r[j] < q[j]);
+    if (len[j] == 1) r += (up ? before<true>(keys[r], q[j]) : before<false>(keys[r], q[j])) ? 1 : 0;
+    bool left_ok = lo[j] == 0 || (up ? before<true>(edge_l[j], q[j]) : before<false>(edge_l[j], q[j]));
+    bool right_ok = hi[j] == n || !(up ? before<true>(edge_r[j], q[j]) : before<false>(edge_r[j], q[j]));
     if (live[j]) {
       if (!(left_ok && (r < hi[j] || right_ok))) {
         ++misses;
-        r = lookup_fallback(keys, n, q[j], lo[j], hi[j], left_ok);
+        r = up ? lookup_fallback<T, true>(keys, n, q[j], lo[j], hi[j], left_ok)
+               : lookup_fallback<T, false>(keys, n, q[j], lo[j], hi[j], left_ok);
       }
       emit(j, r);
     }
@@ -99,32 +125,69 @@ __device__ __forceinline__ void window_search(const T* __restrict__ keys, u64 n,
 // window are read only when the search ends on that edge, so a present key touches its own line alone unless its
 // lower bound is the line's first index.  A window that does not bracket the answer takes the galloping fallback and
 // is counted in `misses`.
-// A statement macro, not a function: the same code as an inlined function compiles to different SASS in
+// Statement macros, not functions: the same code as an inlined function compiles to different SASS in
 // k_lookup_bounded (the edge flags are materialised as bytes before the fallback call), and the move was to leave that
 // kernel's SASS as it was.
+//   RMI_LINE_SEARCH_AS  the same with the predicate of UPPER (a constant): r = the upper bound for true
+//   RMI_LINE_RANGE      both ends, r (lower) and ru (upper), over one window; the counting branch counts both from one
+//                       set of loads; each end is confirmed on its own, and `misses` grows by one per end that missed
 constexpr u64 BOUNDED_COUNT_MAX = 16;
 
-#define RMI_LINE_SEARCH(keys, n, q, lo, hi, width, misses, r)                  \
+#define RMI_LINE_BSEARCH_(keys, q, lo, hi, r, UPPER)                           \
+  do {                                                                         \
+    u64 kb_ = lo, klen_ = hi - lo;                                             \
+    while (klen_ > 1) {                                                        \
+      const u64 h_ = klen_ >> 1;                                               \
+      kb_ = before<UPPER>(keys[kb_ + h_], q) ? kb_ + h_ : kb_;                 \
+      klen_ -= h_;                                                             \
+    }                                                                          \
+    r = klen_ == 1 && before<UPPER>(keys[kb_], q) ? kb_ + 1 : kb_;             \
+  } while (0)
+
+#define RMI_LINE_CONFIRM_(keys, n, q, lo, hi, misses, r, UPPER)                          \
+  do {                                                                                   \
+    const bool left_ok_ = r > lo || lo == 0 || before<UPPER>(keys[lo - 1], q);           \
+    const bool right_ok_ = r < hi || hi == n || !before<UPPER>(keys[hi], q);             \
+    if (!(left_ok_ && right_ok_)) {                                                      \
+      ++misses;                                                                          \
+      r = lookup_fallback<std::remove_cv_t<std::remove_reference_t<decltype(keys[0])>>,  \
+                          UPPER>(keys, n, q, lo, hi, left_ok_);                          \
+    }                                                                                    \
+  } while (0)
+
+#define RMI_LINE_SEARCH_AS(keys, n, q, lo, hi, width, misses, r, UPPER)        \
   do {                                                                         \
     r = lo;                                                                    \
     if ((width) <= BOUNDED_COUNT_MAX) {                                        \
       _Pragma("unroll") for (u64 j_ = 0; j_ < BOUNDED_COUNT_MAX; ++j_)         \
-        if (lo + j_ < hi) r += keys[lo + j_] < q ? 1 : 0;                      \
+        if (lo + j_ < hi) r += before<UPPER>(keys[lo + j_], q) ? 1 : 0;        \
     } else {                                                                   \
-      u64 kb_ = lo, klen_ = hi - lo;                                           \
-      while (klen_ > 1) {                                                      \
-        const u64 h_ = klen_ >> 1;                                             \
-        kb_ = keys[kb_ + h_] < q ? kb_ + h_ : kb_;                             \
-        klen_ -= h_;                                                           \
+      RMI_LINE_BSEARCH_(keys, q, lo, hi, r, UPPER);                            \
+    }                                                                          \
+    RMI_LINE_CONFIRM_(keys, n, q, lo, hi, misses, r, UPPER);                   \
+  } while (0)
+
+#define RMI_LINE_SEARCH(keys, n, q, lo, hi, width, misses, r) \
+  RMI_LINE_SEARCH_AS(keys, n, q, lo, hi, width, misses, r, false)
+
+#define RMI_LINE_RANGE(keys, n, q, lo, hi, width, misses, r, ru)               \
+  do {                                                                         \
+    r = lo;                                                                    \
+    ru = lo;                                                                   \
+    if ((width) <= BOUNDED_COUNT_MAX) {                                        \
+      _Pragma("unroll") for (u64 j_ = 0; j_ < BOUNDED_COUNT_MAX; ++j_) {       \
+        if (lo + j_ < hi) {                                                    \
+          const auto k_ = keys[lo + j_];                                       \
+          r += before<false>(k_, q) ? 1 : 0;                                   \
+          ru += before<true>(k_, q) ? 1 : 0;                                   \
+        }                                                                      \
       }                                                                        \
-      r = klen_ == 1 && keys[kb_] < q ? kb_ + 1 : kb_;                         \
+    } else {                                                                   \
+      RMI_LINE_BSEARCH_(keys, q, lo, hi, r, false);                            \
+      RMI_LINE_BSEARCH_(keys, q, lo, hi, ru, true);                            \
     }                                                                          \
-    const bool left_ok_ = r > lo || lo == 0 || keys[lo - 1] < q;               \
-    const bool right_ok_ = r < hi || hi == n || !(keys[hi] < q);               \
-    if (!(left_ok_ && right_ok_)) {                                            \
-      ++misses;                                                                \
-      r = lookup_fallback(keys, n, q, lo, hi, left_ok_);                       \
-    }                                                                          \
+    RMI_LINE_CONFIRM_(keys, n, q, lo, hi, misses, r, false);                   \
+    RMI_LINE_CONFIRM_(keys, n, q, lo, hi, misses, ru, true);                   \
   } while (0)
 
 // The packed leaf record (kernels_lookup.cu pack_leaf_records): parameters, then the error bound, in 16-byte vectors.

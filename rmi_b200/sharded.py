@@ -810,6 +810,9 @@ class CudaShardIndex:
         L.rmi_shard_index_lower_bound.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p,
                                                   C.c_void_p, C.c_void_p]
         L.rmi_shard_index_last_stats.argtypes = [C.c_void_p, C.POINTER(_LookupStats)]
+        L.rmi_shard_index_route_upper.argtypes = L.rmi_shard_index_route.argtypes
+        L.rmi_shard_index_search_upper.argtypes = L.rmi_shard_index_search.argtypes
+        L.rmi_shard_index_upper_bound.argtypes = L.rmi_shard_index_lower_bound.argtypes
         self.device = eng.device
         self.world = world
         self._ds = eng.ds            # the slab the index searches: kept alive with it
@@ -829,17 +832,24 @@ class CudaShardIndex:
                                                     self._stream()))
         return pos, err
 
-    def route(self, q: torch.Tensor):
+    def route(self, q: torch.Tensor, fn=None):
         send, slot, counts = torch.empty_like(q), self._u64(q.numel()), self._u64(self.world)
-        api._check(self.lib.rmi_shard_index_route(self._h, q.data_ptr(), q.numel(), send.data_ptr(), slot.data_ptr(),
-                                                  counts.data_ptr(), self._stream()))
+        api._check((fn or self.lib.rmi_shard_index_route)(self._h, q.data_ptr(), q.numel(), send.data_ptr(),
+                                                          slot.data_ptr(), counts.data_ptr(), self._stream()))
         return send, slot, counts
 
-    def search(self, recv: torch.Tensor):
+    def search(self, recv: torch.Tensor, fn=None):
         answers, fb = self._u64(recv.numel()), torch.zeros(1, dtype=torch.int64, device=self.device)
-        api._check(self.lib.rmi_shard_index_search(self._h, recv.data_ptr(), recv.numel(), answers.data_ptr(),
-                                                   fb.data_ptr(), self._stream()))
+        api._check((fn or self.lib.rmi_shard_index_search)(self._h, recv.data_ptr(), recv.numel(), answers.data_ptr(),
+                                                           fb.data_ptr(), self._stream()))
         return answers, fb
+
+    def route_upper(self, q: torch.Tensor):
+        """route by <= (the upper bound's rule)"""
+        return self.route(q, self.lib.rmi_shard_index_route_upper)
+
+    def search_upper(self, recv: torch.Tensor):
+        return self.search(recv, self.lib.rmi_shard_index_search_upper)
 
     def gather(self, slot: torch.Tensor, returned: torch.Tensor):
         out = self._u64(slot.numel())
@@ -847,11 +857,14 @@ class CudaShardIndex:
                                                    out.data_ptr(), self._stream()))
         return out
 
-    def lower_bound_native(self, comm, q: torch.Tensor):
+    def lower_bound_native(self, comm, q: torch.Tensor, fn=None):
         out, fb = self._u64(q.numel()), torch.zeros(1, dtype=torch.int64, device=self.device)
-        api._check(self.lib.rmi_shard_index_lower_bound(self._h, comm, q.data_ptr(), q.numel(), out.data_ptr(),
-                                                        fb.data_ptr(), self._stream()))
+        api._check((fn or self.lib.rmi_shard_index_lower_bound)(self._h, comm, q.data_ptr(), q.numel(), out.data_ptr(),
+                                                                fb.data_ptr(), self._stream()))
         return out, fb
+
+    def upper_bound_native(self, comm, q: torch.Tensor):
+        return self.lower_bound_native(comm, q, self.lib.rmi_shard_index_upper_bound)
 
     def last_stats(self) -> dict:
         st = _LookupStats()
@@ -943,7 +956,9 @@ class ShardedRMIIndex:
 
     predict(q) -> (pos, err): the model's prediction over the whole key set; local, no communication.
     lower_bound(q): exact global lower bounds (np.searchsorted(all_keys, q, "left"); 0 for NaN); collective: every
-    rank calls it, with its own queries (0 is fine).  Under an NCCL group it is one library call (route, exchanges,
+    rank calls it, with its own queries (0 is fine).  upper_bound(q): exact global upper bounds
+    (np.searchsorted(all_keys, q, "right"); 0 for NaN), routed by <= (DESIGN §18); equal_range(q): lower_bound then
+    upper_bound, two exchanges.  Under an NCCL group it is one library call (route, exchanges,
     search, gather on the stream); otherwise (gloo, native=False) the phases are driven here with all_to_all_single.
     Queries are a 1-D tensor on the data's device in its storage dtype (int64 for uint64 keys, int32, float64);
     results are int64 tensors (uint64 values) there.  The orchestration is engine-agnostic: the CPU tests plug in a
@@ -992,6 +1007,21 @@ class ShardedRMIIndex:
     def lower_bound(self, q: torch.Tensor, return_fallbacks: bool = False, native: bool | None = None):
         """Exact global lower bounds of this rank's queries.  return_fallbacks: also the number of windows that
         missed among the queries THIS rank searched (the sum over ranks covers every query once)."""
+        return self._bound(q, return_fallbacks, native, upper=False)
+
+    def upper_bound(self, q: torch.Tensor, return_fallbacks: bool = False, native: bool | None = None):
+        """Exact global upper bounds of this rank's queries (the number of keys <= q; 0 for NaN); return_fallbacks
+        and native as for lower_bound."""
+        return self._bound(q, return_fallbacks, native, upper=True)
+
+    def equal_range(self, q: torch.Tensor, return_fallbacks: bool = False, native: bool | None = None):
+        """(first, last): lower_bound(q) and upper_bound(q), one exchange each; return_fallbacks: also the sum of
+        the two calls' counts."""
+        first, fb_lo = self.lower_bound(q, True, native)
+        last, fb_hi = self.upper_bound(q, True, native)
+        return (first, last, fb_lo + fb_hi) if return_fallbacks else (first, last)
+
+    def _bound(self, q: torch.Tensor, return_fallbacks: bool, native: bool | None, upper: bool):
         q = self._queries(q)
         comm = None
         if native is not False and isinstance(self.index, CudaShardIndex):
@@ -999,7 +1029,9 @@ class ShardedRMIIndex:
             if native is True and comm is None:
                 raise api.RMIError("native=True needs an NCCL process group (or a single rank) and a loadable libnccl.so.2")
         if comm is not None:
-            out, fb = self.index.lower_bound_native(comm, q)
+            out, fb = (self.index.upper_bound_native if upper else self.index.lower_bound_native)(comm, q)
+        elif upper:
+            out, fb = self._phases(q, self.index.route_upper, self.index.search_upper)
         else:
             out, fb = self._lower_bound_phases(q)
         return (out, int(fb)) if return_fallbacks else out
