@@ -838,47 +838,25 @@ int index_check_call(const rmi_index* idx, const void* d_queries, uint64_t n, co
   return RMI_OK;
 }
 
-int index_launch(const rmi_index* idx, const void* d_queries, uint64_t n, uint64_t* d_out, uint64_t* d_err,
-                 uint64_t* d_fallbacks, void* cuda_stream, bool lower_bound) {
+// One launch of `mode` (kernels.h: LookupMode) into d_out and d_out2, none for n == 0.
+int index_launch(const rmi_index* idx, LookupMode mode, const void* d_queries, uint64_t n, uint64_t* d_out,
+                 uint64_t* d_out2, uint64_t* d_fallbacks, void* cuda_stream) {
   if (n == 0) return RMI_OK;
   const rmi_dataset* ds = idx->ds;
   CUDA_TRY(cudaSetDevice(ds->device));
   Launch L{(cudaStream_t)cuda_stream, idx->num_sms};
   if (idx->d_knots) {
-    lookup_bounded_batch(L, idx->top, idx->leaf_kind, idx->d_records, idx->N, idx->d_knots, idx->K, idx->line_size,
-                         (const u64*)ds->d_keys, idx->n, (const u64*)d_queries, n, (u64*)d_out, (u64*)d_err,
-                         (u64*)d_fallbacks, lower_bound);
-    CUDA_TRY(cudaGetLastError());
-    return RMI_OK;
+    lookup_bounded_batch(L, mode, idx->top, idx->leaf_kind, idx->d_records, idx->N, idx->d_knots, idx->K,
+                         idx->line_size, (const u64*)ds->d_keys, idx->n, idx->last_key_bits, (const u64*)d_queries, n,
+                         (u64*)d_out, (u64*)d_out2, (u64*)d_fallbacks);
+  } else {
+    with_key_type(ds->key_type, [&](auto k) {
+      using T = decltype(k);
+      lookup_batch<T>(L, mode, idx->top, idx->leaf_kind, idx->d_records, idx->N, (const T*)ds->d_keys, idx->n,
+                      rmihost::key_from_bits<T>(idx->last_key_bits), (const T*)d_queries, n, (u64*)d_out,
+                      (u64*)d_out2, (u64*)d_fallbacks);
+    });
   }
-  with_key_type(ds->key_type, [&](auto k) {
-    using T = decltype(k);
-    lookup_batch<T>(L, idx->top, idx->leaf_kind, idx->d_records, idx->N, (const T*)ds->d_keys, idx->n,
-                    (const T*)d_queries, n, (u64*)d_out, (u64*)d_err, (u64*)d_fallbacks, lower_bound);
-  });
-  CUDA_TRY(cudaGetLastError());
-  return RMI_OK;
-}
-// Upper bounds into d_last, and with d_first non-null the lower bounds too (equal_range): one launch.
-int index_launch_range(const rmi_index* idx, const void* d_queries, uint64_t n, uint64_t* d_first, uint64_t* d_last,
-                       uint64_t* d_fallbacks, void* cuda_stream) {
-  if (n == 0) return RMI_OK;
-  const rmi_dataset* ds = idx->ds;
-  CUDA_TRY(cudaSetDevice(ds->device));
-  Launch L{(cudaStream_t)cuda_stream, idx->num_sms};
-  if (idx->d_knots) {
-    lookup_bounded_range_batch(L, idx->top, idx->leaf_kind, idx->d_records, idx->N, idx->d_knots, idx->K,
-                               idx->line_size, (const u64*)ds->d_keys, idx->n, idx->last_key_bits,
-                               (const u64*)d_queries, n, (u64*)d_first, (u64*)d_last, (u64*)d_fallbacks);
-    CUDA_TRY(cudaGetLastError());
-    return RMI_OK;
-  }
-  with_key_type(ds->key_type, [&](auto k) {
-    using T = decltype(k);
-    lookup_range_batch<T>(L, idx->top, idx->leaf_kind, idx->d_records, idx->N, (const T*)ds->d_keys, idx->n,
-                          rmihost::key_from_bits<T>(idx->last_key_bits), (const T*)d_queries, n, (u64*)d_first,
-                          (u64*)d_last, (u64*)d_fallbacks);
-  });
   CUDA_TRY(cudaGetLastError());
   return RMI_OK;
 }
@@ -1014,26 +992,26 @@ void rmi_index_destroy(rmi_index* idx) {
 int rmi_index_predict(const rmi_index* idx, const void* d_queries, uint64_t n, uint64_t* d_pos, uint64_t* d_err,
                       void* cuda_stream) {
   if (int rc = index_check_call(idx, d_queries, n, d_pos, "rmi_index_predict")) return rc;
-  return index_launch(idx, d_queries, n, d_pos, d_err, nullptr, cuda_stream, false);
+  return index_launch(idx, LOOKUP_PREDICT, d_queries, n, d_pos, d_err, nullptr, cuda_stream);
 }
 
 int rmi_index_lower_bound(const rmi_index* idx, const void* d_queries, uint64_t n, uint64_t* d_out,
                           uint64_t* d_fallbacks, void* cuda_stream) {
   if (int rc = index_check_call(idx, d_queries, n, d_out, "rmi_index_lower_bound")) return rc;
-  return index_launch(idx, d_queries, n, d_out, nullptr, d_fallbacks, cuda_stream, true);
+  return index_launch(idx, LOOKUP_LOWER, d_queries, n, d_out, nullptr, d_fallbacks, cuda_stream);
 }
 
 int rmi_index_upper_bound(const rmi_index* idx, const void* d_queries, uint64_t n, uint64_t* d_out,
                           uint64_t* d_fallbacks, void* cuda_stream) {
   if (int rc = index_check_call(idx, d_queries, n, d_out, "rmi_index_upper_bound")) return rc;
-  return index_launch_range(idx, d_queries, n, nullptr, d_out, d_fallbacks, cuda_stream);
+  return index_launch(idx, LOOKUP_UPPER, d_queries, n, d_out, nullptr, d_fallbacks, cuda_stream);
 }
 
 int rmi_index_equal_range(const rmi_index* idx, const void* d_queries, uint64_t n, uint64_t* d_first, uint64_t* d_last,
                           uint64_t* d_fallbacks, void* cuda_stream) {
   if (int rc = index_check_call(idx, d_queries, n, d_last, "rmi_index_equal_range")) return rc;
   if (n && !d_first) return fail(RMI_ERR_INVALID, "rmi_index_equal_range: null query or output pointer");
-  return index_launch_range(idx, d_queries, n, d_first, d_last, d_fallbacks, cuda_stream);
+  return index_launch(idx, LOOKUP_EQUAL_RANGE, d_queries, n, d_first, d_last, d_fallbacks, cuda_stream);
 }
 
 int rmi_index_range_host(const rmi_index* idx, const void* host_queries, uint64_t n, uint64_t* host_first,
@@ -1042,7 +1020,8 @@ int rmi_index_range_host(const rmi_index* idx, const void* host_queries, uint64_
   if (fallbacks) *fallbacks = 0;
   return index_host_call(idx, host_queries, n, host_last, host_first, fallbacks, "rmi_index_range_host",
                          [&](const void* d_q, uint64_t* d_last, uint64_t* d_first, uint64_t* d_fb, cudaStream_t st) {
-                           return index_launch_range(idx, d_q, n, d_first, d_last, d_fb, st);
+                           return d_first ? index_launch(idx, LOOKUP_EQUAL_RANGE, d_q, n, d_first, d_last, d_fb, st)
+                                         : index_launch(idx, LOOKUP_UPPER, d_q, n, d_last, nullptr, d_fb, st);
                          });
 }
 
@@ -1052,8 +1031,8 @@ int rmi_index_lookup_host(const rmi_index* idx, const void* host_queries, uint64
   return index_host_call(idx, host_queries, n, host_out, lower_bound ? nullptr : host_err,
                          lower_bound ? fallbacks : nullptr, "rmi_index_lookup_host",
                          [&](const void* d_q, uint64_t* d_out, uint64_t* d_err, uint64_t* d_fb, cudaStream_t st) {
-                           return lower_bound ? index_launch(idx, d_q, n, d_out, nullptr, d_fb, st, true)
-                                              : index_launch(idx, d_q, n, d_out, d_err, nullptr, st, false);
+                           return lower_bound ? index_launch(idx, LOOKUP_LOWER, d_q, n, d_out, nullptr, d_fb, st)
+                                              : index_launch(idx, LOOKUP_PREDICT, d_q, n, d_out, d_err, nullptr, st);
                          });
 }
 
@@ -2815,7 +2794,7 @@ int shard_lookup_search(const rmi_shard_index* si, const T* d_recv, uint64_t m, 
   PoolScratch s{nullptr, st};
   CUDA_TRY(cudaMallocAsync(&s.p, 2 * sizeof(u64) * m, st));
   uint64_t* pos = (uint64_t*)s.p;   // m predictions, then their error bounds
-  if (int rc = index_launch(idx, d_recv, m, pos, pos + m, nullptr, st, false)) return rc;
+  if (int rc = index_launch(idx, LOOKUP_PREDICT, d_recv, m, pos, pos + m, nullptr, st)) return rc;
   Launch L{st, idx->num_sms};
   shard_search<T>(L, (const T*)ds->d_keys, ds->n, si->base, si->n_global, d_recv, m, (const u64*)pos,
                   (const u64*)pos + m, d_answers, d_fallbacks, upper, rmihost::key_from_bits<T>(idx->last_key_bits));
@@ -2830,7 +2809,7 @@ int shard_predict_route(const rmi_shard_index* si, const u64* d_q, uint64_t n, u
   PoolScratch s{nullptr, st};
   if (n) CUDA_TRY(cudaMallocAsync(&s.p, 2 * sizeof(u64) * n, st));
   uint64_t* pos = (uint64_t*)s.p;   // n predictions, then their error bounds
-  if (int rc = index_launch(si->idx, d_q, n, pos, pos + n, nullptr, st, false)) return rc;
+  if (int rc = index_launch(si->idx, LOOKUP_PREDICT, d_q, n, pos, pos + n, nullptr, st)) return rc;
   Launch L{st, si->idx->num_sms};
   shard_knot_route_keys(L, (const u64*)pos, (const u64*)pos + n, n, (u64*)pos);
   ShardRoute<u64> route;
@@ -3015,7 +2994,7 @@ int rmi_shard_index_predict(const rmi_shard_index* si, const void* d_queries, ui
     return fail(RMI_ERR_INVALID, "rmi_shard_index_predict: a bounded index predicts collectively "
                                  "(rmi_shard_index_predict_collective, or its phases)");
   if (int rc = index_check_call(si->idx, d_queries, n, d_pos, "rmi_shard_index_predict")) return rc;
-  return index_launch(si->idx, d_queries, n, d_pos, d_err, nullptr, cuda_stream, false);
+  return index_launch(si->idx, LOOKUP_PREDICT, d_queries, n, d_pos, d_err, nullptr, cuda_stream);
 }
 
 }  // extern "C"

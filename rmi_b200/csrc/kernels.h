@@ -3,6 +3,7 @@
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
+#include <type_traits>
 
 #include "models.cuh"
 
@@ -179,39 +180,63 @@ void leaf_statistics_owned(const Launch& L, u64 n, u64 N, const u64* d_errors, c
                            int world, void* d_part_out, void* scratch);
 void leaf_statistics_merge(const Launch& L, const void* d_parts, int world, BuildAux* d_aux);
 
-// ---- batched lookups on a trained index (kernels_lookup.cu) -----------------------------------
-// The model groups the lookup kernel is instantiated for (-1: not a top / leaf model): the linear family shares
+// ---- batched lookups on a trained index (kernels_lookup.cu, kernels_lookup_range.cu) ------------------------------
+// The model groups the lookup kernels are instantiated for (-1: not a top / leaf model): the linear family shares
 // one group, as in compute_leaf_bounds.
-int lookup_top_group(int kind);
-int lookup_leaf_group(int kind);
+inline int lookup_top_group(int kind) {
+  if (kind == M_LINEAR || kind == M_ROBUST_LINEAR || kind == M_LINEAR_SPLINE) return M_LINEAR;
+  return kind >= M_LINEAR && kind <= M_HISTOGRAM ? kind : -1;
+}
+inline int lookup_leaf_group(int kind) {
+  if (kind == M_LINEAR || kind == M_ROBUST_LINEAR || kind == M_LINEAR_SPLINE) return M_LINEAR;
+  return kind >= M_CUBIC && kind <= M_LOGNORMAL ? kind : -1;
+}
+template <int K> using Kind = std::integral_constant<int, K>;
+// f(Kind<TOP>, Kind<LEAF>) for the kernel group of the given top and leaf model kinds.
+template <class F> void with_groups(int top_kind, int leaf_kind, F&& f) {
+  auto leaf = [&](auto top) {
+    switch (lookup_leaf_group(leaf_kind)) {
+      case M_LINEAR: f(top, Kind<M_LINEAR>{}); break;
+      case M_CUBIC: f(top, Kind<M_CUBIC>{}); break;
+      case M_LOGLINEAR: f(top, Kind<M_LOGLINEAR>{}); break;
+      case M_NORMAL: f(top, Kind<M_NORMAL>{}); break;
+      default: f(top, Kind<M_LOGNORMAL>{}); break;
+    }
+  };
+  switch (lookup_top_group(top_kind)) {
+    case M_LINEAR: leaf(Kind<M_LINEAR>{}); break;
+    case M_CUBIC: leaf(Kind<M_CUBIC>{}); break;
+    case M_LOGLINEAR: leaf(Kind<M_LOGLINEAR>{}); break;
+    case M_NORMAL: leaf(Kind<M_NORMAL>{}); break;
+    case M_LOGNORMAL: leaf(Kind<M_LOGNORMAL>{}); break;
+    case M_RADIX: leaf(Kind<M_RADIX>{}); break;
+    case M_RADIX_TABLE: leaf(Kind<M_RADIX_TABLE>{}); break;
+    case M_BRADIX: leaf(Kind<M_BRADIX>{}); break;
+    default: leaf(Kind<M_HISTOGRAM>{}); break;
+  }
+}
 // One packed record per leaf: its parameters in Model::params() order, then its error bound.
 __host__ __device__ constexpr int lookup_record_bytes(int leaf_kind) { return leaf_kind == M_CUBIC ? 64 : 32; }
 // N records (N x lookup_record_bytes bytes at `out`, host memory) from N x ppm parameters and N errors.
 void pack_leaf_records(int leaf_kind, const double* params, const u64* errors, u64 N, void* out);
-// One kernel launch on L.stream (none for nq == 0).  lower_bound = false: out = position estimates, out_err (may be
-// null) = the leaves' error bounds.  lower_bound = true: out = exact lower bounds over keys[0, n); *fallbacks (may be
-// null) grows by the number of queries whose error window missed.  `top` is passed by value; its table pointers
-// (t32, pivots) are device memory.
+// What a lookup computes, and into which of its two outputs:
+//   LOOKUP_PREDICT      out = position estimates, out2 (may be null) = the leaves' error bounds
+//   LOOKUP_LOWER        out = exact lower bounds (the number of keys < q)
+//   LOOKUP_UPPER        out = exact upper bounds (the number of keys <= q; 0 for NaN)
+//   LOOKUP_EQUAL_RANGE  out = lower bounds, out2 = upper bounds, from one window per query
+enum LookupMode { LOOKUP_PREDICT, LOOKUP_LOWER, LOOKUP_UPPER, LOOKUP_EQUAL_RANGE };
+// One kernel launch on L.stream (none for nq == 0) over keys[0, n); last = keys[n-1], and the upper bound of a query
+// >= it is n without a search.  *fallbacks (may be null) grows by the number of queries whose window missed (either
+// end).  `top` is passed by value; its table pointers (t32, pivots) are device memory.
 template <class T>
-void lookup_batch(const Launch& L, const TopModel& top, int leaf_kind, const void* d_records, u64 N, const T* keys, u64 n,
-                  const T* d_queries, u64 nq, u64* d_out, u64* d_out_err, u64* d_fallbacks, bool lower_bound);
+void lookup_batch(const Launch& L, LookupMode mode, const TopModel& top, int leaf_kind, const void* d_records, u64 N,
+                  const T* keys, u64 n, T last, const T* d_queries, u64 nq, u64* d_out, u64* d_out2, u64* d_fallbacks);
 // The same for a bounded (cache-fix) index over u64 keys: the RMI (d_records, N leaves) predicts one of the K knots
-// at d_knots (K x {key, offset}, 16 bytes each), the spline step gives the key's line of line_size keys, and
-// lower_bound searches that line.  out_err receives line_size.
-void lookup_bounded_batch(const Launch& L, const TopModel& top, int leaf_kind, const void* d_records, u64 N,
-                          const void* d_knots, u64 K, u64 line_size, const u64* keys, u64 n, const u64* d_queries,
-                          u64 nq, u64* d_out, u64* d_out_err, u64* d_fallbacks, bool lower_bound);
-// Exact upper bounds (the number of keys <= q; 0 for NaN) of nq queries into d_last, and with d_first non-null the
-// lower bounds too (equal_range), from one window per query (kernels_lookup_range.cu).  last = keys[n-1]; queries >= it
-// get n without a search.  One launch (none for nq == 0); *d_fallbacks (may be null) grows by the queries whose window
-// missed either end.
-template <class T>
-void lookup_range_batch(const Launch& L, const TopModel& top, int leaf_kind, const void* d_records, u64 N, const T* keys,
-                        u64 n, T last, const T* d_queries, u64 nq, u64* d_first, u64* d_last, u64* d_fallbacks);
-// The same on a bounded index (lookup_bounded_batch's arguments), searching the key line of lookup_bounded_batch.
-void lookup_bounded_range_batch(const Launch& L, const TopModel& top, int leaf_kind, const void* d_records, u64 N,
-                                const void* d_knots, u64 K, u64 line_size, const u64* keys, u64 n, u64 last,
-                                const u64* d_queries, u64 nq, u64* d_first, u64* d_last, u64* d_fallbacks);
+// at d_knots (K x {key, offset}, 16 bytes each), the spline step gives the key's line of line_size keys, and the
+// bounds are searched in that line.  A prediction's error bound is line_size.
+void lookup_bounded_batch(const Launch& L, LookupMode mode, const TopModel& top, int leaf_kind, const void* d_records,
+                          u64 N, const void* d_knots, u64 K, u64 line_size, const u64* keys, u64 n, u64 last,
+                          const u64* d_queries, u64 nq, u64* d_out, u64* d_out2, u64* d_fallbacks);
 
 // ---- lookups over a range-partitioned data set (kernels_shard_lookup.cu, DESIGN.md section 14) -------------------
 // A query goes to the last non-empty rank whose first key is < q (the first non-empty rank if none is).

@@ -22,7 +22,6 @@
 // themselves to the positions the route gave (scatter_queries).
 #include "kernels.h"
 #include "lookup_search.cuh"
-#include "spline.cuh"
 
 namespace rmi {
 
@@ -37,7 +36,6 @@ k_shard_bounded(const __grid_constant__ TopModel top, const ulonglong2* __restri
                 const __grid_constant__ BoundedKnotSlab ks, const u64* __restrict__ keys, u64 n_local, u64 base,
                 u64 n_global, const u64* __restrict__ qs, u64 m, u64* __restrict__ out, u64* fallbacks,
                 int lower_bound, u64 last) {
-  using R = Rec<LEAF>;
   const ulonglong2* __restrict__ kext = (const ulonglong2*)ks.knots;
   const u64 K = ks.K, line = ks.line;
   unsigned misses = 0, local_misses = 0;
@@ -47,36 +45,18 @@ k_shard_bounded(const __grid_constant__ TopModel top, const ulonglong2* __restri
       __stcs(out + i, base + n_local);
       continue;
     }
-    u64 t = top_predict<TOP>(top, q);
-    t = t < N - 1 ? t : N - 1;
-    ulonglong2 v[R::LOADS];
-#pragma unroll
-    for (int k = 0; k < R::LOADS; ++k) v[k] = __ldg(recs + t * R::VECS + k);
-    double f[4];
     u64 e;
-    R::unpack(v, f, e);
-    u64 start = leaf_predict64<LEAF>(f, Key<u64>::as_float(q));
-    start = start < K - 1 ? start : K - 1;
-    const u64 lower = e > start ? 0 : start - e;
-    const u64 upper = e >= K - start ? K : start + e;
+    const u64 start = rmi_predict<TOP, LEAF>(top, recs, N, K, q, e);
+    const Window kw = error_window(start, e, K);
     u64 r;
-    if (lower_bound && (upper < ks.a0 || lower > ks.a1)) {
+    if (lower_bound && (kw.hi < ks.a0 || kw.lo > ks.a1)) {
       // far: the whole slab, whose edges confirm themselves
       RMI_LINE_SEARCH_AS(keys, n_local, q, (u64)0, n_local, n_local, local_misses, r, UPPER);
       ++misses;
       __stcs(out + i, base + r);
       continue;
     }
-    const u64 res = knot_window_search(kext, lower - ks.k_lo, upper - ks.k_lo, q) + ks.k_lo;
-    u64 pos;
-    if (res == K) {
-      pos = n_global - 1;
-    } else if (res == 0) {
-      pos = 0;
-    } else {
-      const ulonglong2 p0 = kext[res - ks.k_lo - 1], p1 = kext[res - ks.k_lo];
-      pos = cache_fix_interp(q, p0.x, p0.y, p1.x, p1.y) / line * line;
-    }
+    const u64 pos = bounded_pos(kext, ks.k_lo, kw.lo, kw.hi, K, n_global, line, q);
     if (!lower_bound) {
       __stcs(out + i, pos);
       continue;
@@ -90,40 +70,7 @@ k_shard_bounded(const __grid_constant__ TopModel top, const ulonglong2* __restri
     if (base + r < glo || base + r > ghi) ++misses;
     __stcs(out + i, base + r);
   }
-  if (fallbacks) {
-    misses = __reduce_add_sync(0xffffffffu, misses);
-    if ((threadIdx.x & 31) == 0 && misses) atomicAdd((unsigned long long*)fallbacks, (unsigned long long)misses);
-  }
-}
-
-template <int TOP, int LEAF>
-void launch_shard_bounded(const Launch& L, const TopModel& top, const void* recs, u64 N, const BoundedKnotSlab& ks,
-                          const u64* keys, u64 n_local, u64 base, u64 n_global, const u64* q, u64 m, u64* out,
-                          u64* fallbacks, bool lb, bool upper, u64 last) {
-  u64 blocks = (m + SB_THREADS - 1) / SB_THREADS;
-  const u64 cap = (u64)L.num_sms * SB_MAX_BLOCKS_PER_SM;
-  if (blocks > cap) blocks = cap;
-  if (upper)
-    k_shard_bounded<TOP, LEAF, true><<<(unsigned)blocks, SB_THREADS, 0, L.stream>>>(
-        top, (const ulonglong2*)recs, N, ks, keys, n_local, base, n_global, q, m, out, fallbacks, 1, last);
-  else
-    k_shard_bounded<TOP, LEAF, false><<<(unsigned)blocks, SB_THREADS, 0, L.stream>>>(
-        top, (const ulonglong2*)recs, N, ks, keys, n_local, base, n_global, q, m, out, fallbacks, lb ? 1 : 0, last);
-  count_launch();
-}
-
-#define RMI_SB_ARGS recs, N, ks, keys, n_local, base, n_global, q, m, out, fallbacks, lb, upper, last
-template <int TOP>
-void shard_bounded_leaf(const Launch& L, const TopModel& top, int leaf_kind, const void* recs, u64 N,
-                        const BoundedKnotSlab& ks, const u64* keys, u64 n_local, u64 base, u64 n_global, const u64* q,
-                        u64 m, u64* out, u64* fallbacks, bool lb, bool upper, u64 last) {
-  switch (lookup_leaf_group(leaf_kind)) {
-    case M_LINEAR: launch_shard_bounded<TOP, M_LINEAR>(L, top, RMI_SB_ARGS); break;
-    case M_CUBIC: launch_shard_bounded<TOP, M_CUBIC>(L, top, RMI_SB_ARGS); break;
-    case M_LOGLINEAR: launch_shard_bounded<TOP, M_LOGLINEAR>(L, top, RMI_SB_ARGS); break;
-    case M_NORMAL: launch_shard_bounded<TOP, M_NORMAL>(L, top, RMI_SB_ARGS); break;
-    default: launch_shard_bounded<TOP, M_LOGNORMAL>(L, top, RMI_SB_ARGS); break;
-  }
+  flush_fallbacks(misses, fallbacks);
 }
 
 __global__ void __launch_bounds__(256)
@@ -144,47 +91,40 @@ __global__ void __launch_bounds__(256) k_fill(u64 v, u64 n, u64* __restrict__ ou
   for (u64 i = (u64)blockIdx.x * 256 + threadIdx.x; i < n; i += (u64)gridDim.x * 256) __stcs(out + i, v);
 }
 
-unsigned elementwise_blocks(const Launch& L, u64 n) {
-  u64 blocks = (n + 255) / 256;
-  const u64 cap = (u64)L.num_sms * 16;
-  return (unsigned)(blocks > cap ? cap : blocks);
-}
-
 }  // namespace
 
 void shard_bounded_search(const Launch& L, const TopModel& top, int leaf_kind, const void* recs, u64 N,
                           const BoundedKnotSlab& ks, const u64* keys, u64 n_local, u64 base, u64 n_global, const u64* q,
                           u64 m, u64* out, u64* fallbacks, bool lb, bool upper, u64 last) {
   if (m == 0) return;
-  switch (lookup_top_group(top.kind)) {
-    case M_LINEAR: shard_bounded_leaf<M_LINEAR>(L, top, leaf_kind, RMI_SB_ARGS); break;
-    case M_CUBIC: shard_bounded_leaf<M_CUBIC>(L, top, leaf_kind, RMI_SB_ARGS); break;
-    case M_LOGLINEAR: shard_bounded_leaf<M_LOGLINEAR>(L, top, leaf_kind, RMI_SB_ARGS); break;
-    case M_NORMAL: shard_bounded_leaf<M_NORMAL>(L, top, leaf_kind, RMI_SB_ARGS); break;
-    case M_LOGNORMAL: shard_bounded_leaf<M_LOGNORMAL>(L, top, leaf_kind, RMI_SB_ARGS); break;
-    case M_RADIX: shard_bounded_leaf<M_RADIX>(L, top, leaf_kind, RMI_SB_ARGS); break;
-    case M_RADIX_TABLE: shard_bounded_leaf<M_RADIX_TABLE>(L, top, leaf_kind, RMI_SB_ARGS); break;
-    case M_BRADIX: shard_bounded_leaf<M_BRADIX>(L, top, leaf_kind, RMI_SB_ARGS); break;
-    default: shard_bounded_leaf<M_HISTOGRAM>(L, top, leaf_kind, RMI_SB_ARGS); break;
-  }
+  const unsigned blocks = capped_grid(L, m, SB_THREADS, SB_MAX_BLOCKS_PER_SM);
+  with_groups(top.kind, leaf_kind, [&](auto tk, auto lk) {
+    constexpr int TOP = decltype(tk)::value, LEAF = decltype(lk)::value;
+    if (upper)
+      k_shard_bounded<TOP, LEAF, true><<<blocks, SB_THREADS, 0, L.stream>>>(
+          top, (const ulonglong2*)recs, N, ks, keys, n_local, base, n_global, q, m, out, fallbacks, 1, last);
+    else
+      k_shard_bounded<TOP, LEAF, false><<<blocks, SB_THREADS, 0, L.stream>>>(
+          top, (const ulonglong2*)recs, N, ks, keys, n_local, base, n_global, q, m, out, fallbacks, lb ? 1 : 0, last);
+  });
+  count_launch();
 }
-#undef RMI_SB_ARGS
 
 void shard_knot_route_keys(const Launch& L, const u64* d_pos, const u64* d_err, u64 n, u64* d_out) {
   if (n == 0) return;
-  k_knot_route_keys<<<elementwise_blocks(L, n), 256, 0, L.stream>>>(d_pos, d_err, n, d_out);
+  k_knot_route_keys<<<capped_grid(L, n, 256, 16), 256, 0, L.stream>>>(d_pos, d_err, n, d_out);
   count_launch();
 }
 
 void shard_scatter_queries(const Launch& L, const u64* d_q, const u64* d_slot, u64 n, u64* d_send) {
   if (n == 0) return;
-  k_scatter_queries<<<elementwise_blocks(L, n), 256, 0, L.stream>>>(d_q, d_slot, n, d_send);
+  k_scatter_queries<<<capped_grid(L, n, 256, 16), 256, 0, L.stream>>>(d_q, d_slot, n, d_send);
   count_launch();
 }
 
 void shard_fill(const Launch& L, u64 value, u64 n, u64* d_out) {
   if (n == 0) return;
-  k_fill<<<elementwise_blocks(L, n), 256, 0, L.stream>>>(value, n, d_out);
+  k_fill<<<capped_grid(L, n, 256, 16), 256, 0, L.stream>>>(value, n, d_out);
   count_launch();
 }
 

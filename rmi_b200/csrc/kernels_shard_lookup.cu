@@ -170,18 +170,15 @@ k_shard_search(const T* __restrict__ keys, u64 n_local, u64 base, u64 n_global, 
     const bool live[1] = {true};
     const u64 p = __ldcs(pos + i), e = __ldcs(err + i);
     // the global window, then its part inside this slab
-    const u64 glo = p >= e ? p - e : 0;
-    const u64 ghi = e >= n_global - p ? n_global : p + e;
+    const Window g = error_window(p, e, n_global);
+    const u64 glo = g.lo, ghi = g.hi;
     u64 lo[1], hi[1];
     lo[0] = glo <= base ? 0 : (glo - base < n_local ? glo - base : n_local);
     hi[0] = ghi <= base ? 0 : (ghi - base < n_local ? ghi - base : n_local);
     window_search<T, 1, UPPER ? 1u : 0u>(keys, n_local, q, live, lo, hi, misses,
                                          [&](int, u64 r) { __stcs(out + i, base + r); });
   }
-  if (fallbacks) {
-    misses = __reduce_add_sync(0xffffffffu, misses);
-    if ((threadIdx.x & 31) == 0 && misses) atomicAdd((unsigned long long*)fallbacks, (unsigned long long)misses);
-  }
+  flush_fallbacks(misses, fallbacks);
 }
 
 __global__ void __launch_bounds__(256)
@@ -222,24 +219,19 @@ template <class T>
 void shard_search(const Launch& L, const T* keys, u64 n_local, u64 base, u64 n_global, const T* q, u64 m,
                   const u64* d_pos, const u64* d_err, u64* d_out, u64* d_fallbacks, bool upper, T last) {
   if (m == 0) return;
-  u64 blocks = (m + SEARCH_THREADS - 1) / SEARCH_THREADS;
-  const u64 cap = (u64)L.num_sms * SEARCH_MAX_BLOCKS_PER_SM;
-  if (blocks > cap) blocks = cap;
+  const unsigned blocks = capped_grid(L, m, SEARCH_THREADS, SEARCH_MAX_BLOCKS_PER_SM);
   if (upper)
-    k_shard_search<T, true><<<(unsigned)blocks, SEARCH_THREADS, 0, L.stream>>>(keys, n_local, base, n_global, q, m,
-                                                                              d_pos, d_err, d_out, d_fallbacks, last);
+    k_shard_search<T, true><<<blocks, SEARCH_THREADS, 0, L.stream>>>(keys, n_local, base, n_global, q, m, d_pos, d_err,
+                                                                     d_out, d_fallbacks, last);
   else
-    k_shard_search<T, false><<<(unsigned)blocks, SEARCH_THREADS, 0, L.stream>>>(keys, n_local, base, n_global, q, m,
-                                                                               d_pos, d_err, d_out, d_fallbacks, last);
+    k_shard_search<T, false><<<blocks, SEARCH_THREADS, 0, L.stream>>>(keys, n_local, base, n_global, q, m, d_pos, d_err,
+                                                                      d_out, d_fallbacks, last);
   count_launch();
 }
 
 void shard_gather(const Launch& L, const u64* d_slot, const u64* d_returned, u64 n, u64* d_out) {
   if (n == 0) return;
-  u64 blocks = (n + 255) / 256;
-  const u64 cap = (u64)L.num_sms * 16;
-  if (blocks > cap) blocks = cap;
-  k_shard_gather<<<(unsigned)blocks, 256, 0, L.stream>>>(d_slot, d_returned, n, d_out);
+  k_shard_gather<<<capped_grid(L, n, 256, 16), 256, 0, L.stream>>>(d_slot, d_returned, n, d_out);
   count_launch();
 }
 

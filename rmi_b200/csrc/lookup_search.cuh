@@ -1,7 +1,8 @@
 // lookup_search.cuh — the exact search of a lookup's error window, shared by the single-GPU lookup kernels
 // (kernels_lookup.cu, kernels_lookup_range.cu) and the searches over a rank's slab of a range-partitioned data set
-// (kernels_shard_lookup.cu, kernels_shard_bounded.cu), with the pieces of a bounded lookup every bounded kernel takes:
-// the knot-window search, the key-line step and the packed leaf record.
+// (kernels_shard_lookup.cu, kernels_shard_bounded.cu), with the steps every lookup kernel takes: the packed leaf
+// record and the RMI step over it, the error window, the bounded index's spline step and key-line search, the
+// fallback count and the grid.
 //
 // For a window [lo, hi] of candidate answers over keys[0, n): a branchless binary search over keys [lo, hi),
 // confirmed by the keys just outside the window (lo == 0 and hi == n need no confirmation), and a galloping search
@@ -13,20 +14,43 @@
 #pragma once
 #include <type_traits>
 
+#include "kernels.h"
 #include "models.cuh"
+#include "spline.cuh"
 
 namespace rmi {
 namespace {
 
-// Queries per thread and threads per block of the lookup kernels, measured on an H100 SXM (DESIGN §11) on the headline
-// index (linear,linear 2^20 over 200M uint64 keys, 2^27 random present keys): lower_bound took 27.4 / 34.2 / 36.6 /
-// 37.0 ms at 1 / 2 / 4 / 8 queries per thread with 128 threads (28.4 / 33.9 / 35.2 / 37.2 ms with 256); predict
-// was 2.65-2.72 ms at 1, 2 and 4 and 2.95 ms at 8.  One query per thread needs 32 registers, so 64 warps fit on
-// an SM, and those warps keep more probes in flight than fewer warps carrying several queries each: the lockstep
-// search waits for the longest window of its queries, and the registers it needs cost warps.
-constexpr int LOOKUP_Q = 1;
+// Threads per block of the lookup kernels, each thread one query at a time (grid-stride).  Measured on an H100 SXM
+// (DESIGN §11) on the headline index (linear,linear 2^20 over 200M uint64 keys, 2^27 random present keys):
+// lower_bound took 27.4 / 34.2 / 36.6 / 37.0 ms at 1 / 2 / 4 / 8 queries per thread with 128 threads (28.4 / 33.9 /
+// 35.2 / 37.2 ms with 256); predict was 2.65-2.72 ms at 1, 2 and 4 and 2.95 ms at 8.  One query per thread needs 32
+// registers, so 64 warps fit on an SM, and those warps keep more probes in flight than fewer warps carrying several
+// queries each: a lockstep search waits for the longest window of its queries, and the registers it needs cost warps.
 constexpr int LOOKUP_THREADS = 128;
-constexpr int LOOKUP_MAX_BLOCKS_PER_SM = 32;   // grid cap; beyond it the blocks stride over the tiles
+constexpr int LOOKUP_MAX_BLOCKS_PER_SM = 32;   // grid cap; beyond it the blocks stride over the queries
+
+// The grid of a grid-stride kernel over n items: one block per `threads` items, at most per_sm blocks per SM.
+inline unsigned capped_grid(const Launch& L, u64 n, int threads, int per_sm) {
+  const u64 blocks = (n + threads - 1) / threads, cap = (u64)L.num_sms * per_sm;
+  return (unsigned)(blocks < cap ? blocks : cap);
+}
+
+// Adds the warp's misses to *fallbacks (may be null): the epilogue of every lookup kernel.  Every lane of the warp
+// calls it.
+__device__ __forceinline__ void flush_fallbacks(unsigned misses, u64* fallbacks) {
+  if (fallbacks) {
+    misses = __reduce_add_sync(0xffffffffu, misses);
+    if ((threadIdx.x & 31) == 0 && misses) atomicAdd((unsigned long long*)fallbacks, (unsigned long long)misses);
+  }
+}
+
+// The window [pos-err, pos+err] ∩ [0, rows] for pos < rows, without wrapping.  The arguments are references: taken
+// by value, the comparisons inline with their operands swapped, the same logic in different SASS.
+struct Window { u64 lo, hi; };
+__device__ __forceinline__ Window error_window(const u64& pos, const u64& err, const u64& rows) {
+  return {pos >= err ? pos - err : 0, err >= rows - pos ? rows : pos + err};
+}
 
 // Whether key k counts before q: k < q, or k <= q for UPPER.  search_range and lookup_fallback spell the same
 // conditional out: through this helper the float64 instances of the strict fallback compiled to different SASS.
@@ -210,6 +234,24 @@ template <int LEAF> struct Rec {
   }
 };
 
+// The RMI step of a lookup: leaf t = min(N-1, top(q)), then from its record the position min(rows-1, leaf_t(q)),
+// returned, and the leaf's error bound err.  rows: the keys of a plain index, the knots of a bounded one.
+template <int TOP, int LEAF, class T>
+__device__ __forceinline__ u64 rmi_predict(const TopModel& top, const ulonglong2* __restrict__ recs, u64 N, u64 rows,
+                                           T q, u64& err) {
+  using R = Rec<LEAF>;
+  u64 t = top_predict<TOP>(top, q);
+  t = t < N - 1 ? t : N - 1;
+  ulonglong2 v[R::LOADS];
+#pragma unroll
+  for (int k = 0; k < R::LOADS; ++k) v[k] = __ldg(recs + t * R::VECS + k);
+  double f[4];
+  R::unpack(v, f, err);
+  u64 pos = leaf_predict64<LEAF>(f, Key<T>::as_float(q));
+  pos = pos < rows - 1 ? pos : rows - 1;
+  return pos;
+}
+
 // First index in [lo, hi) whose knot key is not < q, or hi: the generated spline lookup's search of the knot window
 // (codegen.rs:410-437), on {key, offset} knots.
 __device__ __forceinline__ u64 knot_window_search(const ulonglong2* __restrict__ knots, u64 lo, u64 hi, u64 q) {
@@ -220,6 +262,19 @@ __device__ __forceinline__ u64 knot_window_search(const ulonglong2* __restrict__
     len -= h;
   }
   return len == 1 && knots[b].x < q ? b + 1 : b;
+}
+
+// The spline step of a bounded lookup over K knots and n keys, from the knot window [lower, upper) of the RMI step:
+// res = the window's first knot whose key is not < q; n - 1 past the last knot, 0 before the first, else the spline
+// between knots res-1 and res rounded down to its line (codegen.rs:410-437).  knots holds the global knots from k_lo
+// on (0 on one GPU), the window among them.
+__device__ __forceinline__ u64 bounded_pos(const ulonglong2* __restrict__ knots, u64 k_lo, u64 lower, u64 upper, u64 K,
+                                           u64 n, u64 line, u64 q) {
+  const u64 res = knot_window_search(knots, lower - k_lo, upper - k_lo, q) + k_lo;
+  if (res == K) return n - 1;
+  if (res == 0) return 0;
+  const ulonglong2 p0 = knots[res - k_lo - 1], p1 = knots[res - k_lo];
+  return cache_fix_interp(q, p0.x, p0.y, p1.x, p1.y) / line * line;
 }
 
 }  // namespace
