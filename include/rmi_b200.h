@@ -99,6 +99,8 @@ int rmi_dataset_load_file(const char* path, int key_type_or_negative, int device
  * configuration) after the key file has been read once. */
 int rmi_dataset_replicate(const rmi_dataset* src, int device, rmi_dataset** out);
 uint64_t rmi_dataset_len(const rmi_dataset* ds);
+/* Copies the rmi_dataset_len(ds) keys to host_keys, synchronously (for example the keys rmi_delta_merge made). */
+int rmi_dataset_copy_to_host(const rmi_dataset* ds, void* host_keys);
 int rmi_dataset_key_type(const rmi_dataset* ds);
 void rmi_dataset_destroy(rmi_dataset* ds);
 
@@ -246,6 +248,52 @@ int rmi_index_equal_range(const rmi_index* idx, const void* d_queries, uint64_t 
  * (lower bounds into host_first).  *fallbacks (may be NULL) is SET to the fallback count. */
 int rmi_index_range_host(const rmi_index* idx, const void* host_queries, uint64_t n, uint64_t* host_first,
                          uint64_t* host_last, uint64_t* fallbacks);
+
+/* ---- Updatable indexes: lookups over inserted keys (DESIGN.md section 19) -------------------------------------------
+ * An rmi_delta wraps an rmi_index, plain or bounded, and a device-resident sorted array of the keys inserted since that
+ * index was built (the delta, m keys).  Its logical key set is the multiset base keys ∪ inserted keys, and every
+ * answer is exact over it:
+ *   lower_bound(q) = the base index's lower_bound(q) + #{d in delta : d < q}; upper_bound likewise with d <= q;
+ *   equal_range(q) = both.  A NaN query gives [0, 0), as on the base index.  The fallback counts are the base index's:
+ *   the delta's part is an exact search and adds none.
+ * There is no predict: the model's positions refer to the base keys only.
+ * Equal keys keep one order everywhere: base keys before equal inserted keys, earlier inserts before later ones, keys
+ * compared by value (-0.0 == 0.0).  So rmi_delta_merge's keys are the stable sort of the base keys followed by every
+ * batch in insert order.
+ * Concurrency: lookups on one rmi_delta may run concurrently on several streams.  rmi_delta_insert and
+ * rmi_delta_destroy must not overlap any other call on the same handle, lookups still in flight on other streams
+ * included.  The base index is unchanged and immutable; base (and its dataset) must outlive the rmi_delta. */
+typedef struct rmi_delta rmi_delta;
+int rmi_delta_create(const rmi_index* base, rmi_delta** out);
+void rmi_delta_destroy(rmi_delta* d);
+/* Merges a batch into the delta, synchronously: on the calling thread's stream (cudaStreamPerThread), returning when
+ * the merge has finished.  The batch must be a sorted data set (batch->sorted, as rmi_dataset_create and
+ * rmi_dataset_wrap_device find it) of the base's key type on the base's device; duplicates, of any key, are fine.
+ * Refused with RMI_ERR_INVALID: a null argument, another key type or device, an unsorted batch, and (after the merge,
+ * which finds it) a float64 batch that holds a NaN.  A refused batch leaves the delta unchanged.  The delta's storage
+ * is two device buffers that trade places at every insert; a buffer that is too small is replaced by one of twice
+ * the larger capacity (at least the keys it has to hold). */
+int rmi_delta_insert(rmi_delta* d, const rmi_dataset* batch);
+/* Keys inserted so far (m). */
+uint64_t rmi_delta_len(const rmi_delta* d);
+/* As rmi_index_lower_bound / _upper_bound / _equal_range over the logical key set: the base index's launch, then, on
+ * the same stream, one launch that adds the delta's counts to the outputs (none when m == 0, so the answers and the
+ * launch count are then the base index's; none at all for n == 0). */
+int rmi_delta_lower_bound(const rmi_delta* d, const void* d_queries, uint64_t n, uint64_t* d_out,
+                          uint64_t* d_fallbacks, void* cuda_stream);
+int rmi_delta_upper_bound(const rmi_delta* d, const void* d_queries, uint64_t n, uint64_t* d_out,
+                          uint64_t* d_fallbacks, void* cuda_stream);
+int rmi_delta_equal_range(const rmi_delta* d, const void* d_queries, uint64_t n, uint64_t* d_first,
+                          uint64_t* d_last, uint64_t* d_fallbacks, void* cuda_stream);
+/* The same on host arrays, synchronously: lower bounds into host_first, upper bounds into host_last; either may be
+ * NULL, not both.  *fallbacks (may be NULL) is SET to the fallback count. */
+int rmi_delta_range_host(const rmi_delta* d, const void* host_queries, uint64_t n, uint64_t* host_first,
+                         uint64_t* host_last, uint64_t* fallbacks);
+/* A new, owned data set of the n + m merged keys on the base's device (the base keys alone for an empty delta), with
+ * its sorted and no_dups flags found by the same check as rmi_dataset_create's.  Release it with
+ * rmi_dataset_destroy.  Compaction trains or evaluates an index over it (rmi_train, rmi_evaluate,
+ * rmi_cache_fix_device) and wraps that index in a new rmi_delta. */
+int rmi_delta_merge(const rmi_delta* d, rmi_dataset** out);
 
 /* ---- Range-partitioned (multi-GPU) build ----------------------------------------------------
  * One process per GPU; rank r holds the r-th contiguous slab of the globally sorted key array

@@ -14,15 +14,16 @@ The product is the C-ABI shared library ``rmi_b200/lib/librmi_b200.so`` (CUDA, s
 plus RMIIndex and BoundedRMIIndex (a train_bounded build), batched lookups (position estimates and exact lower
 bounds) on the GPU.  cache_fix / train_bounded on an RMITrainingData fit the cache-fix spline on the GPU.
 rmi_b200.sharded (torch.distributed) trains over range-partitioned keys (train_sharded), evaluates a given RMI over
-them (evaluate_sharded) and serves lookups over them (ShardedRMIIndex).
+them (evaluate_sharded) and serves lookups over them (ShardedRMIIndex).  DeltaRMIIndex serves exact lookups over keys
+inserted after an index was built, and compacts them into a fresh index.
 
 and does no arithmetic of its own.  There is no CPU fallback: if the CUDA library is missing
 or no device is present, calls raise.
 """
-from .api import (BoundedRMIIndex, KEY_F64, KEY_U32, KEY_U64, FLAG_LEAF_COUNTS, FLAG_SHARD_ROOT_ONLY, FLAG_STATS_ONLY, FLAG_TOP_FIT_EXACT, RMIError, RMIIndex, RMIPanic,
+from .api import (BoundedRMIIndex, DeltaRMIIndex, KEY_F64, KEY_U32, KEY_U64, FLAG_LEAF_COUNTS, FLAG_SHARD_ROOT_ONLY, FLAG_STATS_ONLY, FLAG_TOP_FIT_EXACT, RMIError, RMIIndex, RMIPanic,
                   RMITrainingData, TrainedRMI, cache_fix, evaluate, find_pareto_efficient_configs, kernel_launch_count, lib_path,
                   load_data, load_library, load_rmi, output_rmi, rmi_size, train, train_bounded, train_for_size, train_stats_batch, version)
 
-__all__ = ["BoundedRMIIndex", "KEY_F64", "KEY_U32", "KEY_U64", "FLAG_LEAF_COUNTS", "FLAG_SHARD_ROOT_ONLY", "FLAG_STATS_ONLY", "FLAG_TOP_FIT_EXACT", "RMIError", "RMIIndex", "RMIPanic",
+__all__ = ["BoundedRMIIndex", "DeltaRMIIndex", "KEY_F64", "KEY_U32", "KEY_U64", "FLAG_LEAF_COUNTS", "FLAG_SHARD_ROOT_ONLY", "FLAG_STATS_ONLY", "FLAG_TOP_FIT_EXACT", "RMIError", "RMIIndex", "RMIPanic",
            "RMITrainingData", "TrainedRMI", "cache_fix", "evaluate", "find_pareto_efficient_configs", "kernel_launch_count", "lib_path",
            "load_data", "load_library", "load_rmi", "output_rmi", "rmi_size", "train", "train_bounded", "train_for_size", "train_stats_batch", "version"]

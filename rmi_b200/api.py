@@ -86,6 +86,7 @@ def load_library():
         L.rmi_dataset_len.restype = C.c_uint64
         L.rmi_dataset_len.argtypes = [C.c_void_p]
         L.rmi_dataset_key_type.argtypes = [C.c_void_p]
+        L.rmi_dataset_copy_to_host.argtypes = [C.c_void_p, C.c_void_p]
         L.rmi_dataset_destroy.argtypes = [C.c_void_p]
         L.rmi_train.argtypes = [C.c_void_p, C.c_char_p, C.c_uint64, C.c_uint32, C.POINTER(C.POINTER(_Result))]
         L.rmi_train_with_top.argtypes = [C.c_void_p, C.c_char_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_uint32,
@@ -116,6 +117,17 @@ def load_library():
         L.rmi_index_equal_range.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p,
                                             C.c_void_p]
         L.rmi_index_range_host.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.rmi_delta_create.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
+        L.rmi_delta_destroy.argtypes = [C.c_void_p]
+        L.rmi_delta_insert.argtypes = [C.c_void_p, C.c_void_p]
+        L.rmi_delta_len.restype = C.c_uint64
+        L.rmi_delta_len.argtypes = [C.c_void_p]
+        L.rmi_delta_lower_bound.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.rmi_delta_upper_bound.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.rmi_delta_equal_range.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p]
+        L.rmi_delta_range_host.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.rmi_delta_merge.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
         _lib = L
     return _lib
 
@@ -157,6 +169,7 @@ class RMITrainingData:
         keys = np.ascontiguousarray(keys)
         self._h = C.c_void_p()
         self.key_type = _key_type_of(keys.dtype)
+        self.device = int(device)
         self._keep = None
         _check(load_library().rmi_dataset_create(keys.ctypes.data_as(C.c_void_p), keys.size, self.key_type, device,
                                                  C.byref(self._h)))
@@ -166,6 +179,7 @@ class RMITrainingData:
         self = cls.__new__(cls)
         self._h = C.c_void_p()
         self.key_type = key_type
+        self.device = int(device)
         self._keep = keep_alive
         _check(load_library().rmi_dataset_wrap_device(C.c_void_p(ptr), n, key_type, device, C.byref(self._h)))
         return self
@@ -174,6 +188,7 @@ class RMITrainingData:
     def from_file(cls, path: str, key_type: int = -1, device: int = 0) -> "RMITrainingData":
         self = cls.__new__(cls)
         self._h = C.c_void_p()
+        self.device = int(device)
         self._keep = None
         _check(load_library().rmi_dataset_load_file(path.encode(), key_type, device, C.byref(self._h)))
         self.key_type = int(load_library().rmi_dataset_key_type(self._h))
@@ -185,12 +200,19 @@ class RMITrainingData:
         other = type(self).__new__(type(self))
         other._h = C.c_void_p()
         other.key_type = self.key_type
+        other.device = int(device)
         other._keep = None
         _check(load_library().rmi_dataset_replicate(self._h, int(device), C.byref(other._h)))
         return other
 
     def __len__(self) -> int:
         return int(load_library().rmi_dataset_len(self._h))
+
+    def to_numpy(self) -> np.ndarray:
+        """A host copy of the keys."""
+        out = np.empty(len(self), dtype=_NP_OF_KEY[self.key_type])
+        _check(load_library().rmi_dataset_copy_to_host(self._h, out.ctypes.data_as(C.c_void_p)))
+        return out
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
@@ -605,7 +627,133 @@ class BoundedRMIIndex(RMIIndex):
         self._trained = trained
         self.line_size = int(line_size)
         k = np.ascontiguousarray(knots, dtype=np.uint64)
+        self.knots = k
         if k.ndim != 2 or k.shape[1] != 2:
             raise ValueError(f"knots must be a (K, 2) array of (key, offset), got shape {k.shape}")
         _check(load_library().rmi_index_create_bounded(_result_ptr(trained), k.ctypes.data_as(C.c_void_p), k.shape[0],
                                                        self.line_size, data._h, C.byref(self._h)))
+
+
+class DeltaRMIIndex:
+    """An updatable index (DESIGN §19): an ``RMIIndex`` or ``BoundedRMIIndex`` (kept alive here) and a sorted delta of
+    the keys inserted since it was built, on the index's device.  The logical key set is the multiset of the base keys
+    and every inserted key, and ``lower_bound``, ``upper_bound`` and ``equal_range`` are exact over it: the base index's
+    answer plus the number of delta keys below (or, for the upper bound, not above) the query.  Equal keys keep base
+    keys first, then inserted keys in insert order, so ``merged_keys()`` is the stable sort of the base keys followed
+    by every batch.  There is no ``predict``: the model's positions refer to the base keys only.
+
+    ``insert`` must not run while another call on the same object, or a lookup it enqueued, is still in flight; lookups
+    may run concurrently on several streams.  ``len(d)`` is n + m, ``num_inserted`` is m."""
+
+    def __init__(self, index: RMIIndex):
+        self._h = C.c_void_p()
+        self.index = index
+        self.key_type = index.key_type
+        _check(load_library().rmi_delta_create(index._h, C.byref(self._h)))
+
+    @property
+    def num_inserted(self) -> int:
+        return int(load_library().rmi_delta_len(self._h))
+
+    def __len__(self) -> int:
+        return len(self.index.data) + self.num_inserted
+
+    def insert(self, keys) -> None:
+        """Merges a batch into the delta and returns when it is there.  ``keys``: a numpy array of the index's key type
+        (sorted here with a stable sort, then copied to the device), or an RMITrainingData on the index's device (for
+        device-resident batches, RMITrainingData.from_device), which must already be sorted.  A batch that is refused
+        (unsorted, another key type or device, a NaN) leaves the delta unchanged."""
+        if isinstance(keys, RMITrainingData):
+            _check(load_library().rmi_delta_insert(self._h, keys._h))
+            return
+        if not isinstance(keys, np.ndarray) or keys.dtype != np.dtype(_NP_OF_KEY[self.key_type]):
+            got = keys.dtype if isinstance(keys, np.ndarray) else type(keys).__name__
+            raise TypeError(f"keys must be a numpy array of {np.dtype(_NP_OF_KEY[self.key_type])}, got {got}")
+        batch = RMITrainingData(np.sort(keys.ravel(), kind="stable"),
+                                device=self.index.data.device)
+        try:
+            _check(load_library().rmi_delta_insert(self._h, batch._h))
+        finally:
+            batch.close()
+
+    def lower_bound(self, q: np.ndarray, return_fallbacks: bool = False):
+        """Exact lower bound over the logical key set per query (np.uint64); with return_fallbacks also the base
+        index's fallback count."""
+        first, _, fb = self._range(q, True, False)
+        return (first, fb) if return_fallbacks else first
+
+    def upper_bound(self, q: np.ndarray, return_fallbacks: bool = False):
+        """Exact upper bound over the logical key set per query (np.uint64), 0 for NaN."""
+        _, last, fb = self._range(q, False, True)
+        return (last, fb) if return_fallbacks else last
+
+    def equal_range(self, q: np.ndarray, return_fallbacks: bool = False):
+        """(first, last) per query over the logical key set."""
+        first, last, fb = self._range(q, True, True)
+        return (first, last, fb) if return_fallbacks else (first, last)
+
+    def _range(self, q, want_first, want_last):
+        q = self.index._queries(q)
+        first = np.empty(q.size, dtype=np.uint64) if want_first else None
+        last = np.empty(q.size, dtype=np.uint64) if want_last else None
+        fb = C.c_uint64(0)
+        ptr = lambda a: None if a is None else a.ctypes.data_as(C.c_void_p)
+        _check(load_library().rmi_delta_range_host(self._h, q.ctypes.data_as(C.c_void_p), q.size, ptr(first), ptr(last),
+                                                    C.byref(fb)))
+        return first, last, int(fb.value)
+
+    def lower_bound_device(self, q_ptr: int, n: int, out_ptr: int, fallbacks_ptr: int = 0, stream: int = 0) -> None:
+        _check(load_library().rmi_delta_lower_bound(self._h, C.c_void_p(q_ptr), int(n), C.c_void_p(out_ptr),
+                                                    C.c_void_p(fallbacks_ptr or None), C.c_void_p(stream or None)))
+
+    def upper_bound_device(self, q_ptr: int, n: int, out_ptr: int, fallbacks_ptr: int = 0, stream: int = 0) -> None:
+        _check(load_library().rmi_delta_upper_bound(self._h, C.c_void_p(q_ptr), int(n), C.c_void_p(out_ptr),
+                                                    C.c_void_p(fallbacks_ptr or None), C.c_void_p(stream or None)))
+
+    def equal_range_device(self, q_ptr: int, n: int, first_ptr: int, last_ptr: int, fallbacks_ptr: int = 0,
+                           stream: int = 0) -> None:
+        _check(load_library().rmi_delta_equal_range(self._h, C.c_void_p(q_ptr), int(n), C.c_void_p(first_ptr),
+                                                    C.c_void_p(last_ptr), C.c_void_p(fallbacks_ptr or None),
+                                                    C.c_void_p(stream or None)))
+
+    def merged_keys(self) -> RMITrainingData:
+        """The n + m merged keys as a new RMITrainingData that owns them, on the index's device (its sortedness found
+        by the same check as any data set's)."""
+        out = RMITrainingData.__new__(RMITrainingData)
+        out._h = C.c_void_p()
+        out.key_type = self.key_type
+        out.device = self.index.data.device
+        out._keep = None
+        _check(load_library().rmi_delta_merge(self._h, C.byref(out._h)))
+        return out
+
+    def compact(self, mode: str = "retrain") -> "DeltaRMIIndex":
+        """A new DeltaRMIIndex with an empty delta over a fresh index on merged_keys(); this one stays valid until it is
+        closed.  mode "retrain" trains the base's spec and branching factor again (train_bounded, with the cache-fix
+        scan on the device, for a bounded base); "evaluate" keeps a plain base's tables and re-derives their error
+        bounds on the merged keys (RMIPanic where the top model is not monotone on them).  A bounded base has no
+        "evaluate": its knots belong to the old keys."""
+        if mode not in ("retrain", "evaluate"):
+            raise ValueError(f'mode must be "retrain" or "evaluate", got {mode!r}')
+        base = self.index
+        bounded = isinstance(base, BoundedRMIIndex)
+        if bounded and mode == "evaluate":
+            raise RMIError("a bounded index cannot be compacted by evaluation: its spline knots belong to the old keys")
+        merged = self.merged_keys()
+        t = base._trained
+        if bounded:
+            r, knots = train_bounded(merged, t.models, t.branching_factor, base.line_size, device=merged.device)
+            return DeltaRMIIndex(BoundedRMIIndex(r, knots, base.line_size, merged))
+        g = train(merged, t.models, t.branching_factor) if mode == "retrain" else evaluate(t, merged, counts=False)
+        return DeltaRMIIndex(RMIIndex(g, merged))
+
+    def close(self):
+        if getattr(self, "_h", None) and self._h.value:
+            load_library().rmi_delta_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

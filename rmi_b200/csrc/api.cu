@@ -791,6 +791,13 @@ int rmi_dataset_replicate(const rmi_dataset* src, int device, rmi_dataset** out)
 }
 
 uint64_t rmi_dataset_len(const rmi_dataset* ds) { return ds ? ds->n : 0; }
+int rmi_dataset_copy_to_host(const rmi_dataset* ds, void* host_keys) {
+  if (!ds || (!host_keys && ds->n)) return fail(RMI_ERR_INVALID, "rmi_dataset_copy_to_host: null argument");
+  if (ds->n == 0) return RMI_OK;
+  CUDA_TRY(cudaSetDevice(ds->device));
+  CUDA_TRY(cudaMemcpy(host_keys, ds->d_keys, (size_t)ds->n * key_bytes(ds->key_type), cudaMemcpyDeviceToHost));
+  return RMI_OK;
+}
 int rmi_dataset_key_type(const rmi_dataset* ds) { return ds ? ds->key_type : -1; }
 void rmi_dataset_destroy(rmi_dataset* ds) {
   if (!ds) return;
@@ -1034,6 +1041,182 @@ int rmi_index_lookup_host(const rmi_index* idx, const void* host_queries, uint64
                            return lower_bound ? index_launch(idx, LOOKUP_LOWER, d_q, n, d_out, nullptr, d_fb, st)
                                               : index_launch(idx, LOOKUP_PREDICT, d_q, n, d_out, d_err, nullptr, st);
                          });
+}
+
+}  // extern "C"
+
+// An updatable index (DESIGN.md section 19): a base index and the sorted keys inserted since it was built, in one of
+// two device buffers; an insert merges the delta and the batch into the other one, which then becomes the delta.
+struct rmi_delta {
+  const rmi_index* base = nullptr;
+  void* buf[2] = {nullptr, nullptr};
+  uint64_t cap[2] = {0, 0};   // keys each buffer holds room for
+  int cur = 0;                // buf[cur] holds the m delta keys
+  uint64_t m = 0;
+  unsigned* d_status = nullptr;
+};
+
+namespace {
+
+int delta_check_call(const rmi_delta* d, const void* d_queries, uint64_t n, const void* d_out, const char* fn) {
+  if (!d) return fail(RMI_ERR_INVALID, std::string(fn) + ": null delta index");
+  if (n && (!d_queries || !d_out)) return fail(RMI_ERR_INVALID, std::string(fn) + ": null query or output pointer");
+  return RMI_OK;
+}
+
+// The base index's launch of `mode`, then, on the same stream, the delta's counts added to its answers.
+int delta_launch(const rmi_delta* d, LookupMode mode, const void* d_queries, uint64_t n, uint64_t* d_first,
+                 uint64_t* d_last, uint64_t* d_fallbacks, void* cuda_stream) {
+  if (n == 0) return RMI_OK;
+  uint64_t* out = mode == LOOKUP_UPPER ? d_last : d_first;
+  if (int rc = index_launch(d->base, mode, d_queries, n, out, mode == LOOKUP_EQUAL_RANGE ? d_last : nullptr, d_fallbacks,
+                            cuda_stream))
+    return rc;
+  if (d->m == 0) return RMI_OK;
+  const DeltaCountMode cm = mode == LOOKUP_LOWER ? DELTA_LOWER : mode == LOOKUP_UPPER ? DELTA_UPPER : DELTA_BOTH;
+  Launch L{(cudaStream_t)cuda_stream, d->base->num_sms};
+  with_key_type(d->base->ds->key_type, [&](auto k) {
+    using T = decltype(k);
+    delta_count<T>(L, cm, (const T*)d->buf[d->cur], d->m, (const T*)d_queries, n, (u64*)d_first, (u64*)d_last);
+  });
+  CUDA_TRY(cudaGetLastError());
+  return RMI_OK;
+}
+
+// a (na keys) and b (nb keys) merged into out on the calling thread's stream, synchronously; *status receives the
+// merge's status word (DELTA_ST_NAN) when d_status is given.
+int delta_merge_sync(const rmi_delta* d, const void* a, uint64_t na, const void* b, uint64_t nb, void* out,
+                     unsigned* d_status, unsigned* status, const char* fn) {
+  const cudaStream_t st = cudaStreamPerThread;
+  if (d_status) CUDA_TRY(cudaMemsetAsync(d_status, 0, sizeof(unsigned), st));
+  Launch L{st, d->base->num_sms};
+  with_key_type(d->base->ds->key_type, [&](auto k) {
+    using T = decltype(k);
+    delta_merge<T>(L, (const T*)a, na, (const T*)b, nb, (T*)out, d_status);
+  });
+  cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess && d_status) e = cudaMemcpyAsync(status, d_status, sizeof(unsigned), cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return fail(RMI_ERR_CUDA, std::string(fn) + ": " + cudaGetErrorString(e));
+  return RMI_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int rmi_delta_create(const rmi_index* base, rmi_delta** out) {
+  if (!base || !out) return fail(RMI_ERR_INVALID, "rmi_delta_create: null argument");
+  CUDA_TRY(cudaSetDevice(base->ds->device));
+  auto* d = new rmi_delta();
+  d->base = base;
+  if (cudaMalloc(&d->d_status, sizeof(unsigned)) != cudaSuccess) {
+    delete d;
+    return fail(RMI_ERR_CUDA, "rmi_delta_create: device allocation failed");
+  }
+  *out = d;
+  return RMI_OK;
+}
+
+void rmi_delta_destroy(rmi_delta* d) {
+  if (!d) return;
+  cudaSetDevice(d->base->ds->device);
+  cudaFree(d->buf[0]);
+  cudaFree(d->buf[1]);
+  cudaFree(d->d_status);
+  delete d;
+}
+
+uint64_t rmi_delta_len(const rmi_delta* d) { return d ? d->m : 0; }
+
+int rmi_delta_insert(rmi_delta* d, const rmi_dataset* batch) {
+  const std::string fn = "rmi_delta_insert";
+  if (!d || !batch) return fail(RMI_ERR_INVALID, fn + ": null argument");
+  const rmi_dataset* ds = d->base->ds;
+  if (batch->key_type != ds->key_type) return fail(RMI_ERR_INVALID, fn + ": the batch's key type differs from the index's");
+  if (batch->device != ds->device) return fail(RMI_ERR_INVALID, fn + ": the batch is on another device than the index");
+  if (!batch->sorted) return fail(RMI_ERR_INVALID, fn + ": the batch is not sorted in ascending order");
+  if (batch->n == 0) return RMI_OK;
+  CUDA_TRY(cudaSetDevice(ds->device));
+  const int spare = 1 - d->cur;
+  const uint64_t need = d->m + batch->n;
+  if (d->cap[spare] < need) {   // double the capacity when the batch does not fit
+    const uint64_t cap = std::max<uint64_t>({need, 2 * std::max(d->cap[0], d->cap[1]), 1024});
+    void* p = nullptr;
+    if (cudaMalloc(&p, (size_t)cap * key_bytes(ds->key_type)) != cudaSuccess) {
+      cudaGetLastError();
+      return fail(RMI_ERR_CUDA, fn + ": device allocation of " + std::to_string(cap) + " keys failed");
+    }
+    cudaFree(d->buf[spare]);
+    d->buf[spare] = p;
+    d->cap[spare] = cap;
+  }
+  unsigned status = 0;
+  if (int rc = delta_merge_sync(d, d->buf[d->cur], d->m, batch->d_keys, batch->n, d->buf[spare], d->d_status, &status,
+                                fn.c_str()))
+    return rc;
+  if (status & DELTA_ST_NAN) return fail(RMI_ERR_INVALID, fn + ": the batch holds a NaN");
+  d->cur = spare;
+  d->m = need;
+  return RMI_OK;
+}
+
+int rmi_delta_lower_bound(const rmi_delta* d, const void* d_queries, uint64_t n, uint64_t* d_out,
+                          uint64_t* d_fallbacks, void* cuda_stream) {
+  if (int rc = delta_check_call(d, d_queries, n, d_out, "rmi_delta_lower_bound")) return rc;
+  return delta_launch(d, LOOKUP_LOWER, d_queries, n, d_out, nullptr, d_fallbacks, cuda_stream);
+}
+
+int rmi_delta_upper_bound(const rmi_delta* d, const void* d_queries, uint64_t n, uint64_t* d_out,
+                          uint64_t* d_fallbacks, void* cuda_stream) {
+  if (int rc = delta_check_call(d, d_queries, n, d_out, "rmi_delta_upper_bound")) return rc;
+  return delta_launch(d, LOOKUP_UPPER, d_queries, n, nullptr, d_out, d_fallbacks, cuda_stream);
+}
+
+int rmi_delta_equal_range(const rmi_delta* d, const void* d_queries, uint64_t n, uint64_t* d_first, uint64_t* d_last,
+                          uint64_t* d_fallbacks, void* cuda_stream) {
+  if (int rc = delta_check_call(d, d_queries, n, d_last, "rmi_delta_equal_range")) return rc;
+  if (n && !d_first) return fail(RMI_ERR_INVALID, "rmi_delta_equal_range: null query or output pointer");
+  return delta_launch(d, LOOKUP_EQUAL_RANGE, d_queries, n, d_first, d_last, d_fallbacks, cuda_stream);
+}
+
+int rmi_delta_range_host(const rmi_delta* d, const void* host_queries, uint64_t n, uint64_t* host_first,
+                         uint64_t* host_last, uint64_t* fallbacks) {
+  const char* fn = "rmi_delta_range_host";
+  if (int rc = delta_check_call(d, host_queries, n, host_first ? (const void*)host_first : host_last, fn)) return rc;
+  if (fallbacks) *fallbacks = 0;
+  if (n == 0) return RMI_OK;
+  // index_host_call fills host_a always and host_b when given: the lower bounds go first whenever they are asked for
+  uint64_t* host_a = host_first ? host_first : host_last;
+  uint64_t* host_b = host_first ? host_last : nullptr;
+  const LookupMode mode = !host_first ? LOOKUP_UPPER : host_last ? LOOKUP_EQUAL_RANGE : LOOKUP_LOWER;
+  return index_host_call(d->base, host_queries, n, host_a, host_b, fallbacks, fn,
+                         [&](const void* d_q, uint64_t* d_a, uint64_t* d_b, uint64_t* d_fb, cudaStream_t st) {
+                           return mode == LOOKUP_UPPER ? delta_launch(d, mode, d_q, n, nullptr, d_a, d_fb, st)
+                                                       : delta_launch(d, mode, d_q, n, d_a, d_b, d_fb, st);
+                         });
+}
+
+int rmi_delta_merge(const rmi_delta* d, rmi_dataset** out) {
+  const std::string fn = "rmi_delta_merge";
+  if (!d || !out) return fail(RMI_ERR_INVALID, fn + ": null argument");
+  const rmi_dataset* base = d->base->ds;
+  CUDA_TRY(cudaSetDevice(base->device));
+  const uint64_t n = base->n + d->m;
+  void* keys = nullptr;
+  // readable up to the next 16-byte boundary, as every dataset the library allocates
+  if (cudaMalloc(&keys, std::max<size_t>(16, ((size_t)n * key_bytes(base->key_type) + 15) & ~(size_t)15)) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(RMI_ERR_CUDA, fn + ": device allocation of " + std::to_string(n) + " keys failed");
+  }
+  auto* ds = new rmi_dataset();
+  ds->d_keys = keys; ds->n = n; ds->key_type = base->key_type; ds->device = base->device;
+  ds->owned = true; ds->pooled = false;
+  int rc = delta_merge_sync(d, base->d_keys, base->n, d->buf[d->cur], d->m, keys, nullptr, nullptr, fn.c_str());
+  if (rc == RMI_OK) rc = verify_sorted(ds);
+  if (rc != RMI_OK) { rmi_dataset_destroy(ds); return rc; }
+  *out = ds;
+  return RMI_OK;
 }
 
 }  // extern "C"

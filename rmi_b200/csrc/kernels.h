@@ -238,6 +238,19 @@ void lookup_bounded_batch(const Launch& L, LookupMode mode, const TopModel& top,
                           u64 N, const void* d_knots, u64 K, u64 line_size, const u64* keys, u64 n, u64 last,
                           const u64* d_queries, u64 nq, u64* d_out, u64* d_out2, u64* d_fallbacks);
 
+// ---- the sorted delta of an updatable index (kernels_delta.cu, DESIGN.md section 19) -----------------------------
+// out[0, na + nb) = the stable merge of the sorted arrays a and b (a's key first on equal keys, compared by value).
+// d_status (may be null) receives DELTA_ST_NAN if b holds a NaN.  One launch (none for na + nb == 0).
+constexpr unsigned DELTA_ST_NAN = 1u;
+template <class T> void delta_merge(const Launch& L, const T* a, u64 na, const T* b, u64 nb, T* out, unsigned* d_status);
+// Adds, per query, the number of the m sorted delta keys d with d < q (DELTA_LOWER, into out_first), d <= q
+// (DELTA_UPPER, into out_last) or both (DELTA_BOTH) to the answers already there.  One launch (none for m == 0 or
+// nq == 0).
+enum DeltaCountMode { DELTA_LOWER, DELTA_UPPER, DELTA_BOTH };
+template <class T>
+void delta_count(const Launch& L, DeltaCountMode mode, const T* delta, u64 m, const T* d_queries, u64 nq,
+                 u64* out_first, u64* out_last);
+
 // ---- lookups over a range-partitioned data set (kernels_shard_lookup.cu, DESIGN.md section 14) -------------------
 // A query goes to the last non-empty rank whose first key is < q (the first non-empty rank if none is).
 constexpr int SHARD_ROUTE_MAX = 64;
