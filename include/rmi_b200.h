@@ -249,19 +249,21 @@ int rmi_index_equal_range(const rmi_index* idx, const void* d_queries, uint64_t 
 int rmi_index_range_host(const rmi_index* idx, const void* host_queries, uint64_t n, uint64_t* host_first,
                          uint64_t* host_last, uint64_t* fallbacks);
 
-/* ---- Updatable indexes: lookups over inserted keys (DESIGN.md section 19) -------------------------------------------
- * An rmi_delta wraps an rmi_index, plain or bounded, and a device-resident sorted array of the keys inserted since that
- * index was built (the delta, m keys).  Its logical key set is the multiset base keys ∪ inserted keys, and every
- * answer is exact over it:
- *   lower_bound(q) = the base index's lower_bound(q) + #{d in delta : d < q}; upper_bound likewise with d <= q;
- *   equal_range(q) = both.  A NaN query gives [0, 0), as on the base index.  The fallback counts are the base index's:
- *   the delta's part is an exact search and adds none.
+/* ---- Updatable indexes: lookups over inserted and removed keys (DESIGN.md section 19) -----------------------------
+ * An rmi_delta wraps an rmi_index, plain or bounded, and two device-resident sorted arrays: the keys inserted since
+ * that index was built (m keys) and the keys removed since (t keys).  Its logical key set is the multiset
+ * base keys ⊎ inserted keys ⊖ removed keys, and every answer is exact over it:
+ *   lower_bound(q) = the base index's lower_bound(q) + #{inserted keys < q} - #{removed keys < q}; upper_bound likewise
+ *   with <=; equal_range(q) = both.  A NaN query gives [0, 0), as on the base index.  The fallback counts are the base
+ *   index's: the delta's part is an exact search and adds none.  The subtraction never drops below 0: every accepted
+ *   removal keeps the removed keys a sub-multiset of the base and inserted keys.
  * There is no predict: the model's positions refer to the base keys only.
  * Equal keys keep one order everywhere: base keys before equal inserted keys, earlier inserts before later ones, keys
- * compared by value (-0.0 == 0.0).  So rmi_delta_merge's keys are the stable sort of the base keys followed by every
- * batch in insert order.
- * Concurrency: lookups on one rmi_delta may run concurrently on several streams.  rmi_delta_insert and
- * rmi_delta_destroy must not overlap any other call on the same handle, lookups still in flight on other streams
+ * compared by value (-0.0 == 0.0).  A removal of value v takes away the first copy of v's run in that order.  So
+ * rmi_delta_merge's keys are the stable sort of the base keys followed by every inserted batch, with the first c(v)
+ * copies of every value v dropped, c(v) being how often v was removed.
+ * Concurrency: lookups on one rmi_delta may run concurrently on several streams.  rmi_delta_insert, rmi_delta_remove
+ * and rmi_delta_destroy must not overlap any other call on the same handle, lookups still in flight on other streams
  * included.  The base index is unchanged and immutable; base (and its dataset) must outlive the rmi_delta. */
 typedef struct rmi_delta rmi_delta;
 int rmi_delta_create(const rmi_index* base, rmi_delta** out);
@@ -276,9 +278,19 @@ void rmi_delta_destroy(rmi_delta* d);
 int rmi_delta_insert(rmi_delta* d, const rmi_dataset* batch);
 /* Keys inserted so far (m). */
 uint64_t rmi_delta_len(const rmi_delta* d);
+/* Removes a batch of keys, synchronously, on the calling thread's stream (cudaStreamPerThread): each key of the batch
+ * removes one copy of its value from the logical key set.  The batch must be a sorted data set of the base's key type
+ * on the base's device, hold no NaN, and hold no value more often than the logical key set does at the time of the
+ * call (values compared by value, so -0.0 == 0.0): a key that is not there, one copy too many, or a copy already
+ * removed is refused.  Refused with RMI_ERR_INVALID: a null argument, another key type or device, an unsorted batch,
+ * a NaN ("holds a NaN") and too many copies ("does not hold").  A refused batch changes nothing.  The removed keys
+ * are stored as the inserted keys are, in two buffers that trade places. */
+int rmi_delta_remove(rmi_delta* d, const rmi_dataset* batch);
+/* Keys removed so far (t). */
+uint64_t rmi_delta_removed_len(const rmi_delta* d);
 /* As rmi_index_lower_bound / _upper_bound / _equal_range over the logical key set: the base index's launch, then, on
- * the same stream, one launch that adds the delta's counts to the outputs (none when m == 0, so the answers and the
- * launch count are then the base index's; none at all for n == 0). */
+ * the same stream, one launch that adds the delta's counts to the outputs (none when m == 0 and t == 0, so the
+ * answers and the launch count are then the base index's; none at all for n == 0). */
 int rmi_delta_lower_bound(const rmi_delta* d, const void* d_queries, uint64_t n, uint64_t* d_out,
                           uint64_t* d_fallbacks, void* cuda_stream);
 int rmi_delta_upper_bound(const rmi_delta* d, const void* d_queries, uint64_t n, uint64_t* d_out,
@@ -289,7 +301,8 @@ int rmi_delta_equal_range(const rmi_delta* d, const void* d_queries, uint64_t n,
  * NULL, not both.  *fallbacks (may be NULL) is SET to the fallback count. */
 int rmi_delta_range_host(const rmi_delta* d, const void* host_queries, uint64_t n, uint64_t* host_first,
                          uint64_t* host_last, uint64_t* fallbacks);
-/* A new, owned data set of the n + m merged keys on the base's device (the base keys alone for an empty delta), with
+/* A new, owned data set of the n + m - t logical keys on the base's device (the base keys alone for an empty delta;
+ * possibly no key at all when every key was removed), in the order given above, with
  * its sorted and no_dups flags found by the same check as rmi_dataset_create's.  Release it with
  * rmi_dataset_destroy.  Compaction trains or evaluates an index over it (rmi_train, rmi_evaluate,
  * rmi_cache_fix_device) and wraps that index in a new rmi_delta. */

@@ -15,7 +15,7 @@ plus RMIIndex and BoundedRMIIndex (a train_bounded build), batched lookups (posi
 bounds) on the GPU.  cache_fix / train_bounded on an RMITrainingData fit the cache-fix spline on the GPU.
 rmi_b200.sharded (torch.distributed) trains over range-partitioned keys (train_sharded), evaluates a given RMI over
 them (evaluate_sharded) and serves lookups over them (ShardedRMIIndex).  DeltaRMIIndex serves exact lookups over keys
-inserted after an index was built, and compacts them into a fresh index.
+inserted into and removed from an index after it was built, and compacts them into a fresh index.
 
 and does no arithmetic of its own.  There is no CPU fallback: if the CUDA library is missing
 or no device is present, calls raise.

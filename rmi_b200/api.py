@@ -122,6 +122,9 @@ def load_library():
         L.rmi_delta_insert.argtypes = [C.c_void_p, C.c_void_p]
         L.rmi_delta_len.restype = C.c_uint64
         L.rmi_delta_len.argtypes = [C.c_void_p]
+        L.rmi_delta_remove.argtypes = [C.c_void_p, C.c_void_p]
+        L.rmi_delta_removed_len.restype = C.c_uint64
+        L.rmi_delta_removed_len.argtypes = [C.c_void_p]
         L.rmi_delta_lower_bound.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]
         L.rmi_delta_upper_bound.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]
         L.rmi_delta_equal_range.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p,
@@ -635,15 +638,18 @@ class BoundedRMIIndex(RMIIndex):
 
 
 class DeltaRMIIndex:
-    """An updatable index (DESIGN §19): an ``RMIIndex`` or ``BoundedRMIIndex`` (kept alive here) and a sorted delta of
-    the keys inserted since it was built, on the index's device.  The logical key set is the multiset of the base keys
-    and every inserted key, and ``lower_bound``, ``upper_bound`` and ``equal_range`` are exact over it: the base index's
-    answer plus the number of delta keys below (or, for the upper bound, not above) the query.  Equal keys keep base
-    keys first, then inserted keys in insert order, so ``merged_keys()`` is the stable sort of the base keys followed
-    by every batch.  There is no ``predict``: the model's positions refer to the base keys only.
+    """An updatable index (DESIGN §19): an ``RMIIndex`` or ``BoundedRMIIndex`` (kept alive here) and two sorted arrays
+    on the index's device, the keys inserted since it was built and the keys removed since.  The logical key set is the
+    multiset base ⊎ inserted ⊖ removed, and ``lower_bound``, ``upper_bound`` and ``equal_range`` are exact over it: the
+    base index's answer plus the number of inserted keys below (or, for the upper bound, not above) the query, minus the
+    number of removed keys below (not above) it.  Equal keys keep base keys first, then inserted keys in insert order,
+    and a removal of a value takes away the first copy of its run, so ``merged_keys()`` is the stable sort of the base
+    keys followed by every inserted batch, without the first c copies of each value removed c times.  There is no
+    ``predict``: the model's positions refer to the base keys only.
 
-    ``insert`` must not run while another call on the same object, or a lookup it enqueued, is still in flight; lookups
-    may run concurrently on several streams.  ``len(d)`` is n + m, ``num_inserted`` is m."""
+    ``insert`` and ``remove`` must not run while another call on the same object, or a lookup it enqueued, is still in
+    flight; lookups may run concurrently on several streams.  ``len(d)`` is n + m - t, ``num_inserted`` is m and
+    ``num_removed`` is t."""
 
     def __init__(self, index: RMIIndex):
         self._h = C.c_void_p()
@@ -655,16 +661,30 @@ class DeltaRMIIndex:
     def num_inserted(self) -> int:
         return int(load_library().rmi_delta_len(self._h))
 
+    @property
+    def num_removed(self) -> int:
+        return int(load_library().rmi_delta_removed_len(self._h))
+
     def __len__(self) -> int:
-        return len(self.index.data) + self.num_inserted
+        return len(self.index.data) + self.num_inserted - self.num_removed
 
     def insert(self, keys) -> None:
         """Merges a batch into the delta and returns when it is there.  ``keys``: a numpy array of the index's key type
         (sorted here with a stable sort, then copied to the device), or an RMITrainingData on the index's device (for
         device-resident batches, RMITrainingData.from_device), which must already be sorted.  A batch that is refused
         (unsorted, another key type or device, a NaN) leaves the delta unchanged."""
+        self._apply(load_library().rmi_delta_insert, keys)
+
+    def remove(self, keys) -> None:
+        """Removes one copy of each key's value from the logical key set and returns when that is done.  ``keys`` as
+        for ``insert``.  Refused with RMIError, changing nothing: a batch that is unsorted, of another key type or
+        device, holds a NaN, or holds a value more often than the logical key set does (a key that is not there, one
+        copy too many, a copy already removed)."""
+        self._apply(load_library().rmi_delta_remove, keys)
+
+    def _apply(self, call, keys):
         if isinstance(keys, RMITrainingData):
-            _check(load_library().rmi_delta_insert(self._h, keys._h))
+            _check(call(self._h, keys._h))
             return
         if not isinstance(keys, np.ndarray) or keys.dtype != np.dtype(_NP_OF_KEY[self.key_type]):
             got = keys.dtype if isinstance(keys, np.ndarray) else type(keys).__name__
@@ -672,7 +692,7 @@ class DeltaRMIIndex:
         batch = RMITrainingData(np.sort(keys.ravel(), kind="stable"),
                                 device=self.index.data.device)
         try:
-            _check(load_library().rmi_delta_insert(self._h, batch._h))
+            _check(call(self._h, batch._h))
         finally:
             batch.close()
 
@@ -717,8 +737,9 @@ class DeltaRMIIndex:
                                                     C.c_void_p(stream or None)))
 
     def merged_keys(self) -> RMITrainingData:
-        """The n + m merged keys as a new RMITrainingData that owns them, on the index's device (its sortedness found
-        by the same check as any data set's)."""
+        """The n + m - t logical keys, in the order the class describes, as a new RMITrainingData that owns them, on
+        the index's device (its sortedness found by the same check as any data set's).  Empty when every key was
+        removed."""
         out = RMITrainingData.__new__(RMITrainingData)
         out._h = C.c_void_p()
         out.key_type = self.key_type

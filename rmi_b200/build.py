@@ -16,7 +16,7 @@ SOURCES = ["kernels_top.cu", "kernels_leaf.cu", "kernels_shard.cu", "kernels_loo
            "kernels_cachefix.cu", "kernels_eval.cu", "kernels_shard_lookup.cu", "kernels_shard_eval.cu",
            "kernels_shard_cachefix.cu", "kernels_shard_bounded.cu", "kernels_delta.cu", "api.cu"]
 HEADERS = ["rust_math.cuh", "models.cuh", "device_util.cuh", "spline.cuh", "lookup_search.cuh", "leaf_resid.cuh",
-           "merge_path.cuh", "kernels.h", "nccl_dl.h",
+           "merge_path.cuh", "multiset_diff.cuh", "kernels.h", "nccl_dl.h",
            os.path.join("..", "..", "include", "rmi_b200.h"), os.path.join("..", "..", "host", "cache_fix.hpp"), os.path.join("..", "..", "host", "codegen.hpp"),
            os.path.join("..", "..", "host", "optimizer.hpp"), os.path.join("..", "..", "host", "artefact_load.hpp"),
            os.path.join("..", "..", "host", "slab_layout.hpp")]

@@ -1045,14 +1045,41 @@ int rmi_index_lookup_host(const rmi_index* idx, const void* host_queries, uint64
 
 }  // extern "C"
 
-// An updatable index (DESIGN.md section 19): a base index and the sorted keys inserted since it was built, in one of
-// two device buffers; an insert merges the delta and the batch into the other one, which then becomes the delta.
-struct rmi_delta {
-  const rmi_index* base = nullptr;
+// A sorted device array of keys in one of two buffers: an update merges the array and a batch into the other one,
+// which then holds the array.
+struct DeltaKeys {
   void* buf[2] = {nullptr, nullptr};
   uint64_t cap[2] = {0, 0};   // keys each buffer holds room for
-  int cur = 0;                // buf[cur] holds the m delta keys
-  uint64_t m = 0;
+  int cur = 0;                // buf[cur] holds the len keys
+  uint64_t len = 0;
+  const void* keys() const { return buf[cur]; }
+  void* spare() const { return buf[1 - cur]; }
+  // Makes the spare buffer hold `need` keys: one of twice the larger capacity (at least `need`, at least 1024 keys)
+  // when it is too small.
+  int reserve_spare(uint64_t need, size_t key_bytes, const std::string& fn) {
+    const int s = 1 - cur;
+    if (cap[s] >= need) return RMI_OK;
+    const uint64_t c = std::max<uint64_t>({need, 2 * std::max(cap[0], cap[1]), 1024});
+    void* p = nullptr;
+    if (cudaMalloc(&p, (size_t)c * key_bytes) != cudaSuccess) {
+      cudaGetLastError();
+      return fail(RMI_ERR_CUDA, fn + ": device allocation of " + std::to_string(c) + " keys failed");
+    }
+    cudaFree(buf[s]);
+    buf[s] = p;
+    cap[s] = c;
+    return RMI_OK;
+  }
+  // The spare buffer, holding n keys, becomes the array.
+  void swap_in(uint64_t n) { cur = 1 - cur; len = n; }
+  void release() { cudaFree(buf[0]); cudaFree(buf[1]); }
+};
+
+// An updatable index (DESIGN.md section 19): a base index, the sorted keys inserted since it was built (m) and the
+// sorted keys removed since (t).  The logical key set is base ⊎ inserted ⊖ removed.
+struct rmi_delta {
+  const rmi_index* base = nullptr;
+  DeltaKeys ins, rem;
   unsigned* d_status = nullptr;
 };
 
@@ -1064,7 +1091,8 @@ int delta_check_call(const rmi_delta* d, const void* d_queries, uint64_t n, cons
   return RMI_OK;
 }
 
-// The base index's launch of `mode`, then, on the same stream, the delta's counts added to its answers.
+// The base index's launch of `mode`, then, on the same stream, the delta's share added to its answers: k_delta_count
+// over the inserted keys while nothing has been removed (no launch for an empty delta), k_delta_adjust otherwise.
 int delta_launch(const rmi_delta* d, LookupMode mode, const void* d_queries, uint64_t n, uint64_t* d_first,
                  uint64_t* d_last, uint64_t* d_fallbacks, void* cuda_stream) {
   if (n == 0) return RMI_OK;
@@ -1072,12 +1100,16 @@ int delta_launch(const rmi_delta* d, LookupMode mode, const void* d_queries, uin
   if (int rc = index_launch(d->base, mode, d_queries, n, out, mode == LOOKUP_EQUAL_RANGE ? d_last : nullptr, d_fallbacks,
                             cuda_stream))
     return rc;
-  if (d->m == 0) return RMI_OK;
+  if (d->ins.len == 0 && d->rem.len == 0) return RMI_OK;
   const DeltaCountMode cm = mode == LOOKUP_LOWER ? DELTA_LOWER : mode == LOOKUP_UPPER ? DELTA_UPPER : DELTA_BOTH;
   Launch L{(cudaStream_t)cuda_stream, d->base->num_sms};
   with_key_type(d->base->ds->key_type, [&](auto k) {
     using T = decltype(k);
-    delta_count<T>(L, cm, (const T*)d->buf[d->cur], d->m, (const T*)d_queries, n, (u64*)d_first, (u64*)d_last);
+    if (d->rem.len == 0)
+      delta_count<T>(L, cm, (const T*)d->ins.keys(), d->ins.len, (const T*)d_queries, n, (u64*)d_first, (u64*)d_last);
+    else
+      delta_adjust<T>(L, cm, (const T*)d->ins.keys(), d->ins.len, (const T*)d->rem.keys(), d->rem.len,
+                      (const T*)d_queries, n, (u64*)d_first, (u64*)d_last);
   });
   CUDA_TRY(cudaGetLastError());
   return RMI_OK;
@@ -1121,13 +1153,15 @@ int rmi_delta_create(const rmi_index* base, rmi_delta** out) {
 void rmi_delta_destroy(rmi_delta* d) {
   if (!d) return;
   cudaSetDevice(d->base->ds->device);
-  cudaFree(d->buf[0]);
-  cudaFree(d->buf[1]);
+  d->ins.release();
+  d->rem.release();
   cudaFree(d->d_status);
   delete d;
 }
 
-uint64_t rmi_delta_len(const rmi_delta* d) { return d ? d->m : 0; }
+uint64_t rmi_delta_len(const rmi_delta* d) { return d ? d->ins.len : 0; }
+
+uint64_t rmi_delta_removed_len(const rmi_delta* d) { return d ? d->rem.len : 0; }
 
 int rmi_delta_insert(rmi_delta* d, const rmi_dataset* batch) {
   const std::string fn = "rmi_delta_insert";
@@ -1138,26 +1172,59 @@ int rmi_delta_insert(rmi_delta* d, const rmi_dataset* batch) {
   if (!batch->sorted) return fail(RMI_ERR_INVALID, fn + ": the batch is not sorted in ascending order");
   if (batch->n == 0) return RMI_OK;
   CUDA_TRY(cudaSetDevice(ds->device));
-  const int spare = 1 - d->cur;
-  const uint64_t need = d->m + batch->n;
-  if (d->cap[spare] < need) {   // double the capacity when the batch does not fit
-    const uint64_t cap = std::max<uint64_t>({need, 2 * std::max(d->cap[0], d->cap[1]), 1024});
-    void* p = nullptr;
-    if (cudaMalloc(&p, (size_t)cap * key_bytes(ds->key_type)) != cudaSuccess) {
-      cudaGetLastError();
-      return fail(RMI_ERR_CUDA, fn + ": device allocation of " + std::to_string(cap) + " keys failed");
-    }
-    cudaFree(d->buf[spare]);
-    d->buf[spare] = p;
-    d->cap[spare] = cap;
-  }
+  const uint64_t need = d->ins.len + batch->n;
+  if (int rc = d->ins.reserve_spare(need, key_bytes(ds->key_type), fn)) return rc;
   unsigned status = 0;
-  if (int rc = delta_merge_sync(d, d->buf[d->cur], d->m, batch->d_keys, batch->n, d->buf[spare], d->d_status, &status,
-                                fn.c_str()))
+  if (int rc = delta_merge_sync(d, d->ins.keys(), d->ins.len, batch->d_keys, batch->n, d->ins.spare(), d->d_status,
+                                &status, fn.c_str()))
     return rc;
   if (status & DELTA_ST_NAN) return fail(RMI_ERR_INVALID, fn + ": the batch holds a NaN");
-  d->cur = spare;
-  d->m = need;
+  d->ins.swap_in(need);
+  return RMI_OK;
+}
+
+int rmi_delta_remove(rmi_delta* d, const rmi_dataset* batch) {
+  const std::string fn = "rmi_delta_remove";
+  if (!d || !batch) return fail(RMI_ERR_INVALID, fn + ": null argument");
+  const rmi_dataset* ds = d->base->ds;
+  if (batch->key_type != ds->key_type) return fail(RMI_ERR_INVALID, fn + ": the batch's key type differs from the index's");
+  if (batch->device != ds->device) return fail(RMI_ERR_INVALID, fn + ": the batch is on another device than the index");
+  if (!batch->sorted) return fail(RMI_ERR_INVALID, fn + ": the batch is not sorted in ascending order");
+  const uint64_t n = batch->n;
+  if (n == 0) return RMI_OK;
+  CUDA_TRY(cudaSetDevice(ds->device));
+  // c(v) for every batch key: its equal range over the logical key set, from the lookup path itself
+  const cudaStream_t st = cudaStreamPerThread;
+  uint64_t* d_range = nullptr;   // first | last
+  CUDA_TRY(cudaMallocAsync((void**)&d_range, (size_t)2 * n * sizeof(u64), st));
+  int rc = delta_launch(d, LOOKUP_EQUAL_RANGE, batch->d_keys, n, d_range, d_range + n, nullptr, st);
+  unsigned status = 0;
+  cudaError_t e = cudaMemsetAsync(d->d_status, 0, sizeof(unsigned), st);
+  if (rc == RMI_OK && e == cudaSuccess) {
+    Launch L{st, d->base->num_sms};
+    with_key_type(ds->key_type, [&](auto k) {
+      using T = decltype(k);
+      delta_check_remove<T>(L, (const T*)batch->d_keys, n, (const u64*)d_range, (const u64*)d_range + n, d->d_status);
+    });
+    e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&status, d->d_status, sizeof(unsigned), cudaMemcpyDeviceToHost, st);
+    const cudaError_t ef = cudaFreeAsync(d_range, st);
+    if (e == cudaSuccess) e = ef;
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  } else {
+    cudaFreeAsync(d_range, st);
+  }
+  if (rc != RMI_OK) return rc;
+  if (e != cudaSuccess) return fail(RMI_ERR_CUDA, fn + ": " + cudaGetErrorString(e));
+  if (status & DELTA_ST_NAN) return fail(RMI_ERR_INVALID, fn + ": the batch holds a NaN");
+  if (status & DELTA_ST_MISSING)
+    return fail(RMI_ERR_INVALID, fn + ": the index does not hold every key of the batch (as many copies of each value)");
+  const uint64_t need = d->rem.len + n;
+  if ((rc = d->rem.reserve_spare(need, key_bytes(ds->key_type), fn))) return rc;
+  if ((rc = delta_merge_sync(d, d->rem.keys(), d->rem.len, batch->d_keys, n, d->rem.spare(), nullptr, nullptr,
+                             fn.c_str())))
+    return rc;
+  d->rem.swap_in(need);
   return RMI_OK;
 }
 
@@ -1202,7 +1269,8 @@ int rmi_delta_merge(const rmi_delta* d, rmi_dataset** out) {
   if (!d || !out) return fail(RMI_ERR_INVALID, fn + ": null argument");
   const rmi_dataset* base = d->base->ds;
   CUDA_TRY(cudaSetDevice(base->device));
-  const uint64_t n = base->n + d->m;
+  const uint64_t m = d->ins.len, t = d->rem.len;
+  const uint64_t n = base->n + m - t;   // t <= base->n + m: every removal was checked against the key set
   void* keys = nullptr;
   // readable up to the next 16-byte boundary, as every dataset the library allocates
   if (cudaMalloc(&keys, std::max<size_t>(16, ((size_t)n * key_bytes(base->key_type) + 15) & ~(size_t)15)) != cudaSuccess) {
@@ -1212,7 +1280,32 @@ int rmi_delta_merge(const rmi_delta* d, rmi_dataset** out) {
   auto* ds = new rmi_dataset();
   ds->d_keys = keys; ds->n = n; ds->key_type = base->key_type; ds->device = base->device;
   ds->owned = true; ds->pooled = false;
-  int rc = delta_merge_sync(d, base->d_keys, base->n, d->buf[d->cur], d->m, keys, nullptr, nullptr, fn.c_str());
+  int rc = RMI_OK;
+  if (t == 0) {
+    rc = delta_merge_sync(d, base->d_keys, base->n, d->ins.keys(), m, keys, nullptr, nullptr, fn.c_str());
+  } else {
+    // base and inserted keys merged into scratch, then the removed keys subtracted into the data set
+    const cudaStream_t st = cudaStreamPerThread;
+    void* merged = nullptr;
+    cudaError_t e = cudaMallocAsync(&merged, std::max<size_t>(16, (size_t)(base->n + m) * key_bytes(base->key_type)), st);
+    if (e == cudaSuccess) {
+      rc = delta_merge_sync(d, base->d_keys, base->n, d->ins.keys(), m, merged, nullptr, nullptr, fn.c_str());
+      if (rc == RMI_OK) {
+        Launch L{st, d->base->num_sms};
+        with_key_type(base->key_type, [&](auto k) {
+          using T = decltype(k);
+          delta_subtract<T>(L, (const T*)merged, base->n + m, (const T*)d->rem.keys(), t, (T*)keys);
+        });
+        e = cudaGetLastError();
+      }
+      const cudaError_t ef = cudaFreeAsync(merged, st);
+      if (e == cudaSuccess) e = ef;
+      if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    } else {
+      cudaGetLastError();
+    }
+    if (rc == RMI_OK && e != cudaSuccess) rc = fail(RMI_ERR_CUDA, fn + ": " + cudaGetErrorString(e));
+  }
   if (rc == RMI_OK) rc = verify_sorted(ds);
   if (rc != RMI_OK) { rmi_dataset_destroy(ds); return rc; }
   *out = ds;

@@ -250,6 +250,20 @@ enum DeltaCountMode { DELTA_LOWER, DELTA_UPPER, DELTA_BOTH };
 template <class T>
 void delta_count(const Launch& L, DeltaCountMode mode, const T* delta, u64 m, const T* d_queries, u64 nq,
                  u64* out_first, u64* out_last);
+// As delta_count for a delta with t > 0 removed keys: adds #{inserted keys before q} (m may be 0) and subtracts
+// #{removed keys before q}, "before" as mode says.  One launch (none for t == 0 or nq == 0).
+template <class T>
+void delta_adjust(const Launch& L, DeltaCountMode mode, const T* ins, u64 m, const T* rem, u64 t, const T* d_queries,
+                  u64 nq, u64* out_first, u64* out_last);
+// For a sorted batch of removals, with [first[j], last[j]) the equal range of batch[j] over the logical key set:
+// d_status receives DELTA_ST_NAN if the batch holds a NaN and DELTA_ST_MISSING if it holds more copies of a value than
+// the key set does (multiset_diff.cuh).  One launch (none for n == 0).
+constexpr unsigned DELTA_ST_MISSING = 2u;
+template <class T>
+void delta_check_remove(const Launch& L, const T* batch, u64 n, const u64* first, const u64* last, unsigned* d_status);
+// out[0, nm - t) = the sorted keys M[0, nm) minus the t sorted removed keys, each removal taking the first copy of its
+// value's run still there; requires rem ⊆ M as a multiset.  One launch (none for nm == 0).
+template <class T> void delta_subtract(const Launch& L, const T* M, u64 nm, const T* rem, u64 t, T* out);
 
 // ---- lookups over a range-partitioned data set (kernels_shard_lookup.cu, DESIGN.md section 14) -------------------
 // A query goes to the last non-empty rank whose first key is < q (the first non-empty rank if none is).
